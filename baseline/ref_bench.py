@@ -1,9 +1,9 @@
-"""Reference arm of ``bench.py``: the UNMODIFIED reference (``baseline/_ref/d9d``) on the headline workload.
+"""Reference arm of ``bench.py``: the UNMODIFIED reference (``oracle/_ref/d9d``, made by ``build()``) on the headline workload.
 
 Everything on the measured path is the reference's own stock code: ``d9d.loop.run.TrainingConfigurator`` /
 ``Trainer.train()``, its ``Qwen3MoEForCausalLM``, its Triton kernels (RMSNorm, SiLU*mul, MoE permute, stochastic
 AdamW), ``GradientSynchronizer`` and ``StochasticAdamW``, driven through the reference example's own
-``ProjectModelProvider`` and ``SFTTask`` (``baseline/_ref/example/qwen3_moe/pretrain.py``).  The dataset provider is
+``ProjectModelProvider`` and ``SFTTask`` (``oracle/_ref/example/qwen3_moe/pretrain.py``).  The dataset provider is
 synthetic (no network for datasets / tokenizers), batches leave a pinned-memory ``StatefulDataLoader`` exactly as in the
 example.  Third-party wheels the reference imports but which cannot be installed offline are replaced by stand-in
 *packages* that live in ``baseline/shims`` and are only importable from this process:
@@ -30,7 +30,7 @@ import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-REF = os.path.join(HERE, "_ref")
+REF = os.path.join(REPO, "oracle", "_ref")
 
 
 def _isolate_sys_path() -> None:
@@ -270,7 +270,7 @@ def run(args, flagship: dict, clock_sampler_cls) -> dict:
             "global_batch": global_batch, "microbatch": args.microbatch, "seq_len": args.seq_len,
             "parallelism": f"dp{world} (reference GradientSynchronizer, NCCL all-reduce)" if world > 1 else "single",
             "optimizer": "stochastic_adamw bf16 states, fp32 grads, clip 5.0",
-            "l2": "working set (>10 GB) exceeds the 126 MB L2; 192 MB flush before timing",
+            "l2": "working set (>10 GB) exceeds the 50 MB L2; 256 MB flush before timing",
         },
         "clocks": clocks,
         # the reference has one code path: Trainer.train() - the device-timed number IS the end-to-end number

@@ -1,4 +1,4 @@
-"""Headline benchmark: Qwen3-MoE pre-training throughput (tokens/s) on N B200s of one node.
+"""Headline benchmark: Qwen3-MoE pre-training throughput (tokens/s) on N H100s of one node.
 
 Model/config = the reference's only end-to-end workload (``example/qwen3_moe/pretrain.json``): 16 layers,
 hidden 768, 16 q / 4 kv heads x 128, 128 experts top-8 (expert FFN 576), vocab 151 669 (split regular/special),
@@ -7,7 +7,8 @@ Synthetic token data, random-init weights.  Weak scaling: every GPU processes ``
 ``8 x seq_len`` tokens per optimizer step (data-parallel replicas, summed gradients).
 
     python bench.py --gpus N --steps K --warmup W            # own implementation
-    python bench.py --impl reference ...                     # unmodified reference from baseline/_ref (baseline/ref_bench.py)
+    python bench.py --impl reference ...                     # unmodified reference from oracle/_ref (baseline/ref_bench.py)
+    python bench.py --dump-outputs DIR ...                   # also write what the last timed step computed as DIR/*.npy
 
 Prints ONE JSON line (rank 0).  Timed region = K optimizer steps bracketed by barrier + cuda synchronize, device
 events, max over ranks.  ``e2e`` repeats the measurement through the public training API with every step's inputs
@@ -42,10 +43,17 @@ FLAGSHIP = {
 }
 
 
+def positive_int(text: str) -> int:
+    value = int(text)
+    if value < 1:
+        raise argparse.ArgumentTypeError(f"must be >= 1, got {value}")
+    return value
+
+
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=positive_int, default=5, help="timed optimizer steps")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="own", choices=["own", "reference"])
     ap.add_argument("--seq-len", type=int, default=2048)
@@ -67,6 +75,9 @@ def parse_args():
     ap.add_argument("--checkpointing", action="store_true", help="per-layer activation checkpointing (needed by the 30b-a3b shape)")
     ap.add_argument("--ep-capacity-factor", type=float, default=2.0,
                     help="receive capacity of an expert-parallel rank as a multiple of its fair share (0 = worst case)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the loss of the last step and a fixed sample of the updated parameters "
+                         "as DIR/<name>.npy (float32), so that two builds can be compared output for output (--layout dp)")
     return ap.parse_args()
 
 
@@ -117,7 +128,7 @@ class ClockSampler:
 
 
 def reference_arm(args) -> None:
-    """Runs the UNMODIFIED reference (``baseline/_ref``, see ``baseline/ref_bench.py``) on the same workload."""
+    """Runs the UNMODIFIED reference (``oracle/_ref``, made by ``build()``; see ``baseline/ref_bench.py``) on the same workload."""
     import importlib.util
 
     here = os.path.dirname(os.path.abspath(__file__))
@@ -133,9 +144,8 @@ def reference_arm(args) -> None:
         spec.loader.exec_module(mod)
         return mod
 
-    if not os.path.isdir(os.path.join(here, "baseline", "_ref", "d9d")):
-        if not (int(os.environ.get("LOCAL_RANK", "0")) == 0 and load("install_reference").install()):
-            return unavailable("baseline/_ref is missing and /root/reference is not present on this machine to install it from")
+    if not os.path.isdir(os.path.join(here, "oracle", "_ref", "d9d")):
+        return unavailable("oracle/_ref is missing: build() makes it where the reference source is present")
     try:
         result = load("ref_bench").run(args, FLAGSHIP, ClockSampler)
     except Exception as exc:  # noqa: BLE001 - the contract is: print the reason, exit 0
@@ -207,7 +217,7 @@ def expert_parallel_arm(args) -> None:
                                        f"stages, NVLink EP dispatch/combine (capacity factor {args.ep_capacity_factor})"),
                        "optimizer": "stochastic_adamw bf16 states, fp32 grads, clip 5.0",
                        "activation_checkpointing": bool(args.checkpointing),
-                       "l2": "working set exceeds the 126 MB L2"},
+                       "l2": "working set exceeds the 50 MB L2"},
             "clocks": clocks,
             "e2e": {"value": value, "unit": "tokens/s", "h2d_bytes_per_step": res["h2d_bytes_per_step"],
                     "d2h_bytes_per_step": res["d2h_bytes_per_step"], "ms_per_step": res["ms_per_step"], "final_loss": res["final_loss"],
@@ -250,8 +260,33 @@ def build_model(args, device):
     return model
 
 
+# parameters sampled by --dump-outputs: at most this many elements of each, at fixed seeded positions
+DUMP_SAMPLES_PER_PARAM = 16384
+
+
+def dump_outputs(out_dir: str, loss, model) -> None:
+    """The loss of the last timed step and a sample of every parameter after its optimizer update (what a caller of the
+    training step receives), as float32 ``.npy`` files.  The sample positions depend only on the parameter's size."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().cpu().numpy().reshape(-1))
+    samples = []
+    for _name, param in sorted(model.named_parameters(), key=lambda kv: kv[0]):
+        flat = param.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLES_PER_PARAM:
+            gen = torch.Generator().manual_seed(flat.numel())
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLES_PER_PARAM,), generator=gen).to(flat.device)
+            flat = flat[idx]
+        samples.append(flat.float().cpu())
+    np.save(os.path.join(out_dir, "params_sample.npy"), torch.cat(samples).numpy())
+
+
 def main():
     args = parse_args()
+    if args.dump_outputs and (args.impl != "own" or args.layout != "dp"):
+        raise SystemExit("--dump-outputs is implemented for the device-timed arm (--impl own --layout dp)")
     if args.model == "30b-a3b" and args.layers == FLAGSHIP["num_hidden_layers"]:
         args.layers = QWEN3_30B_A3B["num_hidden_layers"]
     if args.impl == "reference":
@@ -279,7 +314,7 @@ def main():
     runner = TrainStepRunner(args, device, world, build_model)
     vocab = sum(model_spec(args)["split_vocab_size"].values())
     tokens_per_step_per_gpu = args.accum * args.microbatch * args.seq_len
-    flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=device)
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=device)
 
     def barrier():
         if world > 1:
@@ -303,7 +338,7 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    flush.zero_()  # inputs/weights (6 GB) are far larger than the 126 MB L2; flush once before timing anyway
+    flush.zero_()  # inputs/weights (6 GB) are far larger than the 50 MB L2; flush once before timing anyway
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     start.record()
@@ -317,6 +352,8 @@ def main():
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_per_step = ms.item() / args.steps
     _gc.enable()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, runner.model)
     launches = runner.launch_count() - launches_before
     value = tokens_per_step_per_gpu * world / (ms_per_step / 1e3)
 
@@ -367,7 +404,7 @@ def main():
                 "parallelism": (f"dp{world} ({'NVLink reduce-scatter+AdamW+all-gather kernels' if args.dp_impl == 'nvlink' else 'NCCL all-reduce'})"
                                 if world > 1 else "single"),
                 "optimizer": "stochastic_adamw bf16 states, fp32 grads, clip 5.0",
-                "l2": "working set (>10 GB weights+grads+activations) exceeds the 126 MB L2; 192 MB flush before timing",
+                "l2": "working set (>10 GB weights+grads+activations) exceeds the 50 MB L2; 256 MB flush before timing",
             },
             "clocks": clocks,
             "e2e": e2e,

@@ -1,4 +1,4 @@
-"""Native tcgen05 flash attention (forward, both P variants, and backward) vs PyTorch SDPA on cuDNN, flagship shapes.
+"""Native wgmma flash attention (forward, both P variants, and backward) vs PyTorch SDPA on cuDNN, flagship shapes.
 
 Device-timed with CUDA events, 256 MB L2 flush between iterations, median of 20 after 3 warm-ups.
 FLOPs: forward 4*B*H*Sq*Sk*D (x0.5 causal); backward 2.5x forward (the usual convention: 5 GEMMs vs 2)."""

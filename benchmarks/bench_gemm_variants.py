@@ -1,4 +1,4 @@
-"""GEMM variants side by side on one B200: single-CTA tcgen05 kernel, CTA-pair (cta_group::2) kernel, cuBLAS (torch.matmul),
+"""GEMM variants side by side on one H100: single-CTA wgmma kernel, CTA-pair (two-CTA cluster, B multicast) kernel, cuBLAS (torch.matmul),
 fp8 (row/column scaled) and MXFP8 kernels.  CUDA events, warm-up, L2 flush between iterations, median of ``--iters``.
 
     python benchmarks/bench_gemm_variants.py --out gpurun_out/bench_gemm_variants.json

@@ -23,7 +23,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], d["bf16_tflops"], "measured"
-    return 6650.0, 1590.0, "fallback"
+    return 3350.0, 989.0, "H100 SXM data sheet (HBM3, dense bf16)"
 
 
 _flush = None
@@ -51,7 +51,7 @@ def timeit(fn, iters=10, warmup=3):
 
 def timeit_rotating(make_call, working_set_bytes, iters=5, min_total_bytes=1 << 30):
     """Throughput timing for short memory-bound kernels: ``n`` argument sets whose combined footprint is far larger than
-    the 126 MB L2 are processed back to back between two events (no launch gap in the measurement, every byte comes from
+    the 50 MB L2 are processed back to back between two events (no launch gap in the measurement, every byte comes from
     HBM).  ``make_call(i)`` returns the zero-argument callable for set ``i``.  Returns ms per call."""
     n = max(2, -(-min_total_bytes // max(working_set_bytes, 1)))
     calls = [make_call(i) for i in range(n)]

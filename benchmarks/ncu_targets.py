@@ -54,7 +54,7 @@ def main() -> None:
     pitch = (V + 7) // 8 * 8
     dl = torch.empty(chunk, pitch, **bf)[:, :V]
     ops.ce_dlogits(x[:chunk], wv, tgt[:chunk], lse[:chunk], torch.ones(chunk, device=dev), dl, -100)
-    # 9) flash-attention forward (own tcgen05 kernel), flagship shape
+    # 9) flash-attention forward (own wgmma kernel), flagship shape
     B, S, Hq, Hk, D = 8, 2048, 16, 4, 128
     q = torch.randn(B, S, Hq, D, **bf)
     kk = torch.randn(B, S, Hk, D, **bf)

@@ -1,13 +1,13 @@
 """Fused linear + cross-entropy that never materialises ``[tokens, vocab]`` logits.
 
 Replaces the reference's dependency on the cut-cross-entropy Triton kernels (``d9d/kernel/cce/cce.py:47-298``,
-``main.py:119-225``) with epilogues of the hand-written tcgen05 GEMM:
+``main.py:119-225``) with epilogues of the hand-written wgmma GEMM:
 
-* forward : logits tiles stay in TMEM; the epilogue reduces them to online-softmax partials and the target logit
+* forward : logits tiles stay in registers; the epilogue reduces them to online-softmax partials and the target logit
   (bias and tanh soft-capping are applied in the same epilogue);
 * backward: the vocabulary is walked in *column chunks*.  For a chunk ``C[v0:v1]`` of the classifier the logits are
   recomputed and the epilogue writes ``g * (softmax - onehot) * dsoftcap`` as bf16 into one reusable
-  ``[tokens, v1 - v0]`` buffer, which feeds two more tcgen05 GEMMs: ``dE += dL @ C[v0:v1]`` (fp32 accumulation in the
+  ``[tokens, v1 - v0]`` buffer, which feeds two more wgmma GEMMs: ``dE += dL @ C[v0:v1]`` (fp32 accumulation in the
   epilogue) and ``dC[v0:v1] = dL^T @ E`` (full reduction depth = all tokens, so every row of ``dC`` is written exactly
   once - straight into the pre-allocated gradient buffer when the gradient infrastructure provides one).
   Chunking over *columns* instead of tokens is what keeps the extra memory small (default 256 MiB instead of the
@@ -93,7 +93,7 @@ class _EmulatedOps:
         d.copy_((d.float() + r if accumulate else r).to(d.dtype))
 
 
-def plan_vocab_chunks(split_sizes: Sequence[int], tokens: int, hidden: int, budget_bytes: int, sm_count: int = 148,
+def plan_vocab_chunks(split_sizes: Sequence[int], tokens: int, hidden: int, budget_bytes: int, sm_count: int = 132,
                       ) -> tuple[list[tuple[int, int, int]], int, bool]:
     """Column chunks ``(split, row_begin, row_end)`` of the classifier for the backward pass.
 
@@ -134,7 +134,7 @@ def plan_vocab_chunks(split_sizes: Sequence[int], tokens: int, hidden: int, budg
 def _sm_count(device: torch.device) -> int:
     if device.type == "cuda":
         return torch.cuda.get_device_properties(device).multi_processor_count
-    return 148
+    return 132
 
 
 class _LinearCEFunction(Function):

@@ -16,7 +16,7 @@ Block attention has two implementations:
 * ``plan`` (CUDA default when the native flash kernels support the tensors): every rank's tokens are split into *runs* of
   consecutive global positions (one run for the contiguous layout, two for zig-zag); a (query run, key run) pair is then
   either fully visible, causal with aligned diagonals, or invisible, so a block is a handful of calls of the native
-  tcgen05 flash-attention forward / backward kernels (``ops/csrc/flash_attn.cu``) on row slices - per-call ``(out, lse)``
+  wgmma flash-attention forward / backward kernels (``ops/csrc/flash_attn.cu``) on row slices - per-call ``(out, lse)``
   are merged exactly like whole blocks are, and the backward kernels take the *global* ``out`` / ``lse`` rows.  No score
   matrix is materialised.
 * ``mask`` (CPU, layouts whose run pairs overlap partially, tensors the kernels do not take): PyTorch matmuls over a

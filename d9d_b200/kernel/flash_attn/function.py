@@ -4,7 +4,7 @@ sinks (with analytic ``dsink``), optional LSE.
 
 Backends:
 * ``attention_reference``: exact fp32 math (CPU tensors; the oracle of the numerics tests),
-* CUDA: the native tcgen05 flash-attention forward / backward kernels (``native.py``), every option in-kernel.
+* CUDA: the native wgmma flash-attention forward / backward kernels (``native.py``), every option in-kernel.
 """
 
 from __future__ import annotations
@@ -105,7 +105,7 @@ def flash_attn_func(
 ) -> tuple[torch.Tensor, torch.Tensor | None]:
     """Returns ``(output [B,S,H,Dv], lse [B,H,S] or None)``.
 
-    CUDA bf16 tensors with head size 64 / 128 run the native tcgen05 kernels (forward and backward, every option);
+    CUDA bf16 tensors with head size 64 / 128 run the native wgmma kernels (forward and backward, every option);
     other CUDA inputs use SDPA for plain / causal attention and raise for options it cannot express - the fp32 oracle
     (which materialises the score matrix) is only taken on CPU or for tiny problems.
     """

@@ -1,8 +1,7 @@
-"""CUDA path for attention: the hand-written tcgen05 flash-attention kernels (``ops/csrc/flash_attn.cu``).
+"""CUDA path for attention: the hand-written wgmma flash-attention kernels (``ops/csrc/flash_attn.cu``).
 
-Forward: two 128-row query tiles per CTA ping-ponged over one K/V ring, S and O accumulators in TMEM, P handed to the second
-GEMM through 128B-swizzled shared memory (which frees the S columns for the next score tile at once), lazy online-softmax
-rescaling, LSE out.  Backward: delta pre-pass, a dK/dV
+Forward: one 128-row query tile per CTA (64 rows per consumer warpgroup) over K/V rings filled by TMA, S and O
+accumulators in registers, P handed to the second GEMM as its register A operand, online softmax, LSE out.  Backward: delta pre-pass, a dK/dV
 kernel (K,V resident, Q/dO streamed over the heads of the GQA group) and a dQ kernel (Q,dO resident, K/V streamed); no
 atomics.  Causal / sliding window (left, right) / soft-cap / attention sinks / packed variable-length batches are all
 handled inside the kernels.  There is no library (cuDNN / SDPA) call on this path.

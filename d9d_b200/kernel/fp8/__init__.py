@@ -1,13 +1,13 @@
-"""FP8 (e4m3) linear algebra on the 5th-generation tensor cores.
+"""FP8 (e4m3) linear algebra on the Hopper tensor cores (wgmma).
 
-Two operand recipes, both with fp32 accumulation in tensor memory and a bf16 result:
+Two operand recipes, both with fp32 accumulation in registers and a bf16 result:
 
-* **row / column scaling** (``kind::f8f6f4``): one fp32 scale per row of each operand (per token / per output channel),
+* **row / column scaling**: one fp32 scale per row of each operand (per token / per output channel),
   applied to the accumulator in the GEMM epilogue.  Used by :class:`Fp8LinearFunction` for all three GEMMs of a linear
   layer (forward, input gradient, weight gradient); the two backward GEMMs need K-major operands along the *other*
   dimension, which the transposing column-wise quantiser produces in one pass.
-* **MXFP8** (``kind::mxf8f6f4.block_scale``): OCP micro-scaling - one power-of-two (UE8M0) scale per 32 consecutive
-  K-elements, consumed by the tensor core itself (scale factors staged in tensor memory by ``tcgen05.cp``).
+* **MXFP8**: OCP micro-scaling - one power-of-two (UE8M0) scale per 32 consecutive
+  K-elements; every K=32 wgmma produces a partial product that is added to the accumulator with its two scales.
 
 The reference framework has no fp8 path of its own (its published fp8 numbers come from torchao-style recipes layered on
 top); this module is the native equivalent.  Every function has a PyTorch emulation (same rounding, same scale rules) that
@@ -150,7 +150,7 @@ class Fp8LinearFunction(Function):
 
 class MxFp8LinearFunction(Function):
     """``y = x @ W^T`` with all three GEMMs in **MXFP8** (e4m3 elements, one power-of-two scale per 32 elements of the
-    reduction dimension, consumed by ``tcgen05.mma.kind::mxf8f6f4.block_scale``).
+    reduction dimension, applied to the K=32 partial products of the GEMM).
 
     Every GEMM quantises both operands along *its own* reduction dimension, so the backward GEMMs work on transposed copies:
 

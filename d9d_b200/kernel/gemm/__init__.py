@@ -1,4 +1,4 @@
-"""Dense linear layers on the hand-written tcgen05 GEMM (TMA-fed, TMEM accumulators, persistent, warp-specialised).
+"""Dense linear layers on the hand-written wgmma GEMM (TMA-fed, register accumulators, persistent, warp-specialised).
 
 * forward   ``y = x @ W^T``                       K-major A and B
 * dgrad     ``dx = dy @ W``                       B consumed MN-major straight from ``W[out, in]`` (no transpose)
@@ -73,7 +73,7 @@ class LinearFunction(Function):
 
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = None) -> torch.Tensor:
-    """``x @ weight^T (+ bias)``; native tcgen05 path for bf16 CUDA tensors, ``F.linear`` on CPU."""
+    """``x @ weight^T (+ bias)``; native wgmma path for bf16 CUDA tensors, ``F.linear`` on CPU."""
     if on_gpu(x) and x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16:
         x2 = x.reshape(-1, x.shape[-1])
         if _tma_ok(weight) and x2.shape[-1] % 8 == 0 and weight.shape[0] % 8 == 0 and x2.numel() > 0:

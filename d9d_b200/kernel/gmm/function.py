@@ -2,7 +2,7 @@
 
 The reference delegates to the ``grouped_gemm`` wheel and needs ``batch_sizes`` on the CPU.  This compatibility
 entry keeps that contract (arbitrary group sizes) by re-packing rows into the 128-row aligned layout the native
-tcgen05 grouped GEMM works on; the model path (``GroupedSwiGLU``) uses the aligned layout end-to-end and never
+wgmma grouped GEMM works on; the model path (``GroupedSwiGLU``) uses the aligned layout end-to-end and never
 comes through here.
 """
 

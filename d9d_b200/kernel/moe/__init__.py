@@ -1,8 +1,8 @@
 """MoE token routing kernels.
 
-B200-native path (``layout.py``): a stable counting sort builds a 128-row aligned, expert-sorted layout *on the
+Native path (``layout.py``): a stable counting sort builds a 128-row aligned, expert-sorted layout *on the
 device* (no ``bincount().cpu()``, no host-side ``batch_sizes``), tokens are scattered/gathered by fused kernels and
-the grouped tcgen05 GEMM walks a device-side tile->expert table.
+the grouped wgmma GEMM walks a device-side tile->expert table.
 
 Compatibility surface (``compat.py``): ``fused_indices_to_multihot``, ``moe_permute_with_probs``,
 ``moe_unpermute_mask`` with the reference's signatures (``d9d/kernel/moe/*.py``).

@@ -2,7 +2,7 @@
 
 SR primitive: add 16 counter-based random bits (Philox-4x32-10 keyed by ``(seed, element offset)``) below the kept
 bf16 mantissa, truncate.  Unbiased, reproducible, independent of launch geometry.
-B200 difference: AdamW is a *multi-tensor* launch (one kernel for a whole parameter group) with an optional
+Difference from the reference: AdamW is a *multi-tensor* launch (one kernel for a whole parameter group) with an optional
 device-side gradient scale (fuses ``grad / sum(loss_weight)`` and clipping into the update).
 """
 

@@ -43,7 +43,7 @@ class ExpertParallelCommunicationHandler(ExpertCommunicationHandler):
     2. per-expert counts are exchanged (one small all-to-all), then rows, routing probabilities and local expert
        ids travel with one variable-split all-to-all each;
     3. the receiver builds a 128-row aligned :class:`MoELayout` over what it received (rows arrive ordered by
-       source rank, the layout regroups them by local expert) and the grouped tcgen05 GEMMs consume it directly;
+       source rank, the layout regroups them by local expert) and the grouped wgmma GEMMs consume it directly;
     4. ``combine`` walks the same path backwards and sums each token's ``top_k`` partial outputs in fp32.
 
     The only host synchronisation is the read of the split sizes that NCCL's all-to-all needs.

@@ -25,7 +25,7 @@ def _local_weight(linear: GroupedLinear) -> torch.Tensor:
 class GroupedSwiGLU(nn.Module, ModuleLateInit):
     """All experts' SwiGLU FFNs as three grouped GEMMs: ``probs * down(silu(gate(x)) * up(x))``.
 
-    Parity: reference ``d9d/module/block/moe/grouped_experts.py:10-73``.  On the B200 path the routing probability
+    Parity: reference ``d9d/module/block/moe/grouped_experts.py:10-73``.  On the native path the routing probability
     is folded into the SiLU·mul kernel (``down`` is linear, so scaling its input equals scaling its output).
     """
 

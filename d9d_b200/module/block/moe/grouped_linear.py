@@ -16,7 +16,7 @@ from d9d_b200.module.base import ModuleLateInit
 class GroupedLinear(nn.Module, ModuleLateInit):
     """``E`` independent linear maps with weight ``[E, in, out]`` applied to expert-sorted rows.
 
-    ``x_groups`` is either a device-side :class:`MoELayout` (B200 path: aligned layout, tcgen05 grouped GEMM, no host
+    ``x_groups`` is either a device-side :class:`MoELayout` (native path: aligned layout, wgmma grouped GEMM, no host
     sync) or — for compatibility with the reference contract (``d9d/module/block/moe/grouped_linear.py:12-71``) —
     a CPU tensor with the number of rows per expert.
     """

@@ -1,6 +1,6 @@
 """Rotary embeddings (reference ``d9d/module/block/positional/rope.py:10-216``).
 
-B200 difference: the applicator is one fused kernel per tensor (``d9d_b200.kernel.rope``) instead of eager
+Difference from the reference: the applicator is one fused kernel per tensor (``d9d_b200.kernel.rope``) instead of eager
 ``q*cos + rotate(q)*sin``; cos/sin caches are kept in fp32.
 """
 

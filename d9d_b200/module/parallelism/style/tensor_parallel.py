@@ -7,7 +7,7 @@
 ``RowwiseLinearParallel``  shards the *input* features: ``W -> Shard(1)``; partial outputs are all-reduced
 (all-reduce forward / identity backward) or reduce-scattered along the sequence dim when ``sequence_parallel``.
 
-With ``sequence_parallel=True`` on CUDA the collective is fused into the tcgen05 GEMM over NVLink peer memory
+With ``sequence_parallel=True`` on CUDA the collective is fused into the wgmma GEMM over NVLink peer memory
 (``d9d_b200.kernel.tp``): all-gather→GEMM loads every A tile from the owning peer through TMA, GEMM→reduce-scatter
 TMA reduce-adds every output tile into the owner's shard; backward uses the mirrored kernels.  Otherwise (CPU/gloo,
 unsupported shapes, plain all-reduce TP) the collectives are autograd functions over the ``tp`` process group around

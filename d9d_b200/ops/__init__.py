@@ -1,4 +1,4 @@
-"""Native sm_100a ops for d9d_b200 (hand-written CUDA: tcgen05/TMEM GEMMs fed by TMA, fused elementwise kernels).
+"""Native sm_90a ops for d9d_b200 (hand-written CUDA: wgmma GEMMs fed by TMA, fused elementwise kernels).
 
 ``ops.load()`` loads (building first if necessary) the in-tree extension and returns ``torch.ops.d9d_b200``.
 On a machine with a GPU the ops are mandatory: callers must not silently fall back to PyTorch.

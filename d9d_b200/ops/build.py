@@ -1,6 +1,6 @@
-"""In-tree build of the native sm_100a extension.
+"""In-tree build of the native sm_90a (H100) extension.
 
-* ``*.cu`` translation units are compiled with ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` and do
+* ``*.cu`` translation units are compiled with ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` and do
   not include torch headers (seconds per file).
 * ``bindings.cpp`` (TORCH_LIBRARY registration) is compiled with the host compiler against torch.
 * The result is ``d9d_b200/ops/_lib/d9d_b200_ops.so`` – it lives in-tree so it travels with the repo snapshot to
@@ -28,7 +28,7 @@ STAMP_PATH = LIB_DIR / "d9d_b200_ops.stamp.json"
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",
@@ -109,7 +109,7 @@ def _compile_one(cmd: list[str], src: Path, obj: Path, flags: list[str], verbose
 
 
 def build(verbose: bool = True, force: bool = False) -> Path:
-    """Compile every CUDA/C++ source for sm_100a and link the extension. Returns the .so path."""
+    """Compile every CUDA/C++ source for sm_90a and link the extension. Returns the .so path."""
     import torch
     from torch.utils import cpp_extension
 

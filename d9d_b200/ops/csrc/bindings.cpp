@@ -1,4 +1,4 @@
-// d9d_b200 — torch bindings (TORCH_LIBRARY) for the native sm_100a kernels.
+// d9d_b200 — torch bindings (TORCH_LIBRARY) for the native sm_90a kernels.
 // Compiled with the host compiler only; the kernels live in *.cu translation units that do not include torch.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -194,7 +194,7 @@ std::tuple<Tensor, Tensor> quantize_colwise_t(const Tensor& x) {
 }
 
 // x[M,K] bf16 -> (q[M,K] e4m3, sf uint8 [2*ceil(M/256), K/128, 512]): OCP MXFP8, one UE8M0 scale per 32 elements along K,
-// stored in the 128-row x 4-group block layout tcgen05.cp expects
+// stored in the 128-row x 4-group block layout the MXFP8 GEMM reads
 std::tuple<Tensor, Tensor> quantize_mx(const Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.stride(1) == 1 && x.scalar_type() == at::kBFloat16, "quantize_mx: 2-D bf16 CUDA tensor required");
   TORCH_CHECK(x.size(1) % 128 == 0 && x.stride(0) % 8 == 0 && (reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0,

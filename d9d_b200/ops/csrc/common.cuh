@@ -1,8 +1,9 @@
-// d9d_b200 — shared device-side primitives for sm_100a (B200).
+// d9d_b200 — shared device-side primitives for sm_90a (H100).
 //
-// Everything in here is hand-written inline PTX for the Blackwell execution
-// model: mbarrier pipelines, TMA (cp.async.bulk.tensor), tcgen05 (UMMA) with
-// TMEM accumulators.  No CUTLASS / CuTe dependency.
+// Everything in here is hand-written inline PTX for the Hopper execution
+// model: mbarrier pipelines, TMA (cp.async.bulk.tensor, multicast within a
+// cluster), register-resident wgmma accumulators (wgmma.cuh).  No CUTLASS / CuTe
+// dependency.
 #pragma once
 
 #include <cuda.h>
@@ -10,6 +11,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma.cuh"
 
 #ifndef D9D_WATCHDOG
 #define D9D_WATCHDOG 1  // bounded mbarrier spins: a protocol bug traps instead of hanging the GPU
@@ -108,6 +111,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #endif
 }
 
+// Same wait for kernels that issue wgmma: any function call (printf) in such a kernel makes ptxas serialise every
+// wgmma of it, so the watchdog only traps.
+__device__ __forceinline__ void mbar_wait_wg(uint64_t* bar, uint32_t parity) {
+#if D9D_WATCHDOG
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 24)) __trap();
+  }
+#else
+  while (!mbar_try_wait(bar, parity)) {
+  }
+#endif
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA
 // ----------------------------------------------------------------------------------------------
@@ -171,128 +188,14 @@ __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;\n" ::"n"(N) : "memory");
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
 
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], bf16/fp16 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]  (A operand sourced from tensor memory; used by attention P·V)
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
-
-// 32 lanes x 32 columns of 32-bit: thread t of the warp receives lane (base_lane + t), columns [c, c+32).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts per PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor")
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a 128B-swizzled tile.
-//   bits [0,14)  start address >> 4          bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset >> 4 bits [46,48) version (1 on sm_100)
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulate.
-//   [4,6) c_format (1=f32) [7,10) a_format (1=bf16) [10,13) b_format [15] a_major (1=MN) [16] b_major
-//   [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
+// named barrier over `threads` threads (a multiple of 32) of the CTA
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -336,39 +239,9 @@ __device__ __forceinline__ uint16_t sr_bf16_bits(float x, uint32_t rnd16) {
 }  // namespace d9d
 
 // ----------------------------------------------------------------------------------------------
-// fp8 (kind::f8f6f4) and block-scaled fp8 (kind::mxf8f6f4) MMA, scale-factor staging
+// bulk copies
 // ----------------------------------------------------------------------------------------------
 namespace d9d {
-
-// D[tmem] (+)= A[smem] * B[smem], e4m3 / e5m2 inputs (32 K-elements per instruction), fp32 accumulate.
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Block-scaled variant: every 32 K-elements of a row of A / B carry one UE8M0 scale factor living in tensor memory.
-__device__ __forceinline__ void umma_mxf8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate,
-                                          uint32_t tmem_sfa, uint32_t tmem_sfb) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(tmem_sfa), "r"(tmem_sfb)
-      : "memory");
-}
-
-// smem -> tmem copy of one scale-factor block: 32 rows x 16 bytes, replicated into the four 32-lane quadrants.
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t tmem_dst, uint64_t smem_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;\n" ::"r"(tmem_dst), "l"(smem_desc) : "memory");
-}
 
 // 1-D bulk copy global -> shared, completion counted on an mbarrier (bytes: multiple of 16, both addresses 16-byte aligned)
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
@@ -378,41 +251,13 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_sr
                : "memory");
 }
 
-// Shared-memory matrix descriptor without swizzling (K-major "interleave" layout): 8-row x 16-byte core matrices,
-// `sbo_bytes` between consecutive 8-row groups, `lbo_bytes` between core matrices along K.
-__device__ __forceinline__ uint64_t make_smem_desc_nosw(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
-
-// Instruction descriptor for kind::f8f6f4, e4m3 A/B (format code 0), fp32 accumulate, K-major operands.
-//   [4,6) c_format (1=f32) [7,10) a_format [10,13) b_format [17,23) N>>3 [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(uint32_t m, uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-// Instruction descriptor for kind::mxf8f6f4.block_scale, e4m3 A/B, UE8M0 scales, K-major operands.
-//   [4,6) b_sf_id [7,10) a_format [10,13) b_format [17,23) N>>3 [23] scale format (1 = UE8M0) [24,29) M>>4 [29,31) a_sf_id
-__host__ __device__ constexpr uint32_t make_idesc_mxe4m3(uint32_t m, uint32_t n, uint32_t a_sf_id, uint32_t b_sf_id) {
-  return (b_sf_id << 4) | ((n >> 3) << 17) | (1u << 23) | ((m >> 4) << 24) | (a_sf_id << 29);
-}
-
 }  // namespace d9d
 
 // ----------------------------------------------------------------------------------------------
-// CTA pairs (cta_group::2): two CTAs of a cluster on the two SMs of one TPC execute one 256-row UMMA.
-//   * each CTA stages its own 128 rows of A and its own half of B; the MMA (issued by the even CTA only) reads both
-//     halves, so every CTA loads / keeps only half of B per flop,
-//   * barriers that the issuing CTA waits on live in the even ("leader") CTA: clearing bit 24 of a shared::cluster
-//     address maps it onto the leader of the pair; completions that both CTAs wait on are multicast by tcgen05.commit.
+// Clusters: CTAs of one cluster share operand tiles through TMA multicast and release each other's stages through
+// remote mbarrier arrivals.
 // ----------------------------------------------------------------------------------------------
 namespace d9d {
-
-constexpr uint32_t PAIR_LEADER_MASK = 0xFEFFFFFFu;
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -425,50 +270,27 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
 }
 
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// TMA load into the executing CTA's shared memory whose completion bytes are counted on the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_3d_pair(void* smem_dst, const void* desc, uint64_t* bar, int c0, int c1, int c2) {
+// TMA load whose box lands at the same shared-memory offset in every CTA of `cta_mask`, completing on the mbarrier at
+// the same offset in each of them
+__device__ __forceinline__ void tma_load_3d_multicast(void* smem_dst, const void* desc, uint64_t* bar, uint16_t cta_mask, int c0,
+                                                      int c1, int c2) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-      "[%2];\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar) & PAIR_LEADER_MASK), "r"(c0), "r"(c1), "r"(c2)
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, %6}], "
+      "[%2], %3;\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 
-// D[tmem of both CTAs] (+)= A[256 x 16: 128 rows per CTA] * B[N x 16: N/2 rows per CTA]; issued by one thread of the leader
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// arrive on the mbarrier at this shared-memory offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      ".reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
       : "memory");
-}
-
-// Arrive on the mbarrier at this shared-memory offset in BOTH CTAs of the pair once all prior tcgen05 ops of this thread are done
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  const uint16_t mask = 0b11;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-
-// Arrive on the leader CTA's copy of a barrier (from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];\n" ::"r"(smem_u32(bar) & PAIR_LEADER_MASK) : "memory");
 }
 
 }  // namespace d9d

@@ -7,7 +7,7 @@
 
 namespace d9d {
 
-// ------------------------------------------------------------------ GEMM (tcgen05) ---------------
+// ------------------------------------------------------------------ GEMM (wgmma) -----------------
 struct GemmArgs {
   int mode = 0;        // gemm::Mode
   int epi = 0;         // gemm::Epi
@@ -65,7 +65,7 @@ int gemm_ce_block_n();
 void ce_finalize(const float* part_max, const float* part_sum, const float* tgt_logit, const long long* target,
                  long long ignore_index, int n_tiles, int M, float* lse, float* nll, cudaStream_t stream);
 
-// ------------------------------------------------------------------ fp8 GEMM (tcgen05 kind::f8f6f4 / mxf8f6f4) --
+// ------------------------------------------------------------------ fp8 GEMM (wgmma e4m3, MX block scales) -----
 struct Fp8GemmArgs {
   const void* A = nullptr;   // [M, K] e4m3, K contiguous (row pitch lda bytes)
   const void* B = nullptr;   // [N, K] e4m3

@@ -1,4 +1,4 @@
-// d9d_b200 — bandwidth-bound sm_100a kernels: RMSNorm fwd/bwd, SiLU·mul, stochastic-rounding copy,
+// d9d_b200 — bandwidth-bound sm_90a kernels: RMSNorm fwd/bwd, SiLU·mul, stochastic-rounding copy,
 // multi-tensor SR-AdamW, RoPE, grad utilities.  All 128-bit vectorised, fp32 math.
 #include <stdexcept>
 

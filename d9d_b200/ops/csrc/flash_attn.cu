@@ -1,4 +1,4 @@
-// d9d_b200 — flash attention forward + backward on tcgen05 (sm_100a).
+// d9d_b200 — flash attention forward + backward on wgmma (sm_90a).
 //
 //   O = softmax(scale * Q K^T + mask [, sink]) V            GQA (Hq = g * Hk), causal / sliding window (left, right),
 //                                                           optional tanh soft-cap, optional per-head attention sink,
@@ -7,26 +7,11 @@
 // All tensors are [rows, H, D] row-major views of the projection outputs (rows = B*S, or the packed token count):
 // no transposes, TMA 3-D maps (d, h, row) with 128B swizzle.  LSE / delta are fp32 [B, H, S] (packed: [H, total]).
 //
-// Forward (flash_attn_fwd_kernel): one CTA owns TWO consecutive 128-row query tiles of one (batch, head).
-//   warps 0-3 / 4-7  softmax warpgroup of query tile 0 / 1 (thread = query row): S row TMEM -> registers (the S columns are
-//                    handed back to the tensor core at once), online softmax with lazy rescaling (O is only rescaled when
-//                    the running max grows by more than 2^8), P (bf16) into 128B-swizzled shared memory
-//   warp 8           TMA producer: Q0, Q1 once, then K_j, V_j tiles through one ring
-//   warp 9           MMA issuer: S_w(j+1) = Q_w K_{j+1}^T is issued as soon as S_w(j) has been pulled into registers, so the
-//                    next score tile is computed while the exponentials of the current one are evaluated; O_w += P_w V_j
-//                    follows when P_w(j) is complete and runs under the softmax of j+1
-//   TMEM: S0 [0,128) S1 [128,256) O0 [256,256+D) O1 [256+D,256+2D)
-//
-// Backward = delta pre-pass + two tcgen05 kernels built from one template (no atomics, deterministic):
-//   DKV: CTA owns a 128-key tile of one kv head, keeps K,V resident, streams 64-row Q/dO half-tiles of every query
-//        head of the group:  S^T = K Q^T, dP^T = V dO^T (two threads per key row)  ->  P^T, dS^T as bf16 written back INTO
-//        THE SAME TMEM COLUMNS  ->  dV += P^T dO, dK += dS^T Q with the A operand read from tensor memory, accumulated in
-//        TMEM over the whole loop.
-//   DQ : CTA owns a 128-row query tile of one head, keeps Q,dO resident, streams 64-key K/V half-tiles:
-//        S = Q K^T, dP = dO V^T (two threads per query row) -> dS (TMEM) -> dQ += dS K.
-//   Two groups of 8 softmax warps alternate half-tiles (S/dP double-buffered in TMEM), so the MMAs of half-tile t+1 overlap
-//   the exponentials of half-tile t.   TMEM: S[u] u*64, dP[u] 128+u*64, acc1 [256,256+D), acc2 [256+D,256+2D).
-//
+// Forward (flash_attn_fwd_kernel): one CTA owns a 128-row query tile of one (batch, head); warpgroup 0 streams K / V tiles
+// of 128 keys with TMA, warpgroups 1-2 own 64 query rows each with S, P and O in registers (P is handed to the second
+// GEMM as its register A operand).
+// Backward = delta pre-pass + two wgmma kernels built from one template (no atomics, deterministic): see
+// flash_attn_bwd_kernel.
 // Reference parity: d9d/kernel/flash_attn/function.py:72-178 (fwd/bwd, sink gradient), :181-305 (varlen).
 #include <stdexcept>
 #include <string>
@@ -77,385 +62,229 @@ __device__ __forceinline__ SeqInfo resolve_seq(const FaParams& p, int b) {
   return s;
 }
 
-__device__ __forceinline__ float4 lds_f4(const float* smem_ptr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_u32(smem_ptr)));
-  return v;
-}
-
-// one bf16 row chunk (8 elements, 16 B) into a [rows x 128 B] 128B-swizzled box
-__device__ __forceinline__ void st_swizzled_16B(uint8_t* box, int row, int chunk, uint4 v) {
-  *reinterpret_cast<uint4*>(box + row * 128 + ((chunk ^ (row & 7)) << 4)) = v;
-}
-
 // ======================================================================================================
 // forward
 // ======================================================================================================
-constexpr int FWD_THREADS = 384;  // warps 0-3 / 4-7: softmax of query tile 0 / 1, 8: TMA producer, 9: MMA issuer, 10-11: idle
-                                  // (they complete the third warpgroup so that setmaxnreg can move registers to the softmax warps)
+constexpr int FA_THREADS = 384;  // warpgroup 0: TMA producer; warpgroups 1-2: 64 resident rows each
+constexpr int FA_CONSUMERS = 2;
 
-// Shared-memory descriptors are built once per operand (low word) and advanced by adding (byte offset >> 4): two integer
-// adds per tcgen05.mma instead of re-deriving the full 64-bit descriptor.
-constexpr uint32_t DESC_HI_SW128 = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO = 1024 B, version 1, SWIZZLE_128B
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | ((lbo_bytes >> 4) << 16);
+// wgmma operand descriptors of the [rows x 128 B] 128B-swizzled boxes TMA writes (one box per 64 head-dim columns)
+//   K-major operand (head dim = reduction):  k-step kk of 16 columns at box kk / 4, byte 32 (kk % 4) of every row
+//   MN-major operand (rows = reduction):     k-step kk = rows [16 kk, 16 kk + 16), LBO = distance between the d boxes
+__device__ __forceinline__ uint64_t desc_kmajor(uint32_t base, int box_bytes, int kk) {
+  return make_wgmma_desc(base + (kk >> 2) * box_bytes + (kk & 3) * 32, 16, 1024);
 }
-__device__ __forceinline__ void umma_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(DESC_HI_SW128)
-      : "memory");
+__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t base, int box_bytes, int kk) {
+  return make_wgmma_desc(base + kk * (16 * 128), box_bytes, 1024);
 }
-// offset (in 16-byte units) of UMMA_K step kk inside a K-major operand made of [rows x 128 B] boxes / an MN-major one
-__device__ __forceinline__ constexpr uint32_t koff_kmajor(int rows, int kk) { return ((kk >> 2) * (rows * 128) + (kk & 3) * 32) >> 4; }
-__device__ __forceinline__ constexpr uint32_t koff_mnmajor(int kk) { return (kk * 16 * 128) >> 4; }
 
-template <int N>
-__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
-template <int N>
-__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
+// accumulator columns [16 s, 16 s + 16) of an m64 fragment, rounded to bf16: the A operand of k-step s
+template <int R>
+__device__ __forceinline__ void pack_a_frag(const float (&d)[R], int s, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(d[8 * s + 0], d[8 * s + 1]);
+  a[1] = pack_bf16x2(d[8 * s + 2], d[8 * s + 3]);
+  a[2] = pack_bf16x2(d[8 * s + 4], d[8 * s + 5]);
+  a[3] = pack_bf16x2(d[8 * s + 6], d[8 * s + 7]);
+}
 
 template <int D>
 struct FwdCfg {
-  static constexpr int TILE_BYTES = 128 * D * 2;
-  static constexpr int NSLOT = 3;                       // K_j, V_j, K_{j+1}, ... through one ring
-  static constexpr int P_BYTES = 2 * 128 * 128 * 2;     // P of both query tiles (bf16, 128B-swizzled K-major)
-  static constexpr int SMEM_BYTES = 2 * TILE_BYTES + NSLOT * TILE_BYTES + P_BYTES + 1024 + 256;
+  static constexpr int TILE_BYTES = 128 * D * 2;  // Q tile and every K / V tile: 128 rows
+  static constexpr int NSLOT = 2;                 // K and V rings
+  static constexpr int SMEM_BYTES = TILE_BYTES + 2 * NSLOT * TILE_BYTES + 1024 + 256;
 };
 
-// Schedule.  S_w(j+1) is issued as soon as the softmax warps of tile w have pulled S_w(j) into registers (s_free), so the
-// next score tile is computed WHILE the exponentials of the current one are evaluated and a warpgroup goes from one
-// softmax straight into the next; P travels through shared memory (the S columns of TMEM are free again right away),
-// PV_w(j) is issued when P_w(j) is complete and runs under the softmax of j+1 (o_done orders it before the next P write /
-// O rescale).
+// One CTA owns a 128-row query tile of one (batch, head); each consumer warpgroup owns 64 of its rows and keeps S, P and O
+// in registers: S = Q K_j^T (wgmma from shared memory), online softmax on the fragment (a row lives in the 4 threads of a
+// quad), P packed to bf16 in place as the register A operand of O += P V_j.  The producer streams K_j / V_j through two
+// 2-slot rings, so the loads of tile j+1 run under the math of tile j.
 template <int D>
-__global__ void __launch_bounds__(FWD_THREADS, 1)
+__global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const FaParams p) {
   using C = FwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_q = smem;                                  // [2][TILE]
-  uint8_t* smem_ring = smem_q + 2 * C::TILE_BYTES;         // [NSLOT][TILE]
-  uint8_t* smem_p = smem_ring + C::NSLOT * C::TILE_BYTES;  // [2][128x128 bf16]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_p + C::P_BYTES);
-  uint64_t* bar_q = bars;            // 1
-  uint64_t* ring_full = bars + 1;    // [3]
-  uint64_t* ring_empty = bars + 4;   // [3]
-  uint64_t* s_full = bars + 7;       // [2]  S_w complete (tcgen05.commit)
-  uint64_t* s_free = bars + 9;       // [2]  S_w pulled into registers by its 4 softmax warps
-  uint64_t* p_ready = bars + 11;     // [2]  P_w written to shared memory
-  uint64_t* o_done = bars + 13;      // [2]  PV_w complete (tcgen05.commit)
-  uint64_t* o_final = bars + 15;     // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 17);
+  uint8_t* smem_q = smem;
+  uint8_t* smem_k = smem_q + C::TILE_BYTES;               // [NSLOT][TILE]
+  uint8_t* smem_v = smem_k + C::NSLOT * C::TILE_BYTES;    // [NSLOT][TILE]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + C::NSLOT * C::TILE_BYTES);
+  uint64_t* bar_q = bars;         // 1
+  uint64_t* k_full = bars + 1;    // [2]
+  uint64_t* k_empty = bars + 3;   // [2]
+  uint64_t* v_full = bars + 5;    // [2]
+  uint64_t* v_empty = bars + 7;   // [2]
 
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / (p.Hq / p.Hk);
   const SeqInfo sq = resolve_seq(p, b);
-  const int pair = gridDim.x - 1 - blockIdx.x;  // heavy (late) query tiles first
-  const int q0 = pair * 256;
+  const int q0 = (gridDim.x - 1 - blockIdx.x) * 128;  // heavy (late) query tiles first
   if (q0 >= sq.Sq) return;  // whole CTA exits together (varlen: shorter sequences)
 
-  // kv tile range of each query tile: [jlo[w], jhi[w])
-  int jlo[2], jhi[2];
-#pragma unroll
-  for (int w = 0; w < 2; ++w) {
-    const int qa = q0 + w * 128, qb = min(qa + 127, sq.Sq - 1);
-    if (qa >= sq.Sq) { jlo[w] = jhi[w] = 0; continue; }
-    const int klo = p.wl < 0 ? 0 : max(0, qa + sq.off - p.wl);
-    const int khi = p.wr < 0 ? sq.Sk - 1 : min(sq.Sk - 1, qb + sq.off + p.wr);
-    if (khi < klo) { jlo[w] = jhi[w] = 0; continue; }
-    jlo[w] = klo / 128;
-    jhi[w] = khi / 128 + 1;
-  }
-  int jbeg, jend;
-  if (jhi[0] == jlo[0]) { jbeg = jlo[1]; jend = jhi[1]; }
-  else if (jhi[1] == jlo[1]) { jbeg = jlo[0]; jend = jhi[0]; }
-  else { jbeg = min(jlo[0], jlo[1]); jend = max(jhi[0], jhi[1]); }
+  // kv tile range [jbeg, jend) of the query rows [q0, qb]
+  const int qb = min(q0 + 127, sq.Sq - 1);
+  const int klo = p.wl < 0 ? 0 : max(0, q0 + sq.off - p.wl);
+  const int khi = p.wr < 0 ? sq.Sk - 1 : min(sq.Sk - 1, qb + sq.off + p.wr);
+  const int jbeg = klo / 128, jend = (khi >= klo) ? khi / 128 + 1 : jbeg;
 
-  if (warp == 8 && elect_one()) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
     mbar_init(bar_q, 1);
-    for (int i = 0; i < C::NSLOT; ++i) { mbar_init(&ring_full[i], 1); mbar_init(&ring_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1); mbar_init(&s_free[i], 4); mbar_init(&p_ready[i], 4); mbar_init(&o_done[i], 1); mbar_init(&o_final[i], 1);
+    for (int i = 0; i < C::NSLOT; ++i) {
+      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], FA_CONSUMERS);
+      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], FA_CONSUMERS);
     }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc<512>(tmem_ptr_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp >= 8) {
-    setmaxnreg_dec<56>();
-    if (warp == 8) {
-      // ================= TMA producer =================
-      if (elect_one()) {
-        const int nq = (q0 + 128 < sq.Sq) ? 2 : 1;
-        mbar_arrive_expect_tx(bar_q, nq * C::TILE_BYTES);
-        for (int w = 0; w < nq; ++w)
+  if (warp < 4) {
+    // ================= TMA producer =================
+    setmaxnreg_dec<40>();
+    // a tile without visible keys loads nothing: its consumers never wait on bar_q, and no copy may still be landing in
+    // shared memory when the CTA exits
+    if (warp == 0 && jend > jbeg && elect_one()) {
+      mbar_arrive_expect_tx(bar_q, C::TILE_BYTES);
 #pragma unroll
-          for (int dc = 0; dc < D / 64; ++dc)
-            tma_load_3d(smem_q + w * C::TILE_BYTES + dc * (128 * 128), &tmap_q, bar_q, dc * 64, h, sq.q_start + q0 + w * 128);
-        int n = 0;
-        for (int j = jbeg; j < jend; ++j) {
+      for (int dc = 0; dc < D / 64; ++dc)
+        tma_load_3d(smem_q + dc * (128 * 128), &tmap_q, bar_q, dc * 64, h, sq.q_start + q0);
+      for (int j = jbeg; j < jend; ++j) {
+        const int n = j - jbeg, slot = n % C::NSLOT;
+        const uint32_t ph = (n / C::NSLOT) & 1;
+        mbar_wait_wg(&k_empty[slot], ph ^ 1);
+        mbar_arrive_expect_tx(&k_full[slot], C::TILE_BYTES);
 #pragma unroll
-          for (int kv = 0; kv < 2; ++kv, ++n) {
-            const int slot = n % C::NSLOT;
-            mbar_wait(&ring_empty[slot], ((n / C::NSLOT) & 1) ^ 1);
-            mbar_arrive_expect_tx(&ring_full[slot], C::TILE_BYTES);
+        for (int dc = 0; dc < D / 64; ++dc)
+          tma_load_3d(smem_k + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_k, &k_full[slot], dc * 64, hk, sq.k_start + j * 128);
+        mbar_wait_wg(&v_empty[slot], ph ^ 1);
+        mbar_arrive_expect_tx(&v_full[slot], C::TILE_BYTES);
 #pragma unroll
-            for (int dc = 0; dc < D / 64; ++dc)
-              tma_load_3d(smem_ring + slot * C::TILE_BYTES + dc * (128 * 128), kv == 0 ? &tmap_k : &tmap_v, &ring_full[slot],
-                          dc * 64, hk, sq.k_start + j * 128);
-          }
-        }
-      }
-    } else if (warp == 9) {
-      // ================= MMA issuer =================
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, D, false, true);
-      auto act = [&](int w, int j) { return j >= jlo[w] && j < jhi[w]; };
-      auto ring_wait = [&](int n) { mbar_wait(&ring_full[n % C::NSLOT], (n / C::NSLOT) & 1); tc_fence_after(); };
-      auto release = [&](int n) {
-        if (elect_one()) umma_commit(&ring_empty[n % C::NSLOT]);
-        __syncwarp();
-      };
-      auto issue_s = [&](int w, int n) {  // S_w = Q_w K^T, K tile in ring slot n % NSLOT
-        if (elect_one()) {
-          const uint32_t qa = desc_lo(smem_u32(smem_q + w * C::TILE_BYTES), 16);
-          const uint32_t ka = desc_lo(smem_u32(smem_ring + (n % C::NSLOT) * C::TILE_BYTES), 16);
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk)
-            umma_lo(tmem_base + w * 128, qa + koff_kmajor(128, kk), ka + koff_kmajor(128, kk), idesc_s, kk != 0);
-          umma_commit(&s_full[w]);
-        }
-        __syncwarp();
-      };
-      auto issue_pv = [&](int w, int n, int it, bool last) {  // O_w += P_w V, V tile in ring slot n % NSLOT
-        if (elect_one()) {
-          const uint32_t pa = desc_lo(smem_u32(smem_p + w * (128 * 128 * 2)), 16);
-          const uint32_t va = desc_lo(smem_u32(smem_ring + (n % C::NSLOT) * C::TILE_BYTES), 128 * 128);
-#pragma unroll
-          for (int kk = 0; kk < 128 / 16; ++kk)
-            umma_lo(tmem_base + 256 + w * D, pa + koff_kmajor(128, kk), va + koff_mnmajor(kk), idesc_o, (it | kk) != 0);
-          umma_commit(&o_done[w]);
-          if (last) umma_commit(&o_final[w]);
-        }
-        __syncwarp();
-      };
-      if (jend > jbeg) {
-        mbar_wait(bar_q, 0);
-        ring_wait(0);
-        if (act(0, jbeg)) issue_s(0, 0);
-        if (act(1, jbeg)) issue_s(1, 0);
-        release(0);
-        int it0 = 0, it1 = 0;
-        for (int j = jbeg; j < jend; ++j) {
-          const int n = 2 * (j - jbeg);
-          if (j + 1 < jend) {
-            ring_wait(n + 2);  // K_{j+1}
-            if (act(0, j + 1)) {
-              if (act(0, j)) { mbar_wait(&s_free[0], it0 & 1); tc_fence_after(); }
-              issue_s(0, n + 2);
-            }
-            if (act(1, j + 1)) {
-              if (act(1, j)) { mbar_wait(&s_free[1], it1 & 1); tc_fence_after(); }
-              issue_s(1, n + 2);
-            }
-            release(n + 2);
-          }
-          ring_wait(n + 1);  // V_j
-          if (act(0, j)) {
-            mbar_wait(&p_ready[0], it0 & 1);
-            tc_fence_after();
-            issue_pv(0, n + 1, it0, j == jhi[0] - 1);
-            ++it0;
-          }
-          if (act(1, j)) {
-            mbar_wait(&p_ready[1], it1 & 1);
-            tc_fence_after();
-            issue_pv(1, n + 1, it1, j == jhi[1] - 1);
-            ++it1;
-          }
-          release(n + 1);
-        }
+        for (int dc = 0; dc < D / 64; ++dc)
+          tma_load_3d(smem_v + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_v, &v_full[slot], dc * 64, hk, sq.k_start + j * 128);
       }
     }
   } else {
-    setmaxnreg_inc<224>();
-    // ================= softmax / correction / epilogue (thread = query row) =================
-    const int w = warp >> 2;                      // query tile of this warpgroup
-    const int row = (warp & 3) * 32 + lane;
-    const int qi = q0 + w * 128 + row;            // sequence-local query index
-    const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t tmem_s = tmem_base + w * 128 + lane_base;
-    const uint32_t tmem_o = tmem_base + 256 + w * D + lane_base;
-    const int n_it = jhi[w] - jlo[w];
-    const int k_lo = p.wl < 0 ? 0 : max(0, qi + sq.off - p.wl);
-    const int k_hi = p.wr < 0 ? sq.Sk - 1 : min(sq.Sk - 1, qi + sq.off + p.wr);
+    setmaxnreg_inc<232>();
+    // ================= consumers: softmax + both GEMMs of 64 query rows =================
+    const int cw = (warp >> 2) - 1, wq = warp & 3;
+    const int cq = (lane & 3) * 2;
+    const int row_l = cw * 64 + wq * 16 + (lane >> 2);  // tile rows row_l and row_l + 8 of this thread
+    const bool signal = (wq == 0 && lane == 0);
+    int k_lo[2], k_hi[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int qi = q0 + row_l + 8 * r;
+      k_lo[r] = p.wl < 0 ? 0 : max(0, qi + sq.off - p.wl);
+      k_hi[r] = p.wr < 0 ? sq.Sk - 1 : min(sq.Sk - 1, qi + sq.off + p.wr);
+    }
     const bool capped = p.softcap != 0.f;
     const float scale_eff = capped ? kLog2e : p.scale * kLog2e;  // log2-domain multiplier of the (capped) score
     const float cap_in = capped ? p.scale / p.softcap : 0.f;
-    float m_used = -INFINITY, l = 0.f;
-    for (int it = 0; it < n_it; ++it) {
-      const int k0 = (jlo[w] + it) * 128;
-      mbar_wait(&s_full[w], it & 1);
-      tc_fence_after();
-      uint32_t s[128];
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float o[D / 2];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t (&chunk)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[c * 32]);
-        tmem_ld_32x32b_x32(tmem_s + c * 32, chunk);
-      }
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_free[w]);  // the tensor core may overwrite S_w with the next score tile
-      if (capped) {
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    const uint32_t q_addr = smem_u32(smem_q) + cw * (64 * 128);
+    if (jend > jbeg) mbar_wait_wg(bar_q, 0);
+    for (int j = jbeg; j < jend; ++j) {
+      const int n = j - jbeg, slot = n % C::NSLOT;
+      const uint32_t ph = (n / C::NSLOT) & 1;
+      const int k0 = j * 128;
+      float s[64];
+      mbar_wait_wg(&k_full[slot], ph);
+      const uint32_t k_addr = smem_u32(smem_k + slot * C::TILE_BYTES);
+      wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 128; ++i) s[i] = __float_as_uint(p.softcap * tanhf(__uint_as_float(s[i]) * cap_in));
-      }
-      // boundary tiles only: out-of-window / out-of-sequence keys -> -inf (warp-uniform branches)
-      const int hi_rel = k_hi - k0, lo_rel = k_lo - k0;
-      if (__any_sync(0xffffffffu, hi_rel < 127)) {
+      for (int kk = 0; kk < D / 16; ++kk)
+        wgmma_bf16_ss<128, 0, 0>(s, desc_kmajor(q_addr, 128 * 128, kk), desc_kmajor(k_addr, 128 * 128, kk), kk != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      if (signal) mbar_arrive(&k_empty[slot]);
+      float alpha[2];
 #pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if (i > hi_rel) s[i] = __float_as_uint(-INFINITY);
-      }
-      if (__any_sync(0xffffffffu, lo_rel > 0)) {
+      for (int r = 0; r < 2; ++r) {
+        const int lo_rel = k_lo[r] - k0 - cq, hi_rel = k_hi[r] - k0 - cq;
+        float mx = -INFINITY;
 #pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if (i < lo_rel) s[i] = __float_as_uint(-INFINITY);
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
+        for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-      for (int i = 0; i < 128; i += 4) {
-        mx0 = fmaxf(mx0, __uint_as_float(s[i]));
-        mx1 = fmaxf(mx1, __uint_as_float(s[i + 1]));
-        mx2 = fmaxf(mx2, __uint_as_float(s[i + 2]));
-        mx3 = fmaxf(mx3, __uint_as_float(s[i + 3]));
-      }
-      const float m_new = fmaxf(m_used, fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * scale_eff);
-      // lazy rescaling: keep the stale maximum unless it is off by more than 2^8 (exact: O and l share the scaling)
-      float alpha = 1.f;
-      if (m_new - m_used > 8.f) {  // also true for the first finite maximum (m_used = -inf); false (NaN) while both are -inf
-        alpha = exp2f(m_used - m_new);
-        l *= alpha;
-        m_used = m_new;
-      }
-      if (it > 0) {
-        // PV_w(it-1) reads P_w from shared memory and accumulates into O_w: it must be complete before either is touched
-        mbar_wait(&o_done[w], (it - 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {
-#pragma unroll 1
-          for (int c = 0; c < D / 16; ++c) {  // 16 columns at a time: the S row stays live in registers
-            uint32_t o[16];
-            tmem_ld_32x32b_x16(tmem_o + c * 16, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32b_x16(tmem_o + c * 16, o);
+          for (int e = 0; e < 2; ++e) {
+            float x = s[4 * jj + 2 * r + e];
+            if (capped) x = p.softcap * tanhf(x * cap_in);
+            const int c = 8 * jj + e;  // key k0 + cq + c
+            x = (c < lo_rel || c > hi_rel) ? -INFINITY : x;
+            s[4 * jj + 2 * r + e] = x;
+            mx = fmaxf(mx, x);
           }
-          tmem_st_wait();
         }
-      }
-      const float neg_m = (m_used == -INFINITY) ? 0.f : -m_used;
-      float sum0 = 0.f, sum1 = 0.f;
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m[r], mx * scale_eff);
+        alpha[r] = (m_new == -INFINITY) ? 1.f : exp2f(m[r] - m_new);
+        m[r] = m_new;
+        l[r] *= alpha[r];
+        const float neg_m = (m_new == -INFINITY) ? 0.f : -m_new;
+        float sum = 0.f;
 #pragma unroll
-      for (int c = 0; c < 16; ++c) {  // 8 keys = one 16-byte chunk of the swizzled P row
-        uint32_t pk[4];
+        for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float p0 = exp2f(fmaf(__uint_as_float(s[c * 8 + 2 * e]), scale_eff, neg_m));
-          const float p1 = exp2f(fmaf(__uint_as_float(s[c * 8 + 2 * e + 1]), scale_eff, neg_m));
-          sum0 += p0;
-          sum1 += p1;
-          pk[e] = pack_bf16x2(p0, p1);
+          for (int e = 0; e < 2; ++e) {
+            const float pv = exp2f(fmaf(s[4 * jj + 2 * r + e], scale_eff, neg_m));
+            s[4 * jj + 2 * r + e] = pv;
+            sum += pv;
+          }
         }
-        st_swizzled_16B(smem_p + w * (128 * 128 * 2) + (c >> 3) * (128 * 128), row, c & 7, make_uint4(pk[0], pk[1], pk[2], pk[3]));
+        l[r] += sum;  // partial over this thread's columns; the quad is summed once at the end
       }
-      l += sum0 + sum1;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_ready[w]);
+#pragma unroll
+      for (int jj = 0; jj < D / 8; ++jj) {
+        o[4 * jj + 0] *= alpha[0]; o[4 * jj + 1] *= alpha[0];
+        o[4 * jj + 2] *= alpha[1]; o[4 * jj + 3] *= alpha[1];
+      }
+      uint32_t pa[8][4];
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) pack_a_frag(s, ks, pa[ks]);
+      mbar_wait_wg(&v_full[slot], ph);
+      const uint32_t v_addr = smem_u32(smem_v + slot * C::TILE_BYTES);
+      wgmma_fence_regs(o);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) wgmma_bf16_rs<D, 1>(o, pa[ks], desc_mnmajor(v_addr, 128 * 128, ks), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      if (signal) mbar_arrive(&v_empty[slot]);
     }
     // ---- epilogue: O / l -> global, LSE (natural log; the sink joins the denominator)
-    const bool row_ok = qi < sq.Sq;
-    if (n_it > 0) {
-      mbar_wait(&o_final[w], 0);
-      tc_fence_after();
-    }
-    const float m_safe = (m_used == -INFINITY) ? 0.f : m_used;
-    if (p.sink != nullptr) l += exp2f(p.sink[h] * kLog2e - m_safe);
-    const float inv_l = (l > 0.f) ? 1.f / l : 0.f;
-    if (q0 + w * 128 < sq.Sq) {
-      __nv_bfloat16* dst = p.out + (static_cast<long long>(sq.q_start + qi) * p.Hq + h) * D;
 #pragma unroll
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t o[32];
-        if (n_it > 0) {
-          tmem_ld_32x32b_x32(tmem_o + c * 32, o);
-          tmem_ld_wait();
-        } else {
+    for (int r = 0; r < 2; ++r) {
+      float lr = l[r];
+      lr += __shfl_xor_sync(0xffffffffu, lr, 1);
+      lr += __shfl_xor_sync(0xffffffffu, lr, 2);
+      const float m_safe = (m[r] == -INFINITY) ? 0.f : m[r];
+      if (p.sink != nullptr) lr += exp2f(p.sink[h] * kLog2e - m_safe);
+      const float inv_l = (lr > 0.f) ? 1.f / lr : 0.f;
+      const int qi = q0 + row_l + 8 * r;
+      if (qi < sq.Sq) {
+        __nv_bfloat16* dst = p.out + (static_cast<long long>(sq.q_start + qi) * p.Hq + h) * D + cq;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = 0;
-        }
-        if (row_ok) {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(o[v * 8 + 0]) * inv_l, __uint_as_float(o[v * 8 + 1]) * inv_l);
-            u.y = pack_bf16x2(__uint_as_float(o[v * 8 + 2]) * inv_l, __uint_as_float(o[v * 8 + 3]) * inv_l);
-            u.z = pack_bf16x2(__uint_as_float(o[v * 8 + 4]) * inv_l, __uint_as_float(o[v * 8 + 5]) * inv_l);
-            u.w = pack_bf16x2(__uint_as_float(o[v * 8 + 6]) * inv_l, __uint_as_float(o[v * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(dst + c * 32 + v * 8) = u;
-          }
-        }
+        for (int jj = 0; jj < D / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * r] * inv_l, o[4 * jj + 2 * r + 1] * inv_l);
+        if ((lane & 3) == 0 && p.lse != nullptr)
+          p.lse[sq.lse_base + static_cast<long long>(h) * p.lse_hs + qi] = (lr > 0.f) ? (m_safe + log2f(lr)) * kLn2 : -INFINITY;
       }
-      if (row_ok && p.lse != nullptr)
-        p.lse[sq.lse_base + static_cast<long long>(h) * p.lse_hs + qi] = (l > 0.f) ? (m_safe + log2f(l)) * kLn2 : -INFINITY;
     }
-    tc_fence_before();
   }
-
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 9) tmem_dealloc<512>(tmem_base);
 }
 
 // ======================================================================================================
 // backward
 // ======================================================================================================
-constexpr int BWD_THREADS = 576;  // 16 softmax warps + TMA producer + MMA issuer
-constexpr int BWD_NST = 4;        // streamed half-tile ring depth
-
-__device__ __forceinline__ void umma_ts_lo(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 db;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(DESC_HI_SW128)
-      : "memory");
-}
+constexpr int BWD_NST = 4;  // streamed half-tile ring depth
 
 template <int D, bool DKV>
 struct BwdCfg {
@@ -465,11 +294,14 @@ struct BwdCfg {
   static constexpr int SMEM_BYTES = 2 * RES_BYTES + BWD_NST * 2 * STR_BYTES + VEC_BYTES + 1024 + 256;
 };
 
-// P^T / dS^T (DKV) resp. dS (DQ) never touch shared memory: each softmax thread writes its bf16 values back into the TMEM
-// columns its fp32 S / dP values came from, and the accumulating GEMMs read their A operand from tensor memory.
-//   packed column of streamed index c (0..63) inside the 64-column buffer:  (c / 32) * 32 + (c % 32) / 2
+// Two kernels from one template (no atomics, deterministic):
+//   DKV: CTA owns a 128-key tile of one kv head (64 keys per consumer warpgroup), keeps K,V resident, streams 64-row Q/dO
+//        half-tiles of every query head of the group: S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T (registers, bf16 A operands)
+//        -> dV += P^T dO, dK += dS^T Q accumulated in registers over the whole loop.
+//   DQ : CTA owns a 128-row query tile of one head, keeps Q,dO resident, streams 64-key K/V half-tiles:
+//        S = Q K^T, dP = dO V^T -> dS -> dQ += dS K.
 template <int D, bool DKV>
-__global__ void __launch_bounds__(BWD_THREADS, 1)
+__global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_constant__ CUtensorMap tmap_r2,
                       const __grid_constant__ CUtensorMap tmap_s1, const __grid_constant__ CUtensorMap tmap_s2, const FaParams p) {
   // DKV: r1 = K, r2 = V (128-row boxes), s1 = Q, s2 = dO (64-row boxes).   DQ: r1 = Q, r2 = dO, s1 = K, s2 = V.
@@ -484,10 +316,6 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
   uint64_t* r_full = bars;          // 1
   uint64_t* st_full = bars + 1;     // [NST]
   uint64_t* st_empty = bars + 5;    // [NST]
-  uint64_t* sp_full = bars + 9;     // [2]  S / dP of buffer u complete
-  uint64_t* pd_ready = bars + 11;   // [2]  bf16 P^T / dS^T of buffer u written back to TMEM
-  uint64_t* acc_done = bars + 13;   // 1
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 14);
 
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const int b = blockIdx.z;
@@ -516,27 +344,22 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
   const int nc = chi - clo;
   const int T = DKV ? g * nc : nc;  // streamed half-tiles processed by this CTA
 
-  if (warp == 16 && elect_one()) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_r1);
     tma_prefetch_desc(&tmap_r2);
     tma_prefetch_desc(&tmap_s1);
     tma_prefetch_desc(&tmap_s2);
     mbar_init(r_full, 1);
-    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&st_full[i], DKV ? 2 : 1); mbar_init(&st_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&sp_full[i], 1); mbar_init(&pd_ready[i], 8); }
-    mbar_init(acc_done, 1);
+    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&st_full[i], DKV ? 2 : 1); mbar_init(&st_empty[i], FA_CONSUMERS); }
     fence_barrier_init();
   }
-  if (warp == 17) tmem_alloc<512>(tmem_ptr_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   const float scale_log2 = p.scale * kLog2e;
 
-  if (warp == 16) {
-    // ================= producer: TMA tiles (+ lse / delta vectors in DKV mode) =================
-    if (T > 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    // ================= producer (warp 0): TMA tiles (+ lse / delta vectors in DKV mode) =================
+    if (warp == 0 && T > 0) {
       if (elect_one()) {
         mbar_arrive_expect_tx(r_full, 2 * C::RES_BYTES);
         const int rrow = (DKV ? sq.k_start : sq.q_start) + r0;
@@ -551,7 +374,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
         const int st = t % BWD_NST;
         const int hs = DKV ? head * g + t / nc : hk;   // head of the streamed operand
         const int c0 = (clo + (DKV ? t % nc : t)) * 64;  // first streamed row, sequence-local
-        mbar_wait(&st_empty[st], ((t / BWD_NST) & 1) ^ 1);
+        mbar_wait_wg(&st_empty[st], ((t / BWD_NST) & 1) ^ 1);
         if (elect_one()) {
           mbar_arrive_expect_tx(&st_full[st], 2 * C::STR_BYTES);
           const int srow = (DKV ? sq.q_start : sq.k_start) + c0;
@@ -584,192 +407,134 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
         __syncwarp();
       }
     }
-  } else if (warp == 17) {
-    // ================= MMA issuer =================
-    constexpr uint32_t idesc_sp = make_idesc_bf16(128, 64, false, false);
-    constexpr uint32_t idesc_acc = make_idesc_bf16(128, D, false, true);
-    auto issue_sp = [&](int t) {  // S[u] = R1 s1^T, dP[u] = R2 s2^T
-      const int u = t & 1, st = t % BWD_NST;
-      mbar_wait(&st_full[st], (t / BWD_NST) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a1 = desc_lo(smem_u32(smem_r1), 16), a2 = desc_lo(smem_u32(smem_r2), 16);
-        const uint32_t b1 = desc_lo(smem_u32(smem_s + st * 2 * C::STR_BYTES), 16);
-        const uint32_t b2 = desc_lo(smem_u32(smem_s + st * 2 * C::STR_BYTES + C::STR_BYTES), 16);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_lo(tmem_base + u * 64, a1 + koff_kmajor(128, kk), b1 + koff_kmajor(64, kk), idesc_sp, kk != 0);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_lo(tmem_base + 128 + u * 64, a2 + koff_kmajor(128, kk), b2 + koff_kmajor(64, kk), idesc_sp, kk != 0);
-        umma_commit(&sp_full[u]);
-      }
-      __syncwarp();
-    };
-    auto issue_acc = [&](int t) {  // A operands (bf16 P^T / dS^T) straight from the TMEM columns of buffer u
-      const int u = t & 1, st = t % BWD_NST;
-      mbar_wait(&pd_ready[u], (t >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t b1 = desc_lo(smem_u32(smem_s + st * 2 * C::STR_BYTES), 64 * 128);
-        const uint32_t b2 = desc_lo(smem_u32(smem_s + st * 2 * C::STR_BYTES + C::STR_BYTES), 64 * 128);
-        const uint32_t tp = tmem_base + u * 64, tds = tmem_base + 128 + u * 64;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint32_t aoff = (kk >> 1) * 32 + (kk & 1) * 8;  // packed bf16 columns of streamed rows [16 kk, 16 kk + 16)
-          if constexpr (DKV) {
-            umma_ts_lo(tmem_base + 256, tp + aoff, b2 + koff_mnmajor(kk), idesc_acc, (t | kk) != 0);       // dV += P^T dO
-            umma_ts_lo(tmem_base + 256 + D, tds + aoff, b1 + koff_mnmajor(kk), idesc_acc, (t | kk) != 0);  // dK += dS^T Q
-          } else {
-            umma_ts_lo(tmem_base + 256, tds + aoff, b1 + koff_mnmajor(kk), idesc_acc, (t | kk) != 0);      // dQ += dS K
-          }
-        }
-        umma_commit(&st_empty[st]);
-        if (t == T - 1) umma_commit(acc_done);
-      }
-      __syncwarp();
-    };
-    if (T > 0) {
-      mbar_wait(r_full, 0);
-      issue_sp(0);
-      if (T > 1) issue_sp(1);
-      for (int t = 0; t < T; ++t) {
-        issue_acc(t);                     // reads buffer u = t & 1 ...
-        if (t + 2 < T) issue_sp(t + 2);   // ... which the next S / dP of that buffer overwrites: tcgen05 ops complete in order
-      }
-    }
   } else {
-    // ================= softmax warps: two threads per resident row, 32 streamed columns each =================
-    const int u = warp >> 3;                 // S / dP buffer of this group of 8 warps
-    const int hf = (warp >> 2) & 1;          // column half [hf*32, hf*32+32) of the 64-wide half-tile
-    const int row = (warp & 3) * 32 + lane;
-    const int ri = r0 + row;  // sequence-local key (DKV) / query (DQ) index
-    const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t tmem_s = tmem_base + lane_base + u * 64 + hf * 32;
-    const uint32_t tmem_dp = tmem_s + 128;
+    setmaxnreg_inc<232>();
+    // ================= consumers: 64 resident rows each =================
+    const int cw = (warp >> 2) - 1, wq = warp & 3;
+    const int cq = (lane & 3) * 2;
+    const int row_l = cw * 64 + wq * 16 + (lane >> 2);  // resident rows row_l, row_l + 8 of this thread
+    const bool signal = (wq == 0 && lane == 0);
     const bool capped = p.softcap != 0.f;
     const float cap_in = capped ? p.scale / p.softcap : 0.f;
-    float my_lse2 = INFINITY, my_delta = 0.f;
+    float my_lse2[2] = {INFINITY, INFINITY}, my_delta[2] = {0.f, 0.f};
     if constexpr (!DKV) {
-      if (ri < sq.Sq) {
-        const long long idx = sq.lse_base + static_cast<long long>(head) * p.lse_hs + ri;
-        const float lv = p.lse[idx];
-        my_lse2 = (lv == -INFINITY) ? INFINITY : lv * kLog2e;
-        my_delta = p.delta[idx];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int ri = r0 + row_l + 8 * r;
+        if (ri < sq.Sq) {
+          const long long idx = sq.lse_base + static_cast<long long>(head) * p.lse_hs + ri;
+          const float lv = p.lse[idx];
+          my_lse2[r] = (lv == -INFINITY) ? INFINITY : lv * kLog2e;
+          my_delta[r] = p.delta[idx];
+        }
       }
     }
-    int i = 0;
-    for (int t = u; t < T; t += 2, ++i) {
+    float acc1[D / 2], acc2[D / 2];  // DKV: dV, dK.  DQ: dQ, unused
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) { acc1[i] = 0.f; acc2[i] = 0.f; }
+    const uint32_t r1_addr = smem_u32(smem_r1) + cw * (64 * 128), r2_addr = smem_u32(smem_r2) + cw * (64 * 128);
+    if (T > 0) mbar_wait_wg(r_full, 0);
+    for (int t = 0; t < T; ++t) {
       const int st = t % BWD_NST;
-      const int c0 = (clo + (DKV ? t % nc : t)) * 64 + hf * 32;  // first streamed row of this thread's columns
-      mbar_wait(&sp_full[u], i & 1);
-      tc_fence_after();
-      uint32_t s[32], dp[32];
-      tmem_ld_32x32b_x32(tmem_s, s);
-      tmem_ld_32x32b_x32(tmem_dp, dp);
-      tmem_ld_wait();
-      // visible streamed columns [vlo, vhi] (relative to c0) of this row
-      int vlo, vhi;
-      if constexpr (DKV) {  // row = key ri, column = query c0 + c
-        vlo = p.wr < 0 ? 0 : ri - sq.off - p.wr - c0;
-        vhi = p.wl < 0 ? 31 : ri - sq.off + p.wl - c0;
-      } else {              // row = query ri, column = key c0 + c
-        vlo = p.wl < 0 ? 0 : ri + sq.off - p.wl - c0;
-        vhi = min(sq.Sk - 1, p.wr < 0 ? sq.Sk - 1 : ri + sq.off + p.wr) - c0;
-      }
-      const bool edge = __any_sync(0xffffffffu, vlo > 0 || vhi < 31);
-      const float* vec = smem_vec + st * 128 + hf * 32;
-      if constexpr (DKV) mbar_wait(&st_full[st], (t / BWD_NST) & 1);  // acquire the producer's lse / delta stores
-      uint32_t pk[16], dk[16];
+      const int c0 = (clo + (DKV ? t % nc : t)) * 64;  // first streamed row of this half-tile
+      mbar_wait_wg(&st_full[st], (t / BWD_NST) & 1);
+      const uint32_t s1_addr = smem_u32(smem_s + st * 2 * C::STR_BYTES), s2_addr = s1_addr + C::STR_BYTES;
+      float s[32], dp[32];
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 32; c += 4) {
-        float l2[4], dl[4];
-        if constexpr (DKV) {
-          const float4 a = lds_f4(vec + c), d4 = lds_f4(vec + 64 + c);
-          l2[0] = a.x; l2[1] = a.y; l2[2] = a.z; l2[3] = a.w;
-          dl[0] = d4.x; dl[1] = d4.y; dl[2] = d4.z; dl[3] = d4.w;
-        } else {
+      for (int kk = 0; kk < D / 16; ++kk)
+        wgmma_bf16_ss<64, 0, 0>(s, desc_kmajor(r1_addr, 128 * 128, kk), desc_kmajor(s1_addr, 64 * 128, kk), kk != 0);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) { l2[e] = my_lse2; dl[e] = my_delta; }
+      for (int kk = 0; kk < D / 16; ++kk)
+        wgmma_bf16_ss<64, 0, 0>(dp, desc_kmajor(r2_addr, 128 * 128, kk), desc_kmajor(s2_addr, 64 * 128, kk), kk != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      wgmma_fence_regs(dp);
+      const float* vec = smem_vec + st * 128;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int ri = r0 + row_l + 8 * r;  // sequence-local key (DKV) / query (DQ) index
+        // visible streamed columns [vlo, vhi] (relative to c0) of this row
+        int vlo, vhi;
+        if constexpr (DKV) {  // row = key ri, column = query c0 + c
+          vlo = p.wr < 0 ? 0 : ri - sq.off - p.wr - c0;
+          vhi = p.wl < 0 ? 63 : ri - sq.off + p.wl - c0;
+        } else {              // row = query ri, column = key c0 + c
+          vlo = p.wl < 0 ? 0 : ri + sq.off - p.wl - c0;
+          vhi = min(sq.Sk - 1, p.wr < 0 ? sq.Sk - 1 : ri + sq.off + p.wr) - c0;
         }
-        float pv[4], dsv[4];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          float x = __uint_as_float(s[c + e]), tcap = 0.f;
-          if (capped) {
-            tcap = tanhf(x * cap_in);
-            x = p.softcap * tcap * kLog2e;
-          } else {
-            x *= scale_log2;
-          }
-          pv[e] = exp2f(x - l2[e]);
-          dsv[e] = pv[e] * (__uint_as_float(dp[c + e]) - dl[e]);
-          if (capped) dsv[e] *= (1.f - tcap * tcap);
-        }
-        pk[c >> 1] = pack_bf16x2(pv[0], pv[1]);
-        pk[(c >> 1) + 1] = pack_bf16x2(pv[2], pv[3]);
-        dk[c >> 1] = pack_bf16x2(dsv[0], dsv[1]);
-        dk[(c >> 1) + 1] = pack_bf16x2(dsv[2], dsv[3]);
-      }
-      if (edge) {  // boundary half-tiles only (warp-uniform): zero the columns outside the window / causal range
+        for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-        for (int c = 0; c < 32; c += 2) {
-          const bool k0v = (c >= vlo) && (c <= vhi), k1v = (c + 1 >= vlo) && (c + 1 <= vhi);
-          const uint32_t keep = (k0v ? 0x0000ffffu : 0u) | (k1v ? 0xffff0000u : 0u);
-          pk[c >> 1] &= keep;
-          dk[c >> 1] &= keep;
-        }
-      }
-      // bf16 results back into the first 16 of this thread's own 32 fp32 columns (nobody else reads or writes them)
-      if constexpr (DKV) tmem_st_32x32b_x16(tmem_s, pk);
-      tmem_st_32x32b_x16(tmem_dp, dk);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&pd_ready[u]);
-    }
-    // ---- epilogue: accumulators -> bf16 -> global.  DKV: group 0 stores dV, group 1 stores dK (scaled); DQ: group 0 stores
-    // dQ (scaled).  The two threads of a row take one half of the D columns each.
-    if (T > 0) {
-      mbar_wait(acc_done, 0);
-      tc_fence_after();
-    }
-    const bool row_ok = ri < (DKV ? sq.Sk : sq.Sq);
-    if (DKV || u == 0) {
-      __nv_bfloat16* dst;
-      if constexpr (DKV) dst = (u == 0 ? p.dv : p.dk) + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * D + hf * (D / 2);
-      else dst = p.dq + (static_cast<long long>(sq.q_start + ri) * p.Hq + head) * D + hf * (D / 2);
-      const float mul = (DKV && u == 0) ? 1.f : p.scale;
-      const uint32_t tacc = tmem_base + lane_base + 256 + (DKV ? u * D : 0) + hf * (D / 2);
-#pragma unroll
-      for (int c = 0; c < D / 64; ++c) {
-        uint32_t o[32];
-        if (T > 0) {
-          tmem_ld_32x32b_x32(tacc + c * 32, o);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) o[e] = 0;
-        }
-        if (row_ok) {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 w4;
-            w4.x = pack_bf16x2(__uint_as_float(o[v * 8 + 0]) * mul, __uint_as_float(o[v * 8 + 1]) * mul);
-            w4.y = pack_bf16x2(__uint_as_float(o[v * 8 + 2]) * mul, __uint_as_float(o[v * 8 + 3]) * mul);
-            w4.z = pack_bf16x2(__uint_as_float(o[v * 8 + 4]) * mul, __uint_as_float(o[v * 8 + 5]) * mul);
-            w4.w = pack_bf16x2(__uint_as_float(o[v * 8 + 6]) * mul, __uint_as_float(o[v * 8 + 7]) * mul);
-            *reinterpret_cast<uint4*>(dst + c * 32 + v * 8) = w4;
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * jj + cq + e;
+            const int i = 4 * jj + 2 * r + e;
+            float l2, dl;
+            if constexpr (DKV) { l2 = vec[c]; dl = vec[64 + c]; }
+            else { l2 = my_lse2[r]; dl = my_delta[r]; }
+            float x = s[i], tcap = 0.f;
+            if (capped) {
+              tcap = tanhf(x * cap_in);
+              x = p.softcap * tcap * kLog2e;
+            } else {
+              x *= scale_log2;
+            }
+            float pv = exp2f(x - l2);
+            float dsv = pv * (dp[i] - dl);
+            if (capped) dsv *= (1.f - tcap * tcap);
+            const bool vis = (c >= vlo) && (c <= vhi);
+            s[i] = vis ? pv : 0.f;
+            dp[i] = vis ? dsv : 0.f;
           }
         }
       }
+      uint32_t pf[4][4], df[4][4];
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        pack_a_frag(s, ks, pf[ks]);
+        pack_a_frag(dp, ks, df[ks]);
+      }
+      wgmma_fence_regs(acc1);
+      if constexpr (DKV) wgmma_fence_regs(acc2);
+      wgmma_fence();
+      if constexpr (DKV) {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc1, pf[ks], desc_mnmajor(s2_addr, 64 * 128, ks), 1);  // dV += P^T dO
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc2, df[ks], desc_mnmajor(s1_addr, 64 * 128, ks), 1);  // dK += dS^T Q
+      } else {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc1, df[ks], desc_mnmajor(s1_addr, 64 * 128, ks), 1);  // dQ += dS K
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc1);
+      if constexpr (DKV) wgmma_fence_regs(acc2);
+      if (signal) mbar_arrive(&st_empty[st]);
     }
-    tc_fence_before();
+    // ---- epilogue: accumulators -> bf16 -> global.  DKV: dV, dK (scaled); DQ: dQ (scaled)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int ri = r0 + row_l + 8 * r;
+      if (ri >= (DKV ? sq.Sk : sq.Sq)) continue;
+      if constexpr (DKV) {
+        __nv_bfloat16* dv = p.dv + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * D + cq;
+        __nv_bfloat16* dk = p.dk + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * D + cq;
+#pragma unroll
+        for (int jj = 0; jj < D / 8; ++jj) {
+          *reinterpret_cast<uint32_t*>(dv + 8 * jj) = pack_bf16x2(acc1[4 * jj + 2 * r], acc1[4 * jj + 2 * r + 1]);
+          *reinterpret_cast<uint32_t*>(dk + 8 * jj) =
+              pack_bf16x2(acc2[4 * jj + 2 * r] * p.scale, acc2[4 * jj + 2 * r + 1] * p.scale);
+        }
+      } else {
+        __nv_bfloat16* dq = p.dq + (static_cast<long long>(sq.q_start + ri) * p.Hq + head) * D + cq;
+#pragma unroll
+        for (int jj = 0; jj < D / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(dq + 8 * jj) = pack_bf16x2(acc1[4 * jj + 2 * r] * p.scale, acc1[4 * jj + 2 * r + 1] * p.scale);
+      }
+    }
   }
-
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 17) tmem_dealloc<512>(tmem_base);
 }
 
 // delta[b, h, q] = sum_d dO[q, h, d] * O[q, h, d]   (D/8 lanes per (row, head), 16-byte loads)
@@ -846,8 +611,8 @@ void launch_fwd(const FlashAttnArgs& a, cudaStream_t stream) {
   FaParams p = make_params(a);
   p.out = static_cast<__nv_bfloat16*>(a.out);
   p.lse = a.lse;
-  dim3 grid((a.Sq + 255) / 256, a.Hq, a.B);
-  kern<<<grid, FWD_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  dim3 grid((a.Sq + 127) / 128, a.Hq, a.B);
+  kern<<<grid, FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
 }
 
 template <int D>
@@ -877,7 +642,7 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
     const CUtensorMap tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 128), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 128),
                       tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 64), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, D, 64);
     dim3 grid((a.Sk + 127) / 128, a.Hk, a.B);
-    kern<<<grid, BWD_THREADS, C::SMEM_BYTES, stream>>>(tk, tv, tq, tdo, p);
+    kern<<<grid, FA_THREADS, C::SMEM_BYTES, stream>>>(tk, tv, tq, tdo, p);
   }
   {
     using C = BwdCfg<D, false>;
@@ -890,7 +655,7 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
     const CUtensorMap tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 128), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, D, 128),
                       tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 64), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 64);
     dim3 grid((a.Sq + 127) / 128, a.Hq, a.B);
-    kern<<<grid, BWD_THREADS, C::SMEM_BYTES, stream>>>(tq, tdo, tk, tv, p);
+    kern<<<grid, FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tdo, tk, tv, p);
   }
 }
 

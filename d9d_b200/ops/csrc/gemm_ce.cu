@@ -1,4 +1,4 @@
-// Fused linear + cross-entropy on the tcgen05 GEMM (no [T, V] logits tensor in the forward pass).
+// Fused linear + cross-entropy on the wgmma GEMM (no [T, V] logits tensor in the forward pass).
 //   forward : logits tile -> per-(row, n_tile) online-softmax partials + target logit  (EPI_CE_LSE)
 //   finalize: partials -> lse[row], nll[row]
 //   backward: recompute logits tile, write g*(softmax - onehot) as bf16 chunk          (EPI_CE_DLOGITS)

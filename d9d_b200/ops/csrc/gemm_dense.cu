@@ -1,4 +1,4 @@
-// Dense tcgen05 GEMM instantiations (forward NT, dgrad NN-as-MN-major-B, wgrad TN-as-MN/MN).
+// Dense wgmma GEMM instantiations (forward NT, dgrad NN-as-MN-major-B, wgrad TN-as-MN/MN).
 #include <cstdlib>
 
 #include "gemm_host.cuh"
@@ -9,7 +9,7 @@ using namespace gemm;
 namespace {
 int& pair_mode_ref() {
   static int mode = [] {
-    // CTA pairs are the default for eligible shapes (measured: +7..30 % on large dense GEMMs, neutral on the MoE flagship);
+    // CTA pairs (B tile multicast over a two-CTA cluster) are the default for eligible shapes;
     // D9D_GEMM_PAIR=0 restores the single-CTA kernels everywhere
     const char* e = std::getenv("D9D_GEMM_PAIR");
     return (e != nullptr && e[0] == '0') ? 0 : 1;
@@ -25,7 +25,7 @@ int gemm_set_pair_mode(int mode) {
 }
 int gemm_pair_mode() { return pair_mode_ref(); }
 
-// CTA pairs pay off once there are enough 256-row tiles to fill the 74 TPCs; tiny problems keep the single-CTA kernels
+// CTA pairs pay off once there are enough 256-row tiles to fill the 66 SM pairs; tiny problems keep the single-CTA kernels
 bool gemm_pair_eligible(const GemmArgs& a) { return a.M >= 512 && a.N >= 128 && a.comm == 0; }
 
 void gemm_dense(const GemmArgs& a, cudaStream_t stream) {

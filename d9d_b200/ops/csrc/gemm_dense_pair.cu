@@ -1,5 +1,5 @@
-// Dense tcgen05 GEMM on CTA pairs: tcgen05.mma.cta_group::2 over 256 x {256, 128} tiles, one cluster of two CTAs per TPC.
-// Every CTA stages its own 128 rows of A and half of the B tile; the leader CTA issues the MMAs for both.
+// Dense wgmma GEMM on CTA pairs: 256 x {256, 128} tiles, one cluster of two CTAs per tile.
+// Every CTA stages its own 128 rows of A and loads half of the B tile, multicast into both CTAs.
 #include "gemm_host.cuh"
 
 namespace d9d {

@@ -1,11 +1,11 @@
 // fp8 (e4m3) GEMM launchers + the quantisation kernels that produce their operands.
 //   quantize_rowwise     x[M,K] bf16 -> q[M,K] e4m3, scale[M]            (scale = amax / 448 per row)
 //   quantize_colwise_t   x[R,C] bf16 -> qT[C,R] e4m3, scale[C]           (transposed copy, scale per column of x)
-//   quantize_mx          x[M,K] bf16 -> q[M,K] e4m3, UE8M0 scale blocks  (one scale per 32 K-elements, tcgen05 block layout)
-//   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on kind::f8f6f4 / kind::mxf8f6f4.block_scale
+//   quantize_mx          x[M,K] bf16 -> q[M,K] e4m3, UE8M0 scale blocks  (one scale per 32 K-elements, 128-row x 4-group blocks)
+//   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on wgmma e4m3 (MX: per-32-K scales applied in registers)
 #include <cuda_fp8.h>
 
-#include "gemm_fp8_sm100.cuh"
+#include "gemm_fp8_sm90.cuh"
 #include "gemm_host.cuh"
 
 namespace d9d {
@@ -206,11 +206,11 @@ void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream) {
   if (a.block_scaled) {
     if (a.K % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr)
       throw std::runtime_error("d9d gemm_mxfp8: K must be a multiple of 128 and both scale-factor tensors are required");
-    if (a.N <= 128) launch_fp8<128, fp8::MX>(a, stream);
-    else launch_fp8<256, fp8::MX>(a, stream);
+    launch_fp8<128, fp8::MX>(a, stream);
   } else {
-    if (a.N <= 128) launch_fp8<128, fp8::ROWCOL>(a, stream);
-    else launch_fp8<256, fp8::ROWCOL>(a, stream);
+    // 128-wide tiles only: a 256-wide fp32 accumulator (128 registers per consumer thread) spills at the kernel's
+    // 168-register budget
+    launch_fp8<128, fp8::ROWCOL>(a, stream);
   }
 }
 

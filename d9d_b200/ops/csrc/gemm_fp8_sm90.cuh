@@ -1,0 +1,262 @@
+// d9d_b200 — persistent warp-specialised wgmma GEMM for 8-bit floating point operands (sm_90a).
+//
+//   D[M,N] (bf16) = scale( A[M,K] · B[N,K]^T )       A, B: e4m3, K-major; fp32 accumulation in registers.
+//
+// Two scaling recipes share the mainloop:
+//   ROWCOL  D = acc * scale_a[row] * scale_b[col]  (per-token / per-output-channel or per-tensor scales, applied in the
+//           epilogue)
+//   MX      one UE8M0 scale per 32 K-elements of every row of A and B (OCP MXFP8).  The scale-factor blocks (512 bytes =
+//           128 rows x 4 K-groups per operand tile) are bulk-copied into shared memory next to the A/B tiles; every K=32
+//           wgmma writes a fresh partial product that is added to the accumulator with its row x column scale
+//           (Hopper's tensor core has no block-scaled MMA).
+// Same structure as the bf16 kernel (gemm_sm90.cuh): warpgroup 0 = TMA producer, warpgroups 1-2 = wgmma + epilogue over
+// 64 rows each (registers -> swizzled smem -> TMA store); a stage holds 128 bytes of K (= 128 fp8 elements = 4 MMAs).
+#pragma once
+
+#include "common.cuh"
+
+namespace d9d {
+namespace fp8 {
+
+constexpr int BLOCK_M = 128;
+constexpr int BLOCK_K = 128;  // fp8 elements = bytes = one 128B swizzle row
+constexpr int MMA_K = 32;
+constexpr int NUM_THREADS = 384;
+constexpr int NUM_CONSUMERS = 2;
+constexpr int NUM_EPI_WARPS = 4 * NUM_CONSUMERS;
+constexpr int EPI_BOX_ROWS = 16;
+constexpr int SF_BLOCK_BYTES = 512;  // 128 rows x 4 K-groups of 32 elements
+
+enum Scaling : int { ROWCOL = 0, MX = 1 };
+
+struct Params {
+  int M, N, K;
+  const float* scale_a;  // ROWCOL: [M] or nullptr (=1)
+  const float* scale_b;  // ROWCOL: [N] or nullptr (=1)
+  float scale_scalar;    // ROWCOL: extra scalar factor
+  const uint8_t* sfa;    // MX: [ceil(M/128), K/128, 512] UE8M0 blocks, byte (r%32)*16 + (r/32)*4 + kgroup
+  const uint8_t* sfb;    // MX: [ceil(N/128), K/128, 512]
+};
+
+template <int BLOCK_N, int SCALING>
+struct Cfg {
+  static constexpr bool IS_MX = (SCALING == MX);
+  static_assert(BLOCK_N == 128, "128-wide tiles: wider fp32 accumulators (and MX's second, partial one) spill");
+  static constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K;
+  static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K;
+  static constexpr int SFA_STAGE_BYTES = IS_MX ? SF_BLOCK_BYTES : 0;
+  static constexpr int SFB_BLOCKS = (BLOCK_N + 127) / 128;
+  static constexpr int SFB_STAGE_BYTES = IS_MX ? SFB_BLOCKS * SF_BLOCK_BYTES : 0;
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES + SFA_STAGE_BYTES + SFB_STAGE_BYTES;
+  static constexpr int EPI_BUFS = 2;
+  static constexpr int EPI_STAGING_BYTES = NUM_EPI_WARPS * EPI_BUFS * EPI_BOX_ROWS * 128;
+  static constexpr int SMEM_BUDGET = 227 * 1024 - 2048 - 256 - EPI_STAGING_BYTES;
+  static constexpr int STAGES_RAW = SMEM_BUDGET / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
+  static_assert(STAGES >= 3, "need at least 3 operand stages");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_STAGING_BYTES + 2048 /*two alignments*/ + 256 /*barriers*/;
+};
+
+__device__ __forceinline__ void tile_coord(int tile, int m_tiles, int n_tiles, int& m_blk, int& n_blk) {
+  constexpr int GROUP_M = 8;  // L2-friendly rasterisation (same as the bf16 kernel)
+  const int group_span = GROUP_M * n_tiles;
+  const int gid = tile / group_span;
+  const int first_m = gid * GROUP_M;
+  const int gm = min(m_tiles - first_m, GROUP_M);
+  const int r = tile - gid * group_span;
+  m_blk = first_m + (r % gm);
+  n_blk = r / gm;
+}
+
+__device__ __forceinline__ float ue8m0(uint8_t e) { return __uint_as_float(static_cast<uint32_t>(e) << 23); }
+
+template <int BLOCK_N, int SCALING>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                const __grid_constant__ CUtensorMap tmap_d, const Params p) {
+  using C = Cfg<BLOCK_N, SCALING>;
+  constexpr int STAGES = C::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem_a + STAGES * C::A_STAGE_BYTES;
+  uint8_t* smem_sfa = smem_b + STAGES * C::B_STAGE_BYTES;
+  uint8_t* smem_sfb = smem_sfa + STAGES * C::SFA_STAGE_BYTES;
+  // the swizzled epilogue staging boxes must start on a 1024-byte boundary (the scale-factor regions are 512-byte granular)
+  uint8_t* smem_epi = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(smem_sfb + STAGES * C::SFB_STAGE_BYTES) + 1023) & ~uintptr_t(1023));
+  static_assert((C::A_STAGE_BYTES % 1024) == 0 && (C::B_STAGE_BYTES % 1024) == 0, "operand stages keep the 1024-byte swizzle alignment");
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + C::EPI_STAGING_BYTES);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M, n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
+  const int total_tiles = m_tiles * n_tiles;
+  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int sf_k_blocks = k_blocks;
+
+  if (warp == 0 && elect_one()) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_d);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], NUM_CONSUMERS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ================= TMA producer =================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        tile_coord(tile, m_tiles, n_tiles, m_blk, n_blk);
+        const int m_idx = m_blk * BLOCK_M, n_idx = n_blk * BLOCK_N;
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait_wg(&empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+          tma_load_2d(smem_a + stage * C::A_STAGE_BYTES, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_idx);
+          tma_load_2d(smem_b + stage * C::B_STAGE_BYTES, &tmap_b, &full_bar[stage], kb * BLOCK_K, n_idx);
+          if constexpr (C::IS_MX) {
+            bulk_load_1d(smem_sfa + stage * C::SFA_STAGE_BYTES,
+                         p.sfa + (static_cast<long long>(m_blk) * sf_k_blocks + kb) * SF_BLOCK_BYTES, SF_BLOCK_BYTES, &full_bar[stage]);
+#pragma unroll
+            for (int j = 0; j < C::SFB_BLOCKS; ++j)
+              bulk_load_1d(smem_sfb + stage * C::SFB_STAGE_BYTES + j * SF_BLOCK_BYTES,
+                           p.sfb + (static_cast<long long>(n_blk * C::SFB_BLOCKS + j) * sf_k_blocks + kb) * SF_BLOCK_BYTES,
+                           SF_BLOCK_BYTES, &full_bar[stage]);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ================= consumers: 64 rows each =================
+    setmaxnreg_inc<232>();
+    const int cw = (warp >> 2) - 1;
+    const int wq = warp & 3;
+    const int lane = lane_id();
+    const int cq = (lane & 3) * 2;
+    const int r_loc = cw * 64 + wq * 16 + (lane >> 2);  // tile-local rows r_loc and r_loc + 8 of this thread
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t epi_chunk = 0;
+    float acc[BLOCK_N / 2];
+    auto release = [&](int s) {
+      if (wq == 0 && lane == 0) mbar_arrive(&empty_bar[s]);
+    };
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      int m_blk, n_blk;
+      tile_coord(tile, m_tiles, n_tiles, m_blk, n_blk);
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+      wgmma_fence_regs(acc);
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait_wg(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem_a + stage * C::A_STAGE_BYTES) + cw * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + stage * C::B_STAGE_BYTES);
+        if constexpr (C::IS_MX) {
+          const uint8_t* sfa = smem_sfa + stage * C::SFA_STAGE_BYTES;
+          const uint8_t* sfb = smem_sfb + stage * C::SFB_STAGE_BYTES;
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+            float part[BLOCK_N / 2];
+            wgmma_fence();
+            wgmma_e4m3_ss<BLOCK_N>(part, make_wgmma_desc(a_addr + k * MMA_K, 16, 1024), make_wgmma_desc(b_addr + k * MMA_K, 16, 1024), 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(part);
+            float sa[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = r_loc + 8 * h;
+              sa[h] = ue8m0(sfa[(r % 32) * 16 + (r / 32) * 4 + k]);
+            }
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int n = 8 * j + cq + e;
+                const float sb = ue8m0(sfb[(n / 128) * SF_BLOCK_BYTES + (n % 32) * 16 + ((n % 128) / 32) * 4 + k]);
+                acc[4 * j + e] = fmaf(part[4 * j + e], sa[0] * sb, acc[4 * j + e]);
+                acc[4 * j + 2 + e] = fmaf(part[4 * j + 2 + e], sa[1] * sb, acc[4 * j + 2 + e]);
+              }
+            }
+          }
+          release(stage);
+        } else {
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+            wgmma_e4m3_ss<BLOCK_N>(acc, make_wgmma_desc(a_addr + k * MMA_K, 16, 1024), make_wgmma_desc(b_addr + k * MMA_K, 16, 1024), 1);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0) release(prev);
+          prev = stage;
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      if constexpr (!C::IS_MX) {
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev >= 0) release(prev);
+      }
+
+      const int rbase = m_blk * BLOCK_M + cw * 64 + wq * 16;
+      const int col0 = n_blk * BLOCK_N;
+      if constexpr (!C::IS_MX) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = rbase + (lane >> 2) + 8 * h;
+          float row_scale = p.scale_scalar;
+          if (p.scale_a != nullptr && row < p.M) row_scale *= p.scale_a[row];
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = col0 + 8 * j + cq + e;
+              const float cs = (p.scale_b != nullptr && col < p.N) ? p.scale_b[col] : 1.f;
+              acc[4 * j + 2 * h + e] *= row_scale * cs;
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < BLOCK_N / 64; ++c) {
+        const int cbase = col0 + c * 64;
+        if (cbase >= p.N) break;  // warp-uniform
+        uint8_t* stage_buf = smem_epi + ((cw * 4 + wq) * C::EPI_BUFS + (epi_chunk % C::EPI_BUFS)) * (EPI_BOX_ROWS * 128);
+        ++epi_chunk;
+        if (lane == 0) tma_store_wait_read<C::EPI_BUFS - 1>();
+        __syncwarp();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = (lane >> 2) + 8 * h;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = c * 8 + jj;
+            *reinterpret_cast<uint32_t*>(stage_buf + r * 128 + ((jj ^ (r & 7)) << 4) + (lane & 3) * 4) =
+                pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          }
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          tma_store_3d(&tmap_d, stage_buf, cbase, rbase, 0);
+          tma_store_commit();
+        }
+      }
+    }
+    if (lane == 0) tma_store_wait<0>();
+  }
+}
+
+}  // namespace fp8
+}  // namespace d9d

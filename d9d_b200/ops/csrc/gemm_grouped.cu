@@ -1,4 +1,4 @@
-// Grouped tcgen05 GEMM instantiations for MoE experts:
+// Grouped wgmma GEMM instantiations for MoE experts:
 //   GROUPED_M: Y[r,:] = X[r,:] · W[e(r)]      (forward: B MN-major [E,K,N]; dgrad: B K-major [E,N',K'])
 //   GROUPED_K: dW[e]  = X_e^T · dY_e          (both operands MN-major, reduction over the expert's rows)
 #include "gemm_host.cuh"

@@ -1,4 +1,4 @@
-// Host-side launcher pieces for the tcgen05 GEMM: TMA descriptor encoding + dispatch helpers.
+// Host-side launcher pieces for the wgmma GEMM: TMA descriptor encoding + dispatch helpers.
 #pragma once
 
 #include <mutex>
@@ -6,7 +6,7 @@
 #include <string>
 
 #include "d9d_ops.h"
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 
 namespace d9d {
 namespace gemm {
@@ -46,14 +46,14 @@ inline CUtensorMap make_tmap_bf16_3d(const void* base, uint64_t d0, uint64_t d1,
   return m;
 }
 
-// Output tensor map: [groups, rows, cols] row-major, box = 32 rows x 128 bytes, 128B swizzle (matches the epilogue's
-// staging layout).  Returns false when base / pitches do not meet TMA's 16-byte alignment rules.
+// Output tensor map: [groups, rows, cols] row-major, box = 16 rows x 128 bytes, 128B swizzle (matches the epilogue's
+// per-warp staging layout).  Returns false when base / pitches do not meet TMA's 16-byte alignment rules.
 inline bool make_tmap_out(CUtensorMap* m, void* base, bool bf16, uint64_t cols, uint64_t rows, uint64_t groups,
                           uint64_t row_pitch_elems, uint64_t group_pitch_elems) {
   const uint64_t esz = bf16 ? 2 : 4;
   cuuint64_t dims[3] = {cols, rows, groups};
   cuuint64_t strides[2] = {row_pitch_elems * esz, (groups > 1 ? group_pitch_elems : row_pitch_elems * rows) * esz};
-  cuuint32_t box[3] = {static_cast<cuuint32_t>(128 / esz), 32, 1};
+  cuuint32_t box[3] = {static_cast<cuuint32_t>(128 / esz), EPI_BOX_ROWS, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (strides[0] & 15) != 0 || (strides[1] & 15) != 0) return false;
   CUresult r = get_encode_fn()(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base,
@@ -73,7 +73,7 @@ inline int sm_count() {
   return n;
 }
 
-// number of CTA pairs that can be resident at once (one pair per TPC)
+// number of two-CTA clusters that can be resident at once
 template <typename Kern>
 int max_active_pairs(Kern kern, int smem_bytes) {
   cudaLaunchConfig_t cfg{};
@@ -180,7 +180,7 @@ void launch_one(const GemmArgs& a, cudaStream_t stream) {
   long long tiles = m_tiles * n_tiles * (MODE == GROUPED_K ? a.num_groups : 1) * p.k_splits;
   if (tiles <= 0) return;
   if constexpr (CTAS == 2) {
-    // one CTA pair (cluster of 2 on one TPC) per tile
+    // one CTA pair (cluster of 2) per tile
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(static_cast<unsigned>(2 * (tiles < pairs ? tiles : pairs)));
     cfg.blockDim = dim3(NUM_THREADS);
@@ -232,7 +232,7 @@ inline int pick_block_n(long long m_tiles_x_groups, int N) {
     }                                                                                             \
   } while (0)
 
-// CTA-pair (cta_group::2) variants: 256 x {256, 128} tiles
+// CTA-pair (two-CTA cluster, B multicast) variants: 256 x {256, 128} tiles
 #define D9D_DISPATCH_PAIR_BN(AMN, BMN, EPI, bn, args, stream)                                        \
   do {                                                                                               \
     if ((bn) >= 256) launch_one<DENSE, 256, AMN, BMN, EPI, COMM_NONE, 2>(args, stream);              \

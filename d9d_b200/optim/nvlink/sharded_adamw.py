@@ -199,9 +199,8 @@ class NvlinkShardedAdamW(torch.optim.Optimizer):
         """NVSwitch multicast (``multimem``) path or explicit peer loads/stores (default).
 
         ``multimem.ld_reduce`` / ``multimem.st`` move fewer bytes *into* a GPU, but both phases are bound by what every
-        GPU has to send / receive in total, and measured on B200 the plain peer loads / stores are faster at every
-        size tried (reduce of a 2.73 B-parameter arena: 8.1 vs 16.1 ms on 2 GPUs, 14.2 vs 15.0 ms on 8; update +
-        broadcast 4.3 vs 8.4 ms and 7.2 vs 7.7 ms).  ``D9D_NVLINK_MULTIMEM=1`` selects the multicast path.
+        GPU has to send / receive in total, so the plain peer loads / stores are the default (the two have not been
+        compared on H100).  ``D9D_NVLINK_MULTIMEM=1`` selects the multicast path.
         """
         available = self.param_arena.multicast_ptr != 0 and self.grad_arena.multicast_ptr != 0
         return available and os.environ.get("D9D_NVLINK_MULTIMEM", "0") == "1"

@@ -3,7 +3,7 @@
 Parity: reference ``d9d/optim/stochastic/adamw.py:45-163`` (state layout ``step / exp_avg / exp_avg_sq``, DTensor
 aware state allocation, own CPU generator checkpointed under ``_d9d_generator_state``).
 
-B200 difference: the reference issues one Triton launch *and* one CPU ``randint().item()`` per parameter per step;
+Difference from the reference: the reference issues one Triton launch *and* one CPU ``randint().item()`` per parameter per step;
 here every parameter group is updated by ONE multi-tensor kernel launch with ONE seed draw, the pointer tables live
 on the device and are cached across steps, and an optional device-side ``grad_scale`` scalar lets the caller fold
 ``1/sum(loss_weight)`` and the clipping coefficient into the update (no extra pass over the gradients).

@@ -13,7 +13,7 @@ def pytest_configure(config):
         # the CPU suite runs tiny matmuls: many intra-op threads only add scheduling overhead (and fight with the spawned
         # gloo workers, which use one thread each)
         torch.set_num_threads(min(4, os.cpu_count() or 1))
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "dist: spawns multiple processes (gloo on CPU)")
 
 

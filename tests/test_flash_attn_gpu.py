@@ -1,4 +1,4 @@
-"""Native tcgen05 flash attention (forward + backward) against the fp32 oracle of the same op.
+"""Native wgmma flash attention (forward + backward) against the fp32 oracle of the same op.
 
 Mirrors the reference's coverage of ``flash_attn_func`` / ``flash_attn_varlen_func`` (causal, GQA/MQA, sliding windows,
 learnable sinks with ``dsink``, soft-cap, packed sequences; ``d9d/kernel/flash_attn/function.py``)."""

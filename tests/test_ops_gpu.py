@@ -1,4 +1,4 @@
-"""Numerics of every native sm_100a kernel against a plain PyTorch fp32 reference of the same op."""
+"""Numerics of every native sm_90a kernel against a plain PyTorch fp32 reference of the same op."""
 
 import math
 

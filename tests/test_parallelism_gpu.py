@@ -6,7 +6,7 @@
   batch - ``benchmarks/validate_parallelism_gpu.py`` under ``torchrun`` at the largest world size the box offers;
 * pipeline schedules end to end over NCCL p2p.
 
-Skipped on boxes with fewer than 2 GPUs.  Logs of the runs made on 8 GPUs are kept under ``profiles/``.
+Skipped on boxes with fewer than 2 GPUs.
 """
 
 import os

@@ -1,4 +1,4 @@
-"""FP8 tcgen05 kernels (kind::f8f6f4 with epilogue scales, kind::mxf8f6f4.block_scale) and their quantisers against fp32
+"""FP8 wgmma kernels (e4m3 with epilogue scales, MXFP8 block scales) and their quantisers against fp32
 PyTorch references of the same operations."""
 
 import pytest

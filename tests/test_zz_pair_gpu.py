@@ -1,4 +1,4 @@
-"""CTA-pair (tcgen05 cta_group::2, 256-row tiles) variants of the dense GEMM and of the fused linear-CE GEMMs against fp32
+"""CTA-pair (two-CTA clusters with B multicast, 256-row tiles) variants of the dense GEMM and of the fused linear-CE GEMMs against fp32
 PyTorch references - the same checks the single-CTA kernels pass in ``test_ops_gpu.py``."""
 
 import pytest

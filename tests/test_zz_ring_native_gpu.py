@@ -1,4 +1,4 @@
-"""Ring attention's block plan on the native tcgen05 flash-attention kernels, emulated on ONE GPU: every "rank" walks all
+"""Ring attention's block plan on the native wgmma flash-attention kernels, emulated on ONE GPU: every "rank" walks all
 K/V blocks with the same call plan / merge / gradient routines the distributed ring uses (`kernel/context_parallel/ring.py`),
 and the result is compared with fp32 attention over the whole sequence."""
 

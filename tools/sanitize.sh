@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Run a subset of the GPU kernel tests under NVIDIA compute-sanitizer (needs a B200; one GPU).
+# Run a subset of the GPU kernel tests under NVIDIA compute-sanitizer (needs an H100; one GPU).
 #
 #   tools/sanitize.sh memcheck            # out-of-bounds / misaligned accesses, leaks
 #   tools/sanitize.sh racecheck           # shared-memory hazards between warps (TMA / mbarrier protocols)
