@@ -32,8 +32,18 @@ int epi_for(const Tensor& d, bool accumulate) {
   return accumulate ? 2 : 1;
 }
 
+// block_n: output tile width (0 = the heuristic's choice). Single-CTA dense and grouped kernels are built for 128, 192 and
+// 256; CTA pairs and the fused-communication GEMMs for 128 and 256. Unknown values are rejected, never remapped.
+void check_block_n(int64_t block_n, bool allow_192, const std::string& op) {
+  if (block_n == 0 || block_n == 128 || block_n == 256 || (allow_192 && block_n == 192)) return;
+  throw std::runtime_error(op + ": block_n must be 0, 128, " + (allow_192 ? "192 " : "") + "or 256, got " +
+                           std::to_string(block_n));
+}
+
 // d[M,N] (+)= op(a) · op(b)^T.  a: [M,K] or (a_mn) [K,M];  b: [N,K] or (b_mn) [K,N].  Row strides may be padded.
-void gemm(const Tensor& a, const Tensor& b, Tensor d, bool a_mn, bool b_mn, bool accumulate, int64_t ctas) {
+// ctas: 1 = single CTA, 2 = CTA pair, 0 = process-wide policy.  k_splits (fp32 accumulate only): number of K slices, 0 = heuristic.
+void gemm(const Tensor& a, const Tensor& b, Tensor d, bool a_mn, bool b_mn, bool accumulate, int64_t ctas, int64_t block_n,
+          int64_t k_splits) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && d.is_cuda(), "gemm: CUDA tensors required");
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm: bf16 operands required");
   TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && d.dim() == 2, "gemm: 2-D tensors required");
@@ -50,14 +60,22 @@ void gemm(const Tensor& a, const Tensor& b, Tensor d, bool a_mn, bool b_mn, bool
   g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
   g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(0);
   g.epi = epi_for(d, accumulate);
+  TORCH_CHECK(ctas >= 0 && ctas <= 2, "gemm: ctas must be 0, 1 or 2");
   g.ctas = static_cast<int>(ctas);
+  const bool pair = ctas == 2 || (ctas == 0 && d9d::gemm_pair_mode() == 1 && d9d::gemm_pair_eligible(g));
+  check_block_n(block_n, !pair, pair ? "gemm (CTA pair)" : "gemm");
+  TORCH_CHECK(k_splits >= 0, "gemm: k_splits must be >= 0");
+  TORCH_CHECK(k_splits <= 1 || g.epi == 2, "gemm: k_splits needs an fp32 output with accumulate=True");
+  g.block_n = static_cast<int>(block_n);
+  g.k_splits = static_cast<int>(k_splits);
   d9d::gemm_dense(g, cur_stream());
 }
 
 int64_t gemm_set_pair_mode(int64_t mode) { return d9d::gemm_set_pair_mode(static_cast<int>(mode)); }
 
 // d[R,N] = a[R,K] · W[e(r)];  b: [E,N,K] (b_mn=false) or [E,K,N] (b_mn=true)
-void gemm_grouped_m(const Tensor& a, const Tensor& b, Tensor d, const Tensor& tile_group, bool b_mn, bool accumulate) {
+void gemm_grouped_m(const Tensor& a, const Tensor& b, Tensor d, const Tensor& tile_group, bool b_mn, bool accumulate,
+                    int64_t block_n) {
   CHECK_CUDA_CONTIG(a); CHECK_CUDA_CONTIG(b); CHECK_CUDA_CONTIG(d); CHECK_CUDA_CONTIG(tile_group);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16 && d.scalar_type() == at::kBFloat16);
   TORCH_CHECK(tile_group.scalar_type() == at::kInt && a.size(0) % 128 == 0 && tile_group.numel() == a.size(0) / 128);
@@ -73,11 +91,13 @@ void gemm_grouped_m(const Tensor& a, const Tensor& b, Tensor d, const Tensor& ti
   g.lda = a.stride(0); g.ldb = b.stride(1); g.ldd = d.stride(0);
   g.b_group_stride = b.stride(0);
   g.tile_group = tile_group.data_ptr<int>();
+  check_block_n(block_n, true, "gemm_grouped_m");
+  g.block_n = static_cast<int>(block_n);
   d9d::gemm_grouped(g, cur_stream());
 }
 
 // d[E,M,N] (+)= a[rows_e, M]^T · b[rows_e, N] over each expert's row range group_offsets[e]..[e+1]
-void gemm_grouped_k(const Tensor& a, const Tensor& b, Tensor d, const Tensor& group_offsets, bool accumulate) {
+void gemm_grouped_k(const Tensor& a, const Tensor& b, Tensor d, const Tensor& group_offsets, bool accumulate, int64_t block_n) {
   CHECK_CUDA_CONTIG(a); CHECK_CUDA_CONTIG(b); CHECK_CUDA_CONTIG(d); CHECK_CUDA_CONTIG(group_offsets);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16);
   TORCH_CHECK(group_offsets.scalar_type() == at::kInt && a.size(0) == b.size(0));
@@ -92,6 +112,8 @@ void gemm_grouped_k(const Tensor& a, const Tensor& b, Tensor d, const Tensor& gr
   g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(1); g.d_group_stride = d.stride(0);
   g.group_offsets = group_offsets.data_ptr<int>();
   g.epi = epi_for(d, accumulate);
+  check_block_n(block_n, true, "gemm_grouped_k");
+  g.block_n = static_cast<int>(block_n);
   d9d::gemm_grouped(g, cur_stream());
 }
 
@@ -642,7 +664,7 @@ static std::vector<const void*> to_ptrs(at::IntArrayRef v) {
 
 // d[M,N] = all_gather(a_shards)[M,K] · B ; every peer holds a_shard[rows_local, K] (bf16, leading dim lda)
 void gemm_ag_a(at::IntArrayRef a_peer_ptrs, int64_t rows_local, int64_t lda, int64_t block_rows, const Tensor& b, Tensor d,
-               bool b_mn) {
+               bool b_mn, int64_t block_n) {
   TORCH_CHECK(b.is_cuda() && d.is_cuda() && b.dim() == 2 && d.dim() == 2 && b.stride(1) == 1 && d.stride(1) == 1);
   TORCH_CHECK(b.scalar_type() == at::kBFloat16 && d.scalar_type() == at::kBFloat16);
   c10::cuda::CUDAGuard guard(d.device());
@@ -656,13 +678,15 @@ void gemm_ag_a(at::IntArrayRef a_peer_ptrs, int64_t rows_local, int64_t lda, int
   g.B = b.data_ptr(); g.D = d.data_ptr(); g.ldb = b.stride(0); g.ldd = d.stride(0);
   g.comm = 1; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_peer_ptrs = ptrs.data(); g.comm_rows_local = rows_local; g.comm_ld = lda;
+  check_block_n(block_n, false, "gemm_ag_a");
+  g.block_n = static_cast<int>(block_n);
   d9d::gemm_comm(g, cur_stream());
 }
 
 // d[M,N] = a[M,K] · B where a is a local buffer whose shards (owner(row) per the block mapping) arrive asynchronously:
 // the GEMM starts with this rank's shard and waits on flags[owner] (int32, non-zero = landed) before touching another one
 void gemm_wait_a(const Tensor& a, const Tensor& flags, int64_t rank, int64_t block_rows, const Tensor& b, Tensor d, bool b_mn,
-                 int64_t spare_sms) {
+                 int64_t spare_sms, int64_t block_n) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && d.is_cuda() && a.dim() == 2 && b.dim() == 2 && d.dim() == 2);
   TORCH_CHECK(a.stride(1) == 1 && b.stride(1) == 1 && d.stride(1) == 1);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16 && d.scalar_type() == at::kBFloat16);
@@ -678,12 +702,14 @@ void gemm_wait_a(const Tensor& a, const Tensor& flags, int64_t rank, int64_t blo
   g.comm = 5; g.comm_world = static_cast<int>(flags.numel()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_rank = static_cast<int>(rank); g.comm_flags = flags.data_ptr<int>();
   g.comm_spare_sms = static_cast<int>(spare_sms);
+  check_block_n(block_n, false, "gemm_wait_a");
+  g.block_n = static_cast<int>(block_n);
   d9d::gemm_comm(g, cur_stream());
 }
 
 // d_shards[owner][rows_local, N] += (a[M,K] · B) rows owned by `owner` (bf16 reduce-add over NVLink)
 void gemm_rs_d(const Tensor& a, const Tensor& b, at::IntArrayRef d_peer_ptrs, int64_t rows_local, int64_t ldd, int64_t block_rows,
-               bool b_mn) {
+               bool b_mn, int64_t block_n) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && a.dim() == 2 && b.dim() == 2 && a.stride(1) == 1 && b.stride(1) == 1);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16);
   c10::cuda::CUDAGuard guard(a.device());
@@ -697,12 +723,14 @@ void gemm_rs_d(const Tensor& a, const Tensor& b, at::IntArrayRef d_peer_ptrs, in
   g.A = a.data_ptr(); g.B = b.data_ptr(); g.lda = a.stride(0); g.ldb = b.stride(0);
   g.comm = 2; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_peer_ptrs = ptrs.data(); g.comm_rows_local = rows_local; g.comm_ld = ldd;
+  check_block_n(block_n, false, "gemm_rs_d");
+  g.block_n = static_cast<int>(block_n);
   d9d::gemm_comm(g, cur_stream());
 }
 
 // d[M,N] (+)= A^T · B over the token dim where one operand ([tokens, M] or [tokens, N], MN-major) is sharded by tokens
 void gemm_ag_k(const Tensor& local, at::IntArrayRef peer_ptrs, bool peer_is_a, int64_t rows_local, int64_t peer_ld,
-               int64_t block_rows, Tensor d, bool accumulate) {
+               int64_t block_rows, Tensor d, bool accumulate, int64_t block_n, int64_t k_splits) {
   TORCH_CHECK(local.is_cuda() && d.is_cuda() && local.dim() == 2 && d.dim() == 2 && local.stride(1) == 1 && d.stride(1) == 1);
   TORCH_CHECK(local.scalar_type() == at::kBFloat16);
   c10::cuda::CUDAGuard guard(d.device());
@@ -718,6 +746,11 @@ void gemm_ag_k(const Tensor& local, at::IntArrayRef peer_ptrs, bool peer_is_a, i
   g.epi = epi_for(d, accumulate);
   g.comm = peer_is_a ? 3 : 4; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_peer_ptrs = ptrs.data(); g.comm_rows_local = rows_local; g.comm_ld = peer_ld;
+  check_block_n(block_n, false, "gemm_ag_k");
+  TORCH_CHECK(k_splits >= 0, "gemm_ag_k: k_splits must be >= 0");
+  TORCH_CHECK(k_splits <= 1 || g.epi == 2, "gemm_ag_k: k_splits needs an fp32 output with accumulate=True");
+  g.block_n = static_cast<int>(block_n);
+  g.k_splits = static_cast<int>(k_splits);
   d9d::gemm_comm(g, cur_stream());
 }
 
@@ -787,10 +820,10 @@ void nvl_adamw_shard_(Tensor own_param, const Tensor& own_grad, Tensor exp_avg, 
 }
 
 TORCH_LIBRARY(d9d_b200, m) {
-  m.def("gemm(Tensor a, Tensor b, Tensor(a!) d, bool a_mn, bool b_mn, bool accumulate, int ctas=0) -> ()");
+  m.def("gemm(Tensor a, Tensor b, Tensor(a!) d, bool a_mn, bool b_mn, bool accumulate, int ctas=0, int block_n=0, int k_splits=0) -> ()");
   m.def("gemm_set_pair_mode(int mode) -> int", &gemm_set_pair_mode);
-  m.def("gemm_grouped_m(Tensor a, Tensor b, Tensor(a!) d, Tensor tile_group, bool b_mn, bool accumulate=False) -> ()");
-  m.def("gemm_grouped_k(Tensor a, Tensor b, Tensor(a!) d, Tensor group_offsets, bool accumulate) -> ()");
+  m.def("gemm_grouped_m(Tensor a, Tensor b, Tensor(a!) d, Tensor tile_group, bool b_mn, bool accumulate=False, int block_n=0) -> ()");
+  m.def("gemm_grouped_k(Tensor a, Tensor b, Tensor(a!) d, Tensor group_offsets, bool accumulate, int block_n=0) -> ()");
   m.def("ce_forward(Tensor h, Tensor w, Tensor target, int ignore_index) -> (Tensor, Tensor)");
   m.def("ce_forward_ex(Tensor h, Tensor w, Tensor target, int ignore_index, Tensor? bias=None, float softcap=0.0, int col_offset=0) -> (Tensor, Tensor, Tensor)");
   m.def("ce_dlogits(Tensor h, Tensor w, Tensor target, Tensor lse, Tensor grad, Tensor(a!) out, int ignore_index, Tensor? bias=None, float softcap=0.0, int col_offset=0) -> ()");
@@ -823,11 +856,12 @@ TORCH_LIBRARY(d9d_b200, m) {
         "Tensor inv_rms, bool zero_centered, int style) -> (Tensor, Tensor, Tensor, Tensor)");
   m.def("router_topk_fwd(Tensor logits, Tensor? bias, int k, bool renorm) -> (Tensor, Tensor)");
   m.def("router_topk_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm) -> Tensor");
-  m.def("gemm_ag_a(int[] a_peer_ptrs, int rows_local, int lda, int block_rows, Tensor b, Tensor(a!) d, bool b_mn) -> ()");
-  m.def("gemm_wait_a(Tensor a, Tensor flags, int rank, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int spare_sms=0) -> ()");
-  m.def("gemm_rs_d(Tensor a, Tensor b, int[] d_peer_ptrs, int rows_local, int ldd, int block_rows, bool b_mn) -> ()");
+  m.def("gemm_ag_a(int[] a_peer_ptrs, int rows_local, int lda, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int block_n=0) -> ()");
+  m.def("gemm_wait_a(Tensor a, Tensor flags, int rank, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int spare_sms=0, "
+        "int block_n=0) -> ()");
+  m.def("gemm_rs_d(Tensor a, Tensor b, int[] d_peer_ptrs, int rows_local, int ldd, int block_rows, bool b_mn, int block_n=0) -> ()");
   m.def("gemm_ag_k(Tensor local, int[] peer_ptrs, bool peer_is_a, int rows_local, int peer_ld, int block_rows, Tensor(a!) d, "
-        "bool accumulate) -> ()");
+        "bool accumulate, int block_n=0, int k_splits=0) -> ()");
   m.def("ep_push(Tensor x, Tensor? probs, Tensor dest_rank, Tensor dest_row, int peer_ptrs_dev, int off_x, int off_p, int k) -> ()");
   m.def("ep_pull_sum(int peer_ptrs_dev, int off_y, int off_dp, Tensor dest_rank, Tensor dest_row, int T, int k, int H, bool with_dprobs) "
         "-> (Tensor, Tensor)");

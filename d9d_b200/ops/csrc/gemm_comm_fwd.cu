@@ -11,6 +11,7 @@ void gemm_comm_wgrad(const GemmArgs& a, cudaStream_t stream);
 template <int COMM, int EPI>
 static void dispatch_layout(const GemmArgs& a, int bn, cudaStream_t stream) {
   if (a.a_mn) throw std::runtime_error("d9d gemm_comm: K-major A required");
+  if (bn != 128 && bn != 256) throw std::runtime_error("d9d gemm_comm: BLOCK_N must be 128 or 256");
   if (!a.b_mn) {
     if (bn == 256) launch_one<DENSE, 256, false, false, EPI, COMM>(a, stream);
     else launch_one<DENSE, 128, false, false, EPI, COMM>(a, stream);
@@ -23,8 +24,11 @@ static void dispatch_layout(const GemmArgs& a, int bn, cudaStream_t stream) {
 void gemm_comm(const GemmArgs& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0) return;
   const long long m_tiles = (a.M + BLOCK_M - 1) / BLOCK_M;
-  int bn = a.block_n ? a.block_n : pick_block_n(m_tiles, a.N);
-  if (bn == 192) bn = 256;
+  int bn = a.block_n;
+  if (bn == 0) {
+    bn = pick_block_n(m_tiles, a.N);
+    if (bn == 192) bn = 256;  // the fused-communication GEMMs are built for 128- and 256-wide tiles only
+  }
   switch (a.comm) {
     case COMM_AG_A:
       if (a.epi != EPI_BF16) throw std::runtime_error("d9d gemm_comm: all-gather GEMM stores bf16");

@@ -12,6 +12,7 @@ static void dispatch_epi(const GemmArgs& a, int bn, cudaStream_t stream) {
     if (bn == 256) launch_one<DENSE, 256, true, true, EPI, COMM>(a, stream);  \
     else launch_one<DENSE, 128, true, true, EPI, COMM>(a, stream);            \
   } while (0)
+  if (bn != 128 && bn != 256) throw std::runtime_error("d9d gemm_comm: BLOCK_N must be 128 or 256");
   switch (a.epi) {
     case EPI_F32_ACC: D9D_COMM_W(EPI_F32_ACC); break;
     case EPI_F32: D9D_COMM_W(EPI_F32); break;
@@ -24,8 +25,11 @@ static void dispatch_epi(const GemmArgs& a, int bn, cudaStream_t stream) {
 void gemm_comm_wgrad(const GemmArgs& a, cudaStream_t stream) {
   if (!a.a_mn || !a.b_mn) throw std::runtime_error("d9d gemm_comm: wgrad needs MN-major operands");
   const long long m_tiles = (a.M + BLOCK_M - 1) / BLOCK_M;
-  int bn = a.block_n ? a.block_n : pick_block_n(m_tiles, a.N);
-  if (bn == 192) bn = 256;
+  int bn = a.block_n;
+  if (bn == 0) {
+    bn = pick_block_n(m_tiles, a.N);
+    if (bn == 192) bn = 256;
+  }
   if (a.comm == COMM_AG_KA) dispatch_epi<COMM_AG_KA>(a, bn, stream);
   else dispatch_epi<COMM_AG_KB>(a, bn, stream);
 }

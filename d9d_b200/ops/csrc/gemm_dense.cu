@@ -29,6 +29,9 @@ int gemm_pair_mode() { return pair_mode_ref(); }
 bool gemm_pair_eligible(const GemmArgs& a) { return a.M >= 512 && a.N >= 128 && a.comm == 0; }
 
 void gemm_dense(const GemmArgs& a, cudaStream_t stream) {
+  // MN-major A with K-major B has store epilogues only, whichever kernel (single CTA or pair) the shape would pick
+  if (a.a_mn && !a.b_mn && (a.epi == EPI_F32_ACC || a.epi == EPI_BF16_ACC))
+    throw std::runtime_error("d9d gemm: accumulate epilogue not built for an MN-major A with a K-major B");
   if (a.M <= 0 || a.N <= 0) return;
   if (a.ctas == 2 || (a.ctas == 0 && gemm_pair_mode() == 1 && gemm_pair_eligible(a))) {
     gemm_dense_pair(a, stream);

@@ -47,7 +47,9 @@ inline CUtensorMap make_tmap_bf16_3d(const void* base, uint64_t d0, uint64_t d1,
 }
 
 // Output tensor map: [groups, rows, cols] row-major, box = 16 rows x 128 bytes, 128B swizzle (matches the epilogue's
-// per-warp staging layout).  Returns false when base / pitches do not meet TMA's 16-byte alignment rules.
+// per-warp staging layout).  Returns false when base / pitches do not meet TMA's 16-byte alignment rules, and when a row is
+// not a whole number of 16-byte chunks: the swizzled TMA store clips a row at 16-byte granularity, so it would write
+// past column `cols` into the row padding.
 inline bool make_tmap_out(CUtensorMap* m, void* base, bool bf16, uint64_t cols, uint64_t rows, uint64_t groups,
                           uint64_t row_pitch_elems, uint64_t group_pitch_elems) {
   const uint64_t esz = bf16 ? 2 : 4;
@@ -55,7 +57,8 @@ inline bool make_tmap_out(CUtensorMap* m, void* base, bool bf16, uint64_t cols, 
   cuuint64_t strides[2] = {row_pitch_elems * esz, (groups > 1 ? group_pitch_elems : row_pitch_elems * rows) * esz};
   cuuint32_t box[3] = {static_cast<cuuint32_t>(128 / esz), EPI_BOX_ROWS, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (strides[0] & 15) != 0 || (strides[1] & 15) != 0) return false;
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (strides[0] & 15) != 0 || (strides[1] & 15) != 0 || ((cols * esz) & 15) != 0)
+    return false;
   CUresult r = get_encode_fn()(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base,
                                dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -155,14 +158,21 @@ void launch_one(const GemmArgs& a, cudaStream_t stream) {
     p.tma_epilogue = make_tmap_out(&td, a.D, out_bf16, a.N, a.M, groups, a.ldd, a.d_group_stride) ? 1 : 0;
   }
   p.k_splits = 1;
-  if (MODE == DENSE && EPI == EPI_F32_ACC && p.tma_epilogue) {
-    // split-K: reduce-adds from several CTAs land on the same tile (fp32 adds in L2; order is not deterministic)
-    const long long mn_tiles = ((a.M + C::TILE_M - 1) / C::TILE_M) * ((a.N + BLOCK_N - 1) / BLOCK_N);
-    const long long k_blocks = (a.K + BLOCK_K - 1) / BLOCK_K;
-    long long splits = a.k_splits > 0 ? a.k_splits : (sm_count() / CTAS) / mn_tiles;
-    const long long max_splits = k_blocks / 8;  // keep >= 8 k-blocks (512 deep) per slice
-    if (splits > max_splits) splits = max_splits;
-    if (splits < 1) splits = 1;
+  const bool can_split = MODE == DENSE && EPI == EPI_F32_ACC && p.tma_epilogue;
+  if (a.k_splits > 1 && !can_split)
+    throw std::runtime_error("d9d gemm: split-K needs a dense fp32-accumulate GEMM whose output TMA can address");
+  if (can_split) {
+    // split-K: reduce-adds from several CTAs land on the same tile (fp32 adds in L2; order is not deterministic).
+    // A forced count is honoured exactly: slices past the last k-block are empty and add nothing.
+    long long splits = a.k_splits;
+    if (splits == 0) {
+      const long long mn_tiles = ((a.M + C::TILE_M - 1) / C::TILE_M) * ((a.N + BLOCK_N - 1) / BLOCK_N);
+      const long long k_blocks = (a.K + BLOCK_K - 1) / BLOCK_K;
+      splits = (sm_count() / CTAS) / mn_tiles;
+      const long long max_splits = k_blocks / 8;  // keep >= 8 k-blocks (512 deep) per slice
+      if (splits > max_splits) splits = max_splits;
+      if (splits < 1) splits = 1;
+    }
     p.k_splits = static_cast<int>(splits);
   }
   p.M = a.M; p.N = a.N; p.K = a.K; p.num_groups = a.num_groups;
@@ -218,7 +228,8 @@ inline int pick_block_n(long long m_tiles_x_groups, int N) {
   do {                                                                             \
     if ((bn) == 256) launch_one<MODE, 256, AMN, BMN, EPI>(args, stream);           \
     else if ((bn) == 192) launch_one<MODE, 192, AMN, BMN, EPI>(args, stream);      \
-    else launch_one<MODE, 128, AMN, BMN, EPI>(args, stream);                       \
+    else if ((bn) == 128) launch_one<MODE, 128, AMN, BMN, EPI>(args, stream);      \
+    else throw std::runtime_error("d9d gemm: BLOCK_N must be 128, 192 or 256");   \
   } while (0)
 
 #define D9D_DISPATCH_EPI4(MODE, AMN, BMN, epi, bn, args, stream)                                  \
@@ -235,8 +246,9 @@ inline int pick_block_n(long long m_tiles_x_groups, int N) {
 // CTA-pair (two-CTA cluster, B multicast) variants: 256 x {256, 128} tiles
 #define D9D_DISPATCH_PAIR_BN(AMN, BMN, EPI, bn, args, stream)                                        \
   do {                                                                                               \
-    if ((bn) >= 256) launch_one<DENSE, 256, AMN, BMN, EPI, COMM_NONE, 2>(args, stream);              \
-    else launch_one<DENSE, 128, AMN, BMN, EPI, COMM_NONE, 2>(args, stream);                          \
+    if ((bn) == 256) launch_one<DENSE, 256, AMN, BMN, EPI, COMM_NONE, 2>(args, stream);              \
+    else if ((bn) == 128) launch_one<DENSE, 128, AMN, BMN, EPI, COMM_NONE, 2>(args, stream);         \
+    else throw std::runtime_error("d9d gemm: CTA-pair BLOCK_N must be 128 or 256");                 \
   } while (0)
 
 #define D9D_DISPATCH_PAIR_EPI4(AMN, BMN, epi, bn, args, stream)                                      \

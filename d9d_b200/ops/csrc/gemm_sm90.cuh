@@ -38,7 +38,8 @@ enum Epi : int {
   EPI_BF16 = 0,       // D(bf16) = acc
   EPI_F32 = 1,        // D(f32) = acc
   EPI_F32_ACC = 2,    // D(f32) += acc
-  EPI_BF16_ACC = 3,   // D(bf16) += acc   (fp32 add, rn)
+  EPI_BF16_ACC = 3,   // D(bf16) += acc   TMA path: rn(D + rn_bf16(acc)), the add done in bf16 in L2;
+                      //                  direct-store path: rn(D + acc) with the add in fp32
   EPI_CE_LSE = 4,     // fused linear-CE forward: per (row, n_tile) running max / sum-exp / target logit
   EPI_CE_DLOGITS = 5  // fused linear-CE backward: D(bf16) = g[row] * (exp(acc - lse[row]) - [col == target[row]])
 };
