@@ -55,8 +55,10 @@ class _NativeFlashAttention(torch.autograd.Function):
         dsink = None
         if sink is not None and ctx.needs_input_grad[3]:
             # out_i = sum_j e^{a_ij} v_j / (L_i + e^s):  d/ds = -sum_{b,i} e^{s_h - lse} * (dout . out - dlse)
+            # packed rows outside every sequence have lse = -inf and take no part
             sink_col = sink.float()[:, None] if lse.dim() == 2 else sink.float()[None, :, None]
-            dsink = -(torch.exp(sink_col - lse) * delta).sum(dim=1 if lse.dim() == 2 else (0, 2)).to(sink.dtype)
+            p_sink = torch.where(lse == -math.inf, 0.0, torch.exp(sink_col - lse))
+            dsink = -(p_sink * delta).sum(dim=1 if lse.dim() == 2 else (0, 2)).to(sink.dtype)
         return dq, dk, dv, dsink, None, None, None, None, None, None, None, None
 
 

@@ -164,6 +164,8 @@ void scale_inplace(void* x, long long n, int dtype, const float* scale, cudaStre
 // Sk = maximum sequence lengths).  lse / delta: fp32 [B, Hq, Sq] (packed: [Hq, total_q]).
 // window: key k is visible to query q iff q + (Sk - Sq) - window_left <= k <= q + (Sk - Sq) + window_right (-1 = unbounded;
 // causal = window_right 0).  softcap 0 = off.  sink: per-head logit joining the softmax denominator (or nullptr).
+// Packed rows outside every sequence (before cu_q[0] / cu_k[0] or from cu_q[B] / cu_k[B] on) come back with out = dq = dk =
+// dv = 0 and lse = -inf.  A query without a visible key gets out = 0, dq = 0 and lse = -inf (with a sink: lse = sink).
 struct FlashAttnArgs {
   const void *q, *k, *v;
   void* out;            // forward: written; backward: read
@@ -178,8 +180,8 @@ struct FlashAttnArgs {
   int window_left, window_right;
   float scale, softcap;
 };
-// variant: reserved (the forward hands P to the PV GEMM through swizzled shared memory; the backward kernels read P^T / dS^T
-// as the A operand straight from tensor memory)
+// variant: reserved and ignored (there is one forward: P stays in registers as the A operand of the PV wgmma, as P^T / dS^T
+// do in the backward kernels)
 void flash_attn_fwd(const FlashAttnArgs& a, int variant, cudaStream_t stream);
 // backward = delta pre-pass (delta[b,h,q] = sum_d dO*O, written to a.delta) followed by the dK/dV and dQ kernels (which read
 // a.delta; the caller may subtract d(lse) from it in between)

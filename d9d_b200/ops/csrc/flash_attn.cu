@@ -62,6 +62,35 @@ __device__ __forceinline__ SeqInfo resolve_seq(const FaParams& p, int b) {
   return s;
 }
 
+// The grid is one-dimensional (gridDim.z would cap a packed batch at 65535 sequences):
+//   blockIdx.x = tile + tiles * (head + H * b), the dispatch order of a (tiles, H, B) grid
+struct TileIdx {
+  int tile, head, b;
+};
+__device__ __forceinline__ TileIdx decode_block(int tiles, int H) {
+  const int x = static_cast<int>(blockIdx.x), th = tiles * H;
+  TileIdx t;
+  t.b = x / th;
+  t.head = (x - t.b * th) / tiles;
+  t.tile = x - t.b * th - t.head * tiles;
+  return t;
+}
+
+// A streamed tile that runs past the end of its sequence holds rows of the next sequence, batch element or padding.  Masking
+// zeroes their P / dS, but 0 * NaN = NaN on the tensor core, so the rows themselves must be zero.  The producer warp lands
+// such a tile on a separate barrier, zeroes rows [r_from, box_rows) of its `nbox` [box_rows x 128 B] boxes with this
+// function and only then arrives on the consumers' full barrier; whole tiles take the plain TMA path.  The 128B swizzle only
+// permutes the 16-byte chunks inside a row: whole rows need no un-swizzling.
+__device__ __forceinline__ void zero_tile_rows(uint8_t* tile, int box_rows, int nbox, int r_from, int lane) {
+  const int n = (box_rows - r_from) * 8;
+  for (int bx = 0; bx < nbox; ++bx) {
+    uint8_t* base = tile + bx * box_rows * 128 + r_from * 128;
+    for (int i = lane; i < n; i += 32) *reinterpret_cast<uint4*>(base + i * 16) = make_uint4(0u, 0u, 0u, 0u);
+  }
+  fence_proxy_async_smem();  // generic-proxy zeros before the wgmma (async proxy) reads
+  __syncwarp();
+}
+
 // ======================================================================================================
 // forward
 // ======================================================================================================
@@ -114,12 +143,15 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   uint64_t* k_empty = bars + 3;   // [2]
   uint64_t* v_full = bars + 5;    // [2]
   uint64_t* v_empty = bars + 7;   // [2]
+  uint64_t* v_land = bars + 9;    // 1: the partial last V tile, zeroed past Sk before v_full
 
   const int warp = threadIdx.x >> 5, lane = lane_id();
-  const int h = blockIdx.y, b = blockIdx.z;
+  const int tiles = (p.Sq + 127) / 128;
+  const TileIdx bi = decode_block(tiles, p.Hq);
+  const int h = bi.head, b = bi.b;
   const int hk = h / (p.Hq / p.Hk);
   const SeqInfo sq = resolve_seq(p, b);
-  const int q0 = (gridDim.x - 1 - blockIdx.x) * 128;  // heavy (late) query tiles first
+  const int q0 = (tiles - 1 - bi.tile) * 128;  // heavy (late) query tiles first
   if (q0 >= sq.Sq) return;  // whole CTA exits together (varlen: shorter sequences)
 
   // kv tile range [jbeg, jend) of the query rows [q0, qb]
@@ -133,6 +165,7 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
     mbar_init(bar_q, 1);
+    mbar_init(v_land, 1);
     for (int i = 0; i < C::NSLOT; ++i) {
       mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], FA_CONSUMERS);
       mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], FA_CONSUMERS);
@@ -146,24 +179,37 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     setmaxnreg_dec<40>();
     // a tile without visible keys loads nothing: its consumers never wait on bar_q, and no copy may still be landing in
     // shared memory when the CTA exits
-    if (warp == 0 && jend > jbeg && elect_one()) {
-      mbar_arrive_expect_tx(bar_q, C::TILE_BYTES);
-#pragma unroll
-      for (int dc = 0; dc < D / 64; ++dc)
-        tma_load_3d(smem_q + dc * (128 * 128), &tmap_q, bar_q, dc * 64, h, sq.q_start + q0);
-      for (int j = jbeg; j < jend; ++j) {
-        const int n = j - jbeg, slot = n % C::NSLOT;
-        const uint32_t ph = (n / C::NSLOT) & 1;
-        mbar_wait_wg(&k_empty[slot], ph ^ 1);
-        mbar_arrive_expect_tx(&k_full[slot], C::TILE_BYTES);
+    // shared memory when the CTA exits.  Only the last key tile can run past Sk: its V rows there are zeroed (K rows past
+    // Sk only reach masked scores)
+    if (warp == 0 && jend > jbeg) {
+      if (elect_one()) {
+        mbar_arrive_expect_tx(bar_q, C::TILE_BYTES);
 #pragma unroll
         for (int dc = 0; dc < D / 64; ++dc)
-          tma_load_3d(smem_k + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_k, &k_full[slot], dc * 64, hk, sq.k_start + j * 128);
-        mbar_wait_wg(&v_empty[slot], ph ^ 1);
-        mbar_arrive_expect_tx(&v_full[slot], C::TILE_BYTES);
+          tma_load_3d(smem_q + dc * (128 * 128), &tmap_q, bar_q, dc * 64, h, sq.q_start + q0);
+        for (int j = jbeg; j < jend; ++j) {
+          const int n = j - jbeg, slot = n % C::NSLOT;
+          const uint32_t ph = (n / C::NSLOT) & 1;
+          mbar_wait_wg(&k_empty[slot], ph ^ 1);
+          mbar_arrive_expect_tx(&k_full[slot], C::TILE_BYTES);
 #pragma unroll
-        for (int dc = 0; dc < D / 64; ++dc)
-          tma_load_3d(smem_v + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_v, &v_full[slot], dc * 64, hk, sq.k_start + j * 128);
+          for (int dc = 0; dc < D / 64; ++dc)
+            tma_load_3d(smem_k + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_k, &k_full[slot], dc * 64, hk, sq.k_start + j * 128);
+          mbar_wait_wg(&v_empty[slot], ph ^ 1);
+          uint64_t* vbar = (j * 128 + 128 > sq.Sk) ? v_land : &v_full[slot];
+          mbar_arrive_expect_tx(vbar, C::TILE_BYTES);
+#pragma unroll
+          for (int dc = 0; dc < D / 64; ++dc)
+            tma_load_3d(smem_v + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_v, vbar, dc * 64, hk, sq.k_start + j * 128);
+        }
+      }
+      __syncwarp();
+      const int jl = jend - 1, k_last = jl * 128;
+      if (k_last + 128 > sq.Sk) {
+        const int slot = (jl - jbeg) % C::NSLOT;
+        mbar_wait_wg(v_land, 0);
+        zero_tile_rows(smem_v + slot * C::TILE_BYTES, 128, D / 64, sq.Sk - k_last, lane);
+        if (lane == 0) mbar_arrive(&v_full[slot]);
       }
     }
   } else {
@@ -262,12 +308,23 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     // ---- epilogue: O / l -> global, LSE (natural log; the sink joins the denominator)
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      float lr = l[r];
+      float lr = l[r], m_fin = m[r], o_scale = 1.f;
       lr += __shfl_xor_sync(0xffffffffu, lr, 1);
       lr += __shfl_xor_sync(0xffffffffu, lr, 2);
-      const float m_safe = (m[r] == -INFINITY) ? 0.f : m[r];
-      if (p.sink != nullptr) lr += exp2f(p.sink[h] * kLog2e - m_safe);
-      const float inv_l = (lr > 0.f) ? 1.f / lr : 0.f;
+      if (p.sink != nullptr) {
+        // the sink joins the running max, so that a sink far above every score (or a row without visible keys) cannot
+        // overflow l
+        const float s2 = p.sink[h] * kLog2e;
+        if (s2 > m[r]) {
+          o_scale = exp2f(m[r] - s2);
+          lr = lr * o_scale + 1.f;
+          m_fin = s2;
+        } else if (m[r] != -INFINITY) {
+          lr += exp2f(s2 - m[r]);
+        }
+      }
+      const float m_safe = (m_fin == -INFINITY) ? 0.f : m_fin;
+      const float inv_l = (lr > 0.f) ? o_scale / lr : 0.f;
       const int qi = q0 + row_l + 8 * r;
       if (qi < sq.Sq) {
         __nv_bfloat16* dst = p.out + (static_cast<long long>(sq.q_start + qi) * p.Hq + h) * D + cq;
@@ -316,17 +373,20 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
   uint64_t* r_full = bars;          // 1
   uint64_t* st_full = bars + 1;     // [NST]
   uint64_t* st_empty = bars + 5;    // [NST]
+  uint64_t* st_land = bars + 9;     // 1: a streamed half-tile past the end of the sequence, zeroed there before st_full
 
   const int warp = threadIdx.x >> 5, lane = lane_id();
-  const int b = blockIdx.z;
+  const int tiles = ((DKV ? p.Sk : p.Sq) + 127) / 128;
+  const TileIdx bi = decode_block(tiles, DKV ? p.Hk : p.Hq);
+  const int b = bi.b;
   const SeqInfo sq = resolve_seq(p, b);
   const int g = p.Hq / p.Hk;
   // first resident row (key for DKV, query for DQ), sequence-local.  Blocks are dispatched in blockIdx order: under a causal
   // mask the heavy tiles are the early keys (DKV: natural order) and the LATE queries (DQ: reversed order), so that the light
   // tiles fill the tail of the grid
-  const int r0 = (DKV ? static_cast<int>(blockIdx.x) : static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x)) * 128;
+  const int r0 = (DKV ? bi.tile : tiles - 1 - bi.tile) * 128;
   if (r0 >= (DKV ? sq.Sk : sq.Sq)) return;
-  const int head = blockIdx.y;      // DKV: kv head; DQ: query head
+  const int head = bi.head;         // DKV: kv head; DQ: query head
   const int hk = DKV ? head : head / g;
 
   // streamed half-tile range [clo, chi) in units of 64 rows
@@ -350,6 +410,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
     tma_prefetch_desc(&tmap_s1);
     tma_prefetch_desc(&tmap_s2);
     mbar_init(r_full, 1);
+    mbar_init(st_land, 1);
     for (int i = 0; i < BWD_NST; ++i) { mbar_init(&st_full[i], DKV ? 2 : 1); mbar_init(&st_empty[i], FA_CONSUMERS); }
     fence_barrier_init();
   }
@@ -370,20 +431,33 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
         }
       }
       __syncwarp();
+      const int s_len = DKV ? sq.Sq : sq.Sk;
+      int n_land = 0;
       for (int t = 0; t < T; ++t) {
         const int st = t % BWD_NST;
         const int hs = DKV ? head * g + t / nc : hk;   // head of the streamed operand
         const int c0 = (clo + (DKV ? t % nc : t)) * 64;  // first streamed row, sequence-local
+        const bool partial = c0 + 64 > s_len;
+        uint64_t* bar = partial ? st_land : &st_full[st];
         mbar_wait_wg(&st_empty[st], ((t / BWD_NST) & 1) ^ 1);
         if (elect_one()) {
-          mbar_arrive_expect_tx(&st_full[st], 2 * C::STR_BYTES);
+          mbar_arrive_expect_tx(bar, 2 * C::STR_BYTES);
           const int srow = (DKV ? sq.q_start : sq.k_start) + c0;
           uint8_t* dst = smem_s + st * 2 * C::STR_BYTES;
 #pragma unroll
           for (int dc = 0; dc < D / 64; ++dc) {
-            tma_load_3d(dst + dc * (64 * 128), &tmap_s1, &st_full[st], dc * 64, hs, srow);
-            tma_load_3d(dst + C::STR_BYTES + dc * (64 * 128), &tmap_s2, &st_full[st], dc * 64, hs, srow);
+            tma_load_3d(dst + dc * (64 * 128), &tmap_s1, bar, dc * 64, hs, srow);
+            tma_load_3d(dst + C::STR_BYTES + dc * (64 * 128), &tmap_s2, bar, dc * 64, hs, srow);
           }
+        }
+        if (partial) {
+          // DKV: Q and dO rows past Sq (both feed a second GEMM).  DQ: K rows past Sk; its V rows only reach dP, which the
+          // mask selects away
+          __syncwarp();
+          mbar_wait_wg(st_land, n_land & 1);
+          ++n_land;
+          zero_tile_rows(smem_s + st * 2 * C::STR_BYTES, 64, DKV ? 2 * (D / 64) : D / 64, s_len - c0, lane);
+          if (lane == 0) mbar_arrive(&st_full[st]);
         }
         if constexpr (DKV) {
           // per-query statistics of this half-tile: lse in the log2 domain (+inf -> P = 0 for rows outside the sequence)
@@ -570,6 +644,38 @@ __global__ void flash_attn_delta_kernel(const __nv_bfloat16* __restrict__ o, con
   }
 }
 
+// Packed batches: rows outside every sequence (before cu[0] or from cu[B] on) belong to no kernel above.  Zero them in x0 /
+// x1 ([rows, row_elems] bf16, either may be null) and set lse[h, row] = -inf (lse may be null), reading cu on the device.
+__global__ void flash_attn_zero_outside_kernel(__nv_bfloat16* __restrict__ x0, __nv_bfloat16* __restrict__ x1, float* __restrict__ lse,
+                                               const int* __restrict__ cu, int B, long long rows, int row_elems, int H) {
+  const long long head = cu[0], tail_from = cu[B];
+  const long long n_out = head + (rows - tail_from);
+  const int chunks = row_elems / 8;  // 16-byte chunks per row
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_out * chunks; i += stride) {
+    const long long k = i / chunks, row = k < head ? k : tail_from + (k - head);
+    const long long off = row * row_elems + (i % chunks) * 8;
+    if (x0 != nullptr) *reinterpret_cast<uint4*>(x0 + off) = make_uint4(0u, 0u, 0u, 0u);
+    if (x1 != nullptr) *reinterpret_cast<uint4*>(x1 + off) = make_uint4(0u, 0u, 0u, 0u);
+  }
+  if (lse != nullptr)
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_out * H; i += stride) {
+      const long long k = i / H, row = k < head ? k : tail_from + (k - head);
+      lse[(i % H) * rows + row] = -INFINITY;
+    }
+}
+
+void check_launch(const char* what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) throw std::runtime_error(std::string("d9d flash_attn: launch of ") + what + " failed: " + cudaGetErrorString(e));
+}
+
+void zero_outside(void* x0, void* x1, float* lse, const int* cu, int B, long long rows, int row_elems, int H, cudaStream_t stream) {
+  flash_attn_zero_outside_kernel<<<128, 256, 0, stream>>>(static_cast<__nv_bfloat16*>(x0), static_cast<__nv_bfloat16*>(x1), lse, cu, B,
+                                                          rows, row_elems, H);
+  check_launch("the packed-batch padding pass");
+}
+
 // [rows, H, D] bf16 -> 3-D tensor map (d, h, row), box = 64 x 1 x box_rows, 128B swizzle
 CUtensorMap make_tmap_rhd(const void* base, long long rows, int H, int D, int box_rows) {
   CUtensorMap m;
@@ -583,6 +689,13 @@ CUtensorMap make_tmap_rhd(const void* base, long long rows, int H, int D, int bo
                                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("d9d flash_attn: cuTensorMapEncodeTiled failed: " + std::to_string(r));
   return m;
+}
+
+// (tiles of 128 rows) x H x B blocks, flattened as decode_block expects
+unsigned grid_1d(int S, int H, int B) {
+  const long long n = static_cast<long long>((S + 127) / 128) * H * B;
+  if (n > 0x7fffffffLL) throw std::runtime_error("d9d flash_attn: more than 2^31 - 1 tiles in one launch");
+  return static_cast<unsigned>(n);
 }
 
 FaParams make_params(const FlashAttnArgs& a) {
@@ -611,8 +724,8 @@ void launch_fwd(const FlashAttnArgs& a, cudaStream_t stream) {
   FaParams p = make_params(a);
   p.out = static_cast<__nv_bfloat16*>(a.out);
   p.lse = a.lse;
-  dim3 grid((a.Sq + 127) / 128, a.Hq, a.B);
-  kern<<<grid, FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  kern<<<grid_1d(a.Sq, a.Hq, a.B), FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  check_launch("the forward kernel");
 }
 
 template <int D>
@@ -621,6 +734,7 @@ void launch_delta(const FlashAttnArgs& a, cudaStream_t stream) {
   flash_attn_delta_kernel<D><<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(a.out), static_cast<const __nv_bfloat16*>(a.dout), a.delta, a.cu_q, a.B, a.Sq, a.Hq,
       a.total_q, static_cast<long long>(a.Hq) * a.Sq, a.cu_q != nullptr ? a.total_q : a.Sq);
+  check_launch("the delta kernel");
 }
 
 template <int D>
@@ -631,7 +745,7 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
   p.dq = static_cast<__nv_bfloat16*>(a.dq);
   p.dk = static_cast<__nv_bfloat16*>(a.dk);
   p.dv = static_cast<__nv_bfloat16*>(a.dv);
-  {
+  if (a.Sk > 0) {
     using C = BwdCfg<D, true>;
     auto kern = flash_attn_bwd_kernel<D, true>;
     static bool configured = false;
@@ -641,10 +755,10 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
     }
     const CUtensorMap tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 128), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 128),
                       tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 64), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, D, 64);
-    dim3 grid((a.Sk + 127) / 128, a.Hk, a.B);
-    kern<<<grid, FA_THREADS, C::SMEM_BYTES, stream>>>(tk, tv, tq, tdo, p);
+    kern<<<grid_1d(a.Sk, a.Hk, a.B), FA_THREADS, C::SMEM_BYTES, stream>>>(tk, tv, tq, tdo, p);
+    check_launch("the dK/dV kernel");
   }
-  {
+  if (a.Sq > 0) {
     using C = BwdCfg<D, false>;
     auto kern = flash_attn_bwd_kernel<D, false>;
     static bool configured = false;
@@ -654,8 +768,8 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
     }
     const CUtensorMap tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 128), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, D, 128),
                       tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 64), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 64);
-    dim3 grid((a.Sq + 127) / 128, a.Hq, a.B);
-    kern<<<grid, FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tdo, tk, tv, p);
+    kern<<<grid_1d(a.Sq, a.Hq, a.B), FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tdo, tk, tv, p);
+    check_launch("the dQ kernel");
   }
 }
 
@@ -668,9 +782,11 @@ void check_args(const FlashAttnArgs& a) {
 }  // namespace
 
 void flash_attn_fwd(const FlashAttnArgs& a, int variant, cudaStream_t stream) {
-  if (a.B == 0 || a.Sq == 0 || a.Hq == 0 || a.total_q == 0) return;
+  if (a.B == 0 || a.Hq == 0 || a.total_q == 0) return;
   check_args(a);
   (void)variant;
+  if (a.cu_q != nullptr) zero_outside(a.out, nullptr, a.lse, a.cu_q, a.B, a.total_q, a.Hq * a.D, a.Hq, stream);
+  if (a.Sq == 0) return;
   if (a.D == 64) launch_fwd<64>(a, stream);
   else launch_fwd<128>(a, stream);
 }
@@ -683,8 +799,17 @@ void flash_attn_bwd_delta(const FlashAttnArgs& a, cudaStream_t stream) {
 }
 
 void flash_attn_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
-  if (a.B == 0 || a.Hq == 0 || a.total_q == 0 || a.total_k == 0) return;
+  if (a.B == 0 || a.Hq == 0 || a.total_q == 0) return;
   check_args(a);
+  if (a.total_k == 0) {  // no key anywhere: dq = 0
+    if (cudaMemsetAsync(a.dq, 0, static_cast<size_t>(a.total_q) * a.Hq * a.D * 2, stream) != cudaSuccess)
+      throw std::runtime_error("d9d flash_attn: cudaMemsetAsync failed");
+    return;
+  }
+  if (a.cu_q != nullptr) {
+    zero_outside(a.dq, nullptr, nullptr, a.cu_q, a.B, a.total_q, a.Hq * a.D, 0, stream);
+    zero_outside(a.dk, a.dv, nullptr, a.cu_k, a.B, a.total_k, a.Hk * a.D, 0, stream);
+  }
   if (a.D == 64) launch_bwd<64>(a, stream);
   else launch_bwd<128>(a, stream);
 }
