@@ -125,6 +125,21 @@ __device__ __forceinline__ void mbar_wait_wg(uint64_t* bar, uint32_t parity) {
 #endif
 }
 
+// Same wait for warps that raised their register budget with setmaxnreg.inc: a trap anywhere in such a region makes ptxas
+// allocate all of it under the launch bound's cap (168 registers at 384 threads), with spills and serialised wgmma.  A
+// timeout sets `stuck` and every later wait returns at once; the caller traps after the region ends.
+__device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, bool& stuck) {
+#if D9D_WATCHDOG
+  uint32_t spins = 0;
+  while (!stuck && !mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 24)) stuck = true;
+  }
+#else
+  while (!mbar_try_wait(bar, parity)) {
+  }
+#endif
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA
 // ----------------------------------------------------------------------------------------------

@@ -349,6 +349,11 @@ struct BwdCfg {
   static constexpr int STR_BYTES = 64 * D * 2;        // one streamed half-tile
   static constexpr int VEC_BYTES = DKV ? BWD_NST * 2 * 64 * 4 : 0;
   static constexpr int SMEM_BYTES = 2 * RES_BYTES + BWD_NST * 2 * STR_BYTES + VEC_BYTES + 1024 + 256;
+  // per-thread register budgets (setmaxnreg; 2 x 128 x CONSUMER + 128 x PRODUCER <= 64 K).  The D = 128 consumers hold
+  // two 64 x 128 fp32 accumulators, S, dP and the bf16 A operands with wgmma in flight: below 240 ptxas serialises them
+  // (C7512).  The D = 64 producer spills at 24.
+  static constexpr int CONSUMER_REGS = D == 128 ? 240 : 232;
+  static constexpr int PRODUCER_REGS = D == 128 ? 24 : 40;
 };
 
 // Two kernels from one template (no atomics, deterministic):
@@ -416,9 +421,10 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
   }
   __syncthreads();
   const float scale_log2 = p.scale * kLog2e;
+  bool stuck = false;  // a consumer's mbarrier wait timed out (see mbar_wait_flag)
 
   if (warp < 4) {
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<C::PRODUCER_REGS>();
     // ================= producer (warp 0): TMA tiles (+ lse / delta vectors in DKV mode) =================
     if (warp == 0 && T > 0) {
       if (elect_one()) {
@@ -482,7 +488,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
       }
     }
   } else {
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<C::CONSUMER_REGS>();
     // ================= consumers: 64 resident rows each =================
     const int cw = (warp >> 2) - 1, wq = warp & 3;
     const int cq = (lane & 3) * 2;
@@ -507,86 +513,101 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) { acc1[i] = 0.f; acc2[i] = 0.f; }
     const uint32_t r1_addr = smem_u32(smem_r1) + cw * (64 * 128), r2_addr = smem_u32(smem_r2) + cw * (64 * 128);
-    if (T > 0) mbar_wait_wg(r_full, 0);
+    // Commit groups per half-tile, in issue order: S, dP, [dV,] dK / dQ.  The exp of P runs while dP is on the tensor
+    // cores and dS is formed while dV runs.  The half-tile's groups all retire before the next one starts: groups still in
+    // flight across the loop's back edge make ptxas serialise every wgmma (C7515).
+    if (T > 0) mbar_wait_flag(r_full, 0, stuck);
     for (int t = 0; t < T; ++t) {
       const int st = t % BWD_NST;
       const int c0 = (clo + (DKV ? t % nc : t)) * 64;  // first streamed row of this half-tile
-      mbar_wait_wg(&st_full[st], (t / BWD_NST) & 1);
+      mbar_wait_flag(&st_full[st], (t / BWD_NST) & 1, stuck);
       const uint32_t s1_addr = smem_u32(smem_s + st * 2 * C::STR_BYTES), s2_addr = s1_addr + C::STR_BYTES;
-      float s[32], dp[32];
+      float s[32], dp[32];          // S (then P times the soft-cap derivative), dP
+      uint32_t pf[4][4], df[4][4];  // P and dS in bf16: the A operands of the second GEMMs
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < D / 16; ++kk)
         wgmma_bf16_ss<64, 0, 0>(s, desc_kmajor(r1_addr, 128 * 128, kk), desc_kmajor(s1_addr, 64 * 128, kk), kk != 0);
+      wgmma_commit();
 #pragma unroll
       for (int kk = 0; kk < D / 16; ++kk)
         wgmma_bf16_ss<64, 0, 0>(dp, desc_kmajor(r2_addr, 128 * 128, kk), desc_kmajor(s2_addr, 64 * 128, kk), kk != 0);
       wgmma_commit();
-      wgmma_wait<0>();
+      wgmma_wait<1>();  // S
       wgmma_fence_regs(s);
-      wgmma_fence_regs(dp);
       const float* vec = smem_vec + st * 128;
+      int vlo[2], vhi[2];  // visible streamed columns [vlo, vhi] (relative to c0) of this thread's two rows
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int ri = r0 + row_l + 8 * r;  // sequence-local key (DKV) / query (DQ) index
-        // visible streamed columns [vlo, vhi] (relative to c0) of this row
-        int vlo, vhi;
         if constexpr (DKV) {  // row = key ri, column = query c0 + c
-          vlo = p.wr < 0 ? 0 : ri - sq.off - p.wr - c0;
-          vhi = p.wl < 0 ? 63 : ri - sq.off + p.wl - c0;
+          vlo[r] = p.wr < 0 ? 0 : ri - sq.off - p.wr - c0;
+          vhi[r] = p.wl < 0 ? 63 : ri - sq.off + p.wl - c0;
         } else {              // row = query ri, column = key c0 + c
-          vlo = p.wl < 0 ? 0 : ri + sq.off - p.wl - c0;
-          vhi = min(sq.Sk - 1, p.wr < 0 ? sq.Sk - 1 : ri + sq.off + p.wr) - c0;
+          vlo[r] = p.wl < 0 ? 0 : ri + sq.off - p.wl - c0;
+          vhi[r] = min(sq.Sk - 1, p.wr < 0 ? sq.Sk - 1 : ri + sq.off + p.wr) - c0;
         }
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
+          float pv[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int c = 8 * jj + cq + e;
             const int i = 4 * jj + 2 * r + e;
-            float l2, dl;
-            if constexpr (DKV) { l2 = vec[c]; dl = vec[64 + c]; }
-            else { l2 = my_lse2[r]; dl = my_delta[r]; }
-            float x = s[i], tcap = 0.f;
+            const float l2 = DKV ? vec[c] : my_lse2[r];
+            float x = s[i], dcap = 1.f;
             if (capped) {
-              tcap = tanhf(x * cap_in);
+              const float tcap = tanhf(x * cap_in);
               x = p.softcap * tcap * kLog2e;
+              dcap = 1.f - tcap * tcap;
             } else {
               x *= scale_log2;
             }
-            float pv = exp2f(x - l2);
-            float dsv = pv * (dp[i] - dl);
-            if (capped) dsv *= (1.f - tcap * tcap);
-            const bool vis = (c >= vlo) && (c <= vhi);
-            s[i] = vis ? pv : 0.f;
-            dp[i] = vis ? dsv : 0.f;
+            const bool vis = (c >= vlo[r]) && (c <= vhi[r]);
+            pv[e] = vis ? exp2f(x - l2) : 0.f;
+            s[i] = pv[e] * dcap;
           }
+          pf[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(pv[0], pv[1]);  // = pack_a_frag(P, jj / 2)
         }
       }
-      uint32_t pf[4][4], df[4][4];
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        pack_a_frag(s, ks, pf[ks]);
-        pack_a_frag(dp, ks, df[ks]);
-      }
-      wgmma_fence_regs(acc1);
-      if constexpr (DKV) wgmma_fence_regs(acc2);
-      wgmma_fence();
       if constexpr (DKV) {
+        wgmma_fence_regs(acc1);
+        wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc1, pf[ks], desc_mnmajor(s2_addr, 64 * 128, ks), 1);  // dV += P^T dO
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc2, df[ks], desc_mnmajor(s1_addr, 64 * 128, ks), 1);  // dK += dS^T Q
-      } else {
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc1, df[ks], desc_mnmajor(s1_addr, 64 * 128, ks), 1);  // dQ += dS K
+        wgmma_commit();
       }
+      wgmma_wait<DKV ? 1 : 0>();  // dP
+      wgmma_fence_regs(dp);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          float ds[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * jj + cq + e;
+            const int i = 4 * jj + 2 * r + e;
+            const float dl = DKV ? vec[64 + c] : my_delta[r];
+            // dP may be NaN at masked columns (DQ: V rows past the end of the sequence), where dS must be exactly 0
+            const bool vis = (c >= vlo[r]) && (c <= vhi[r]);
+            ds[e] = vis ? s[i] * (dp[i] - dl) : 0.f;
+          }
+          df[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(ds[0], ds[1]);
+        }
+      }
+      float(&acc_ds)[D / 2] = DKV ? acc2 : acc1;
+      wgmma_fence_regs(acc_ds);
+      wgmma_fence();
+      // DKV: dK += dS^T Q.  DQ: dQ += dS K
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc_ds, df[ks], desc_mnmajor(s1_addr, 64 * 128, ks), 1);
       wgmma_commit();
       wgmma_wait<0>();
-      wgmma_fence_regs(acc1);
-      if constexpr (DKV) wgmma_fence_regs(acc2);
       if (signal) mbar_arrive(&st_empty[st]);
     }
+    wgmma_fence_regs(acc1);
+    if constexpr (DKV) wgmma_fence_regs(acc2);
     // ---- epilogue: accumulators -> bf16 -> global.  DKV: dV, dK (scaled); DQ: dQ (scaled)
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -609,6 +630,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
       }
     }
   }
+  if (stuck) __trap();
 }
 
 // delta[b, h, q] = sum_d dO[q, h, d] * O[q, h, d]   (D/8 lanes per (row, head), 16-byte loads)
