@@ -20,6 +20,8 @@
 //   has few output tiles but a long reduction dim.
 #pragma once
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace d9d {
@@ -32,6 +34,13 @@ constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: 
 constexpr int NUM_CONSUMERS = 2;
 constexpr int NUM_EPI_WARPS = 4 * NUM_CONSUMERS;
 constexpr int EPI_BOX_ROWS = 16;  // output staging box: one warp's 16 accumulator rows x 128 bytes
+// per-thread register budgets (setmaxnreg; 2 x 128 x CONSUMER_REGS + 128 x PRODUCER_REGS <= 64 K).  A consumer holds a
+// 64 x BLOCK_N fp32 accumulator, 128 registers at BLOCK_N = 256, and the fused-CE epilogues work on all of it in place.
+// The producer's tile walk and peer tensor-map selection spill at 24 and 32 (the fused-communication GEMMs), so 240 / 24
+// is not spill-free; at 232 / 40 no instance spills.  The consumers only get this budget because their waits cannot trap
+// (see mbar_wait_flag): under a reachable trap ptxas holds them to the launch bound's 168.
+constexpr int CONSUMER_REGS = 232;
+constexpr int PRODUCER_REGS = 40;
 
 enum Mode : int { DENSE = 0, GROUPED_M = 1, GROUPED_K = 2 };
 enum Epi : int {
@@ -241,9 +250,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   if constexpr (CTAS == 2) cluster_sync_all();  // the peer's barriers are initialised before anything is multicast into it
   else __syncthreads();
 
+  bool stuck = false;  // a consumer's mbarrier wait timed out (see mbar_wait_flag)
+
   if (warp < 4) {
     // ================= TMA producer (one thread of warpgroup 0) =================
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
@@ -321,7 +332,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
   } else {
     // ================= consumers: wgmma over 64 rows each, then the epilogue of those rows =================
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = (warp >> 2) - 1;  // consumer warpgroup: rows [64 cw, 64 cw + 64) of this CTA's 128
     const int wq = warp & 3;         // warp inside the warpgroup: 16 rows
     const int lane = lane_id();
@@ -350,7 +361,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       wgmma_fence_regs(acc);
       int prev = -1;
       for (int kb = 0; kb < t.k_blocks; ++kb) {
-        mbar_wait_wg(&full_bar[stage], phase);
+        mbar_wait_flag(&full_bar[stage], phase, stuck);
         const uint32_t a_addr = smem_u32(smem_a + stage * C::A_STAGE_BYTES);
         const uint32_t b_addr = smem_u32(smem_b + stage * C::B_STAGE_BYTES);
         wgmma_fence();
@@ -377,33 +388,45 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       const bool have_acc = t.k_blocks > 0;
 
       if constexpr (EPI == EPI_CE_LSE) {
-        // softmax statistics of this tile's columns; a row's columns are spread over the 4 threads of a quad
+        // softmax statistics of this tile's columns; a row's columns are spread over the 4 threads of a quad.  Accumulator
+        // column o = 8 j + e of this thread is class col0 + cq + o: the column loops compare o with per-row bounds only
         const bool ce_xf = (p.ce_bias != nullptr) || (p.ce_softcap > 0.f);  // warp-uniform
         const float ce_inv_cap = p.ce_softcap > 0.f ? 1.f / p.ce_softcap : 0.f;
+        const int ncol = p.N - col0 - cq;  // columns o >= ncol lie past the last class
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = rbase + (lane >> 2) + 8 * h;
           const bool row_ok = row < p.M;
           long long tgt = row_ok ? p.ce_target[row] : -1;
           tgt = (tgt == p.ce_ignore_index) ? -1 : tgt - p.ce_col_offset;  // class id relative to this slice of the classifier
-          float mx = -INFINITY;
+          // the target's column o when this thread holds it (o % 8 is 0 or 1), else -1
+          const long long tgt_o = tgt - col0 - cq;
+          const bool mine = tgt >= 0 && tgt_o >= 0 && tgt_o < BLOCK_N && tgt_o < ncol && (tgt_o & 6) == 0;
+          const int trel = mine ? static_cast<int>(tgt_o) : -1;
+          float mx = -INFINITY, tgt_logit = 0.f;
+          // one loop per transform: a branch on ce_xf inside the unrolled loop keeps both paths' temporaries live
+          auto logits = [&](auto xf) {
 #pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int col = col0 + 8 * j + cq + e;
-              float v = acc[4 * j + 2 * h + e];
-              if (ce_xf) {
-                float dz;
-                const float b = (p.ce_bias != nullptr && col < p.N) ? p.ce_bias[col] : 0.f;
-                v = ce_transform(v, b, p.ce_softcap, ce_inv_cap, dz);
+              for (int e = 0; e < 2; ++e) {
+                const int o = 8 * j + e;
+                float v = acc[4 * j + 2 * h + e];
+                if constexpr (decltype(xf)::value) {
+                  float dz;
+                  const float b = (p.ce_bias != nullptr && o < ncol) ? p.ce_bias[col0 + cq + o] : 0.f;
+                  v = ce_transform(v, b, p.ce_softcap, ce_inv_cap, dz);
+                }
+                v = (o < ncol) ? v : -INFINITY;
+                acc[4 * j + 2 * h + e] = v;
+                mx = fmaxf(mx, v);
+                if (o == trel) tgt_logit = v;
               }
-              v = (col < p.N) ? v : -INFINITY;
-              acc[4 * j + 2 * h + e] = v;
-              mx = fmaxf(mx, v);
-              if (row_ok && col == tgt && col < p.N) p.ce_tgt_logit[row] = v;
             }
-          }
+          };
+          if (ce_xf) logits(std::true_type{});
+          else logits(std::false_type{});
+          if (row_ok && trel >= 0) p.ce_tgt_logit[row] = tgt_logit;
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
           float sum = 0.f;
@@ -421,9 +444,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         }
       } else {
         if constexpr (EPI == EPI_CE_DLOGITS) {
-          // D(bf16) = g[row] * (softmax - onehot) * dz/dacc, computed in place on the accumulator
+          // D(bf16) = g[row] * (softmax - onehot) * dz/dacc, computed in place on the accumulator (column o as in EPI_CE_LSE)
           const bool ce_xf = (p.ce_bias != nullptr) || (p.ce_softcap > 0.f);  // warp-uniform
           const float ce_inv_cap = p.ce_softcap > 0.f ? 1.f / p.ce_softcap : 0.f;
+          const int ncol = p.N - col0 - cq;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = rbase + (lane >> 2) + 8 * h;
@@ -435,21 +459,28 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
               g = (tgt == p.ce_ignore_index) ? 0.f : p.ce_grad[row];
               tgt = (tgt == p.ce_ignore_index) ? -1 : tgt - p.ce_col_offset;
             }
+            const long long tgt_o = tgt - col0 - cq;
+            const int trel = (tgt >= 0 && tgt_o >= 0 && tgt_o < BLOCK_N) ? static_cast<int>(tgt_o) : -1;
+            auto dlogits = [&](auto xf) {
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) {
+              for (int j = 0; j < BLOCK_N / 8; ++j) {
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int col = col0 + 8 * j + cq + e;
-                float dz = 1.f, z = acc[4 * j + 2 * h + e];
-                if (ce_xf) {
-                  const float b = (p.ce_bias != nullptr && col < p.N) ? p.ce_bias[col] : 0.f;
-                  z = ce_transform(z, b, p.ce_softcap, ce_inv_cap, dz);
+                for (int e = 0; e < 2; ++e) {
+                  const int o = 8 * j + e;
+                  float z = acc[4 * j + 2 * h + e];
+                  float dz = 1.f;
+                  if constexpr (decltype(xf)::value) {
+                    const float b = (p.ce_bias != nullptr && o < ncol) ? p.ce_bias[col0 + cq + o] : 0.f;
+                    z = ce_transform(z, b, p.ce_softcap, ce_inv_cap, dz);
+                  }
+                  float pr = __expf(z - lse);
+                  if (o == trel) pr -= 1.f;
+                  acc[4 * j + 2 * h + e] = pr * g * dz;
                 }
-                float pr = __expf(z - lse);
-                if (col == tgt) pr -= 1.f;
-                acc[4 * j + 2 * h + e] = pr * g * dz;
               }
-            }
+            };
+            if (ce_xf) dlogits(std::true_type{});
+            else dlogits(std::false_type{});
           }
         }
         constexpr bool OUT_BF16 = (EPI == EPI_BF16 || EPI == EPI_BF16_ACC || EPI == EPI_CE_DLOGITS);
@@ -564,6 +595,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 
   // pair: neither CTA leaves while its peer may still multicast into its smem or arrive on its barriers
   if constexpr (CTAS == 2) cluster_sync_all();
+  // A stuck consumer fell through its later waits (it still released every stage and stored its tiles, so neither the
+  // producer nor the pair's peer waits on it forever) and turns the hang into a trap here, outside the region whose
+  // register budget setmaxnreg raised.
+  if (stuck) __trap();
 }
 
 }  // namespace gemm
