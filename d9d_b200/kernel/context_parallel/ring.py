@@ -220,7 +220,7 @@ def _take(t: torch.Tensor, rows: slice | None) -> torch.Tensor:
 
 
 def _attend_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: float, mode: int) -> tuple[torch.Tensor, torch.Tensor]:
-    """``(out [B,Sq,H,D], lse [B,H,Sq] fp32)`` of one call: the native kernel on CUDA, the fp32 oracle elsewhere."""
+    """``(out [B,Sq,H,Dv], lse [B,H,Sq] fp32)`` of one call: the native kernel on CUDA, the fp32 oracle elsewhere."""
     if q.is_cuda:
         from d9d_b200.kernel._native import native_ops
 

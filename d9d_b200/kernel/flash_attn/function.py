@@ -72,7 +72,7 @@ _REFERENCE_SCORE_LIMIT = 1 << 22  # the fp32 oracle materialises [B,H,Sq,Sk]: te
 
 
 def _library_path_ok(q: torch.Tensor, k: torch.Tensor, causal, window_size, learnable_sink, softcap) -> bool:
-    """Shapes / dtypes outside the native kernels (e.g. latent attention with different qk / v head sizes, fp16): plain or
+    """Shapes / dtypes outside the native kernels (e.g. fp16, or qk / v head sizes the kernels are not built for): plain or
     causal attention goes to PyTorch SDPA (library flash kernels)."""
     if learnable_sink is not None or (softcap and softcap > 0):
         return False
@@ -82,11 +82,16 @@ def _library_path_ok(q: torch.Tensor, k: torch.Tensor, causal, window_size, lear
 
 
 def _sdpa(q, k, v, softmax_scale, causal):
+    """SDPA's flash kernels need one head size: a narrower V is zero-padded to the qk head size and the output sliced back."""
     import torch.nn.functional as F
 
+    dv = v.shape[-1]
+    if dv < q.shape[-1]:
+        v = F.pad(v, (0, q.shape[-1] - dv))
     qh, kh, vh = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
     out = F.scaled_dot_product_attention(qh, kh, vh, is_causal=causal, scale=softmax_scale, enable_gqa=qh.shape[1] != kh.shape[1])
-    return out.transpose(1, 2)
+    out = out.transpose(1, 2)
+    return out[..., :dv] if dv < q.shape[-1] else out
 
 
 def flash_attn_func(
@@ -105,9 +110,10 @@ def flash_attn_func(
 ) -> tuple[torch.Tensor, torch.Tensor | None]:
     """Returns ``(output [B,S,H,Dv], lse [B,H,S] or None)``.
 
-    CUDA bf16 tensors with head size 64 / 128 run the native wgmma kernels (forward and backward, every option);
-    other CUDA inputs use SDPA for plain / causal attention and raise for options it cannot express - the fp32 oracle
-    (which materialises the score matrix) is only taken on CPU or for tiny problems.
+    CUDA bf16 tensors with (qk, v) head sizes (64, 64), (128, 128) or (192, 128) run the native wgmma kernels (forward
+    and backward, every option); other CUDA inputs use SDPA for plain / causal attention (V zero-padded to the qk head
+    size when it is narrower) and raise for options it cannot express - the fp32 oracle (which materialises the score
+    matrix) is only taken on CPU or for tiny problems.
     """
     del num_splits, pack_gqa, deterministic  # the native backward is atomic-free: always deterministic
     if q.is_cuda:
@@ -121,7 +127,7 @@ def flash_attn_func(
         if q.shape[0] * q.shape[2] * q.shape[1] * k.shape[1] > _REFERENCE_SCORE_LIMIT:
             raise NotImplementedError(
                 f"attention with dtype {q.dtype}, head sizes {q.shape[-1]}/{v.shape[-1]} and these options has no fused CUDA "
-                "path (native kernels: bf16, head size 64 or 128, equal qk / v head sizes)")
+                "path (native kernels: bf16, (qk, v) head sizes (64, 64), (128, 128) or (192, 128))")
     out, lse = attention_reference(q, k, v, softmax_scale, causal, window_size, learnable_sink, softcap)
     return out, (lse if return_lse else None)
 
@@ -147,8 +153,8 @@ def flash_attn_varlen_func(
     deterministic: bool = False,
     return_lse: bool = False,
 ) -> tuple[torch.Tensor, torch.Tensor | None]:
-    """Packed variable-length attention: q ``[total_q, H, D]``, k/v ``[total_k, Hk, D]`` with ``cu_seqlens``; the LSE is
-    ``[H, total_q]``.  On CUDA the sequence boundaries are resolved inside the kernels (no host synchronisation when
+    """Packed variable-length attention: q ``[total_q, H, Dqk]``, k ``[total_k, Hk, Dqk]``, v ``[total_k, Hk, Dv]`` with
+    ``cu_seqlens``; the output is ``[total_q, H, Dv]`` and the LSE ``[H, total_q]``.  On CUDA the sequence boundaries are resolved inside the kernels (no host synchronisation when
     ``max_seqlen_q`` / ``max_seqlen_k`` are given)."""
     del num_splits, pack_gqa, deterministic
     if page_table is not None or seqused_q is not None or seqused_k is not None:

@@ -6,6 +6,9 @@ kernel (K,V resident, Q/dO streamed over the heads of the GQA group) and a dQ ke
 atomics.  Causal / sliding window (left, right) / soft-cap / attention sinks / packed variable-length batches are all
 handled inside the kernels.  There is no library (cuDNN / SDPA) call on this path.
 
+Head dims (qk, v): (64, 64), (128, 128) and (192, 128), the last for multi-head latent attention (128 nope + 64 rope query /
+key columns, 128 value columns); V, the output and dO keep their own width.
+
 """
 
 from __future__ import annotations
@@ -17,9 +20,12 @@ import torch
 from .._native import native_ops
 
 
+NATIVE_HEAD_DIMS = ((64, 64), (128, 128), (192, 128))  # (qk head dim, v head dim) pairs the kernels are built for
+
+
 def native_supported(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor) -> bool:
     return (q.is_cuda and q.dtype == torch.bfloat16 and k.dtype == torch.bfloat16 and v.dtype == torch.bfloat16
-            and q.shape[-1] in (64, 128) and v.shape[-1] == q.shape[-1] and k.shape[-1] == q.shape[-1]
+            and (q.shape[-1], v.shape[-1]) in NATIVE_HEAD_DIMS and k.shape[-1] == q.shape[-1]
             and q.shape[-2] % k.shape[-2] == 0)
 
 
@@ -31,7 +37,7 @@ def _window(causal: bool, window_size: tuple[int | None, int | None]) -> tuple[i
 
 
 class _NativeFlashAttention(torch.autograd.Function):
-    """(q, k, v[, sink]) -> (out, lse); q/k/v are [B,S,H,D] or packed [total,H,D] with ``cu_seqlens``."""
+    """(q, k, v[, sink]) -> (out, lse); q/k are [B,S,H,Dqk], v / out [B,S,H,Dv], or packed [total,H,D] with ``cu_seqlens``."""
 
     @staticmethod
     def forward(ctx, q, k, v, sink, scale, wl, wr, softcap, cu_q, cu_k, max_q, max_k):
@@ -66,7 +72,8 @@ def flash_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_s
                     window_size: tuple[int | None, int | None] = (None, None), learnable_sink: torch.Tensor | None = None,
                     softcap: float = 0.0, cu_seqlens_q: torch.Tensor | None = None, cu_seqlens_k: torch.Tensor | None = None,
                     max_seqlen_q: int = 0, max_seqlen_k: int = 0) -> tuple[torch.Tensor, torch.Tensor]:
-    """``(out, lse)``; fixed-length: q ``[B,S,H,D]``, lse ``[B,H,S]``; packed: q ``[total,H,D]``, lse ``[H,total]``."""
+    """``(out, lse)``; fixed-length: q ``[B,S,H,Dqk]``, out ``[B,S,H,Dv]``, lse ``[B,H,S]``; packed: q ``[total,H,Dqk]``,
+    out ``[total,H,Dv]``, lse ``[H,total]``."""
     scale = float(softmax_scale) if softmax_scale is not None else 1.0 / math.sqrt(q.shape[-1])
     wl, wr = _window(causal, window_size)
     if cu_seqlens_q is not None:

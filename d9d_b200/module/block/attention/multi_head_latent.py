@@ -1,7 +1,6 @@
 from __future__ import annotations
 
 import torch
-import torch.nn.functional as F
 from torch import nn
 
 from d9d_b200.module.base import ModuleLateInit
@@ -31,7 +30,8 @@ class LowRankProjection(nn.Module, ModuleLateInit):
 
 class MultiHeadLatentAttention(nn.Module, ModuleLateInit):
     """DeepSeek-V2 multi-head latent attention (reference ``d9d/module/block/attention/multi_head_latent.py:11-220``):
-    low-rank KV latent + shared rotary key, decoupled nope/rope query parts; V is zero-padded to the QK head dim.
+    low-rank KV latent + shared rotary key, decoupled nope/rope query parts.  V keeps its own head dim: the attention
+    kernels take qk and v head dims separately (the native CUDA kernels at (192, 128), DeepSeek-V2 / V3's dims).
     """
 
     def __init__(self, hidden_size: int, num_attention_heads: int, qk_nope_head_dim: int, qk_rope_head_dim: int,
@@ -84,12 +84,7 @@ class MultiHeadLatentAttention(nn.Module, ModuleLateInit):
         q = torch.cat([q_nope, q_rope], dim=-1)
         k = torch.cat([k_nope, k_rope.expand(-1, -1, h, -1)], dim=-1)
 
-        pad = self._qk - self._v
-        if pad > 0:
-            v = F.pad(v, (0, pad))
         out = self.kernel(q, k, v, attention_mask=attention_mask, is_causal=self._is_causal, scale=self._scaling)
-        if pad > 0:
-            out = out[..., : self._v]
         return self.o_proj(out.reshape(b, s, h * self._v))
 
     def reset_parameters(self) -> None:

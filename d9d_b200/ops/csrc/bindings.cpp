@@ -494,14 +494,17 @@ void scale_inplace_(Tensor x, const Tensor& scale) {
 }  // namespace
 
 // ------------------------------------------------------------------ flash attention forward / backward
-// q [B, Sq, Hq, D] (or packed [total_q, Hq, D] with cu_seqlens), k / v likewise.  window_left / window_right: -1 = unbounded.
+// q [B, Sq, Hq, Dqk] (or packed [total_q, Hq, Dqk] with cu_seqlens), k likewise with Hk heads, v like k but with Dv columns.
+// window_left / window_right: -1 = unbounded.
 static d9d::FlashAttnArgs fa_args(const Tensor& q, const Tensor& k, const Tensor& v, double scale, int64_t window_left,
                                   int64_t window_right, double softcap, const c10::optional<Tensor>& sink,
                                   const c10::optional<Tensor>& cu_q, const c10::optional<Tensor>& cu_k, int64_t max_q, int64_t max_k) {
   CHECK_CUDA_CONTIG(q); CHECK_CUDA_CONTIG(k); CHECK_CUDA_CONTIG(v);
   TORCH_CHECK(q.scalar_type() == at::kBFloat16 && k.scalar_type() == at::kBFloat16 && v.scalar_type() == at::kBFloat16,
               "flash_attn: bf16 tensors expected");
-  TORCH_CHECK(k.sizes() == v.sizes(), "flash_attn: k and v must have the same shape");
+  TORCH_CHECK(k.dim() == v.dim() && k.dim() >= 1 && k.sizes().slice(0, k.dim() - 1) == v.sizes().slice(0, v.dim() - 1),
+              "flash_attn: k and v must agree in every dimension but the last");
+  TORCH_CHECK(q.dim() == k.dim() && q.size(-1) == k.size(-1), "flash_attn: q and k must have the same head dim");
   d9d::FlashAttnArgs a{};
   a.q = q.data_ptr(); a.k = k.data_ptr(); a.v = v.data_ptr();
   const bool varlen = cu_q.has_value();
@@ -514,14 +517,15 @@ static d9d::FlashAttnArgs fa_args(const Tensor& q, const Tensor& k, const Tensor
     a.B = static_cast<int>(cu_q->numel() - 1);
     a.Sq = static_cast<int>(max_q); a.Sk = static_cast<int>(max_k);
     a.total_q = q.size(0); a.total_k = k.size(0);
-    a.Hq = static_cast<int>(q.size(1)); a.Hk = static_cast<int>(k.size(1)); a.D = static_cast<int>(q.size(2));
-    TORCH_CHECK(k.size(2) == a.D);
+    a.Hq = static_cast<int>(q.size(1)); a.Hk = static_cast<int>(k.size(1));
+    a.Dqk = static_cast<int>(q.size(2)); a.Dv = static_cast<int>(v.size(2));
     a.cu_q = cu_q->data_ptr<int>(); a.cu_k = cu_k->data_ptr<int>();
   } else {
     TORCH_CHECK(q.dim() == 4 && k.dim() == 4, "flash_attn: [B, S, H, D] tensors expected");
-    TORCH_CHECK(q.size(0) == k.size(0) && q.size(3) == k.size(3));
+    TORCH_CHECK(q.size(0) == k.size(0));
     a.B = static_cast<int>(q.size(0)); a.Sq = static_cast<int>(q.size(1)); a.Sk = static_cast<int>(k.size(1));
-    a.Hq = static_cast<int>(q.size(2)); a.Hk = static_cast<int>(k.size(2)); a.D = static_cast<int>(q.size(3));
+    a.Hq = static_cast<int>(q.size(2)); a.Hk = static_cast<int>(k.size(2));
+    a.Dqk = static_cast<int>(q.size(3)); a.Dv = static_cast<int>(v.size(3));
     a.total_q = static_cast<long long>(a.B) * a.Sq; a.total_k = static_cast<long long>(a.B) * a.Sk;
   }
   a.window_left = static_cast<int>(window_left); a.window_right = static_cast<int>(window_right);
@@ -532,6 +536,13 @@ static d9d::FlashAttnArgs fa_args(const Tensor& q, const Tensor& k, const Tensor
     a.sink = sink->data_ptr<float>();
   }
   return a;
+}
+
+// out / dout: q's shape with v's head dim
+static std::vector<int64_t> fa_out_shape(const d9d::FlashAttnArgs& a, const Tensor& q) {
+  std::vector<int64_t> s = q.sizes().vec();
+  s.back() = a.Dv;
+  return s;
 }
 
 static Tensor fa_stats_like(const d9d::FlashAttnArgs& a, const Tensor& q) {
@@ -545,7 +556,7 @@ std::tuple<Tensor, Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, cons
                                           int64_t max_k, int64_t variant) {
   c10::cuda::CUDAGuard guard(q.device());
   d9d::FlashAttnArgs a = fa_args(q, k, v, scale, window_left, window_right, softcap, sink, cu_q, cu_k, max_q, max_k);
-  Tensor out = at::empty_like(q);
+  Tensor out = at::empty(fa_out_shape(a, q), q.options());
   Tensor lse = fa_stats_like(a, q);
   a.out = out.data_ptr();
   a.lse = lse.data_ptr<float>();
@@ -561,8 +572,10 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> flash_attn_bwd(const Tensor& dout, co
   c10::cuda::CUDAGuard guard(q.device());
   CHECK_CUDA_CONTIG(dout); CHECK_CUDA_CONTIG(out); CHECK_CUDA_CONTIG(lse);
   TORCH_CHECK(dout.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16 && lse.scalar_type() == at::kFloat);
-  TORCH_CHECK(dout.sizes() == q.sizes() && out.sizes() == q.sizes(), "flash_attn_bwd: dout / out must match q");
   d9d::FlashAttnArgs a = fa_args(q, k, v, scale, window_left, window_right, softcap, c10::nullopt, cu_q, cu_k, max_q, max_k);
+  const std::vector<int64_t> out_shape = fa_out_shape(a, q);
+  TORCH_CHECK(dout.sizes() == c10::IntArrayRef(out_shape) && out.sizes() == c10::IntArrayRef(out_shape),
+              "flash_attn_bwd: dout / out must have q's shape with v's head dim");
   Tensor delta = fa_stats_like(a, q);
   TORCH_CHECK(lse.numel() == delta.numel(), "flash_attn_bwd: lse has the wrong shape");
   Tensor dq = at::empty_like(q), dk = at::empty_like(k), dv = at::empty_like(v);

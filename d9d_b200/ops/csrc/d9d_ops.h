@@ -159,7 +159,8 @@ void sumsq_accumulate(const void* x, long long n, int dtype, float* out, cudaStr
 void scale_inplace(void* x, long long n, int dtype, const float* scale, cudaStream_t stream);
 
 // ------------------------------------------------------------------ flash attention (forward / backward) --
-// q / out / dout / dq [total_q, Hq, D], k / v / dk / dv [total_k, Hk, D] bf16 contiguous, where total = B * S for
+// q / dq [total_q, Hq, Dqk], out / dout [total_q, Hq, Dv], k / dk [total_k, Hk, Dqk], v / dv [total_k, Hk, Dv] bf16
+// contiguous, (Dqk, Dv) one of (64, 64), (128, 128), (192, 128), where total = B * S for
 // fixed-length batches (cu_q == cu_k == nullptr) or the packed token count (cu_q / cu_k: [B + 1] int32 device arrays, Sq /
 // Sk = maximum sequence lengths).  lse / delta: fp32 [B, Hq, Sq] (packed: [Hq, total_q]).
 // window: key k is visible to query q iff q + (Sk - Sq) - window_left <= k <= q + (Sk - Sq) + window_right (-1 = unbounded;
@@ -175,7 +176,7 @@ struct FlashAttnArgs {
   void *dq, *dk, *dv;   // backward outputs
   const float* sink;
   const int *cu_q, *cu_k;
-  int B, Sq, Sk, Hq, Hk, D;
+  int B, Sq, Sk, Hq, Hk, Dqk, Dv;
   long long total_q, total_k;
   int window_left, window_right;
   float scale, softcap;

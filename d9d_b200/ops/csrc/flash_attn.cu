@@ -6,6 +6,8 @@
 //
 // All tensors are [rows, H, D] row-major views of the projection outputs (rows = B*S, or the packed token count):
 // no transposes, TMA 3-D maps (d, h, row) with 128B swizzle.  LSE / delta are fp32 [B, H, S] (packed: [H, total]).
+// Q / K / dQ / dK have head dim DQK, V / O / dO / dV head dim DV; the built pairs (DQK, DV) are (64, 64), (128, 128) and
+// (192, 128) (multi-head latent attention: 128 nope + 64 rope query / key columns, 128 value columns).
 //
 // Forward (flash_attn_fwd_kernel): one CTA owns a 128-row query tile of one (batch, head); warpgroup 0 streams K / V tiles
 // of 128 keys with TMA, warpgroups 1-2 own 64 query rows each with S, P and O in registers (P is handed to the second
@@ -116,28 +118,36 @@ __device__ __forceinline__ void pack_a_frag(const float (&d)[R], int s, uint32_t
   a[3] = pack_bf16x2(d[8 * s + 6], d[8 * s + 7]);
 }
 
-template <int D>
+// select one of two lvalues at compile time (they may have different types)
+template <bool FIRST, class A, class B>
+__device__ __forceinline__ auto& pick(A& a, B& b) {
+  if constexpr (FIRST) return a;
+  else return b;
+}
+
+template <int DQK, int DV>
 struct FwdCfg {
-  static constexpr int TILE_BYTES = 128 * D * 2;  // Q tile and every K / V tile: 128 rows
+  static constexpr int QK_BYTES = 128 * DQK * 2;  // Q tile and every K tile: 128 rows
+  static constexpr int V_BYTES = 128 * DV * 2;    // every V tile
   static constexpr int NSLOT = 2;                 // K and V rings
-  static constexpr int SMEM_BYTES = TILE_BYTES + 2 * NSLOT * TILE_BYTES + 1024 + 256;
+  static constexpr int SMEM_BYTES = QK_BYTES + NSLOT * (QK_BYTES + V_BYTES) + 1024 + 256;
 };
 
 // One CTA owns a 128-row query tile of one (batch, head); each consumer warpgroup owns 64 of its rows and keeps S, P and O
 // in registers: S = Q K_j^T (wgmma from shared memory), online softmax on the fragment (a row lives in the 4 threads of a
 // quad), P packed to bf16 in place as the register A operand of O += P V_j.  The producer streams K_j / V_j through two
 // 2-slot rings, so the loads of tile j+1 run under the math of tile j.
-template <int D>
+template <int DQK, int DV>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const FaParams p) {
-  using C = FwdCfg<D>;
+  using C = FwdCfg<DQK, DV>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_q = smem;
-  uint8_t* smem_k = smem_q + C::TILE_BYTES;               // [NSLOT][TILE]
-  uint8_t* smem_v = smem_k + C::NSLOT * C::TILE_BYTES;    // [NSLOT][TILE]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + C::NSLOT * C::TILE_BYTES);
+  uint8_t* smem_k = smem_q + C::QK_BYTES;               // [NSLOT][QK tile]
+  uint8_t* smem_v = smem_k + C::NSLOT * C::QK_BYTES;    // [NSLOT][V tile]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + C::NSLOT * C::V_BYTES);
   uint64_t* bar_q = bars;         // 1
   uint64_t* k_full = bars + 1;    // [2]
   uint64_t* k_empty = bars + 3;   // [2]
@@ -183,24 +193,24 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     // Sk only reach masked scores)
     if (warp == 0 && jend > jbeg) {
       if (elect_one()) {
-        mbar_arrive_expect_tx(bar_q, C::TILE_BYTES);
+        mbar_arrive_expect_tx(bar_q, C::QK_BYTES);
 #pragma unroll
-        for (int dc = 0; dc < D / 64; ++dc)
+        for (int dc = 0; dc < DQK / 64; ++dc)
           tma_load_3d(smem_q + dc * (128 * 128), &tmap_q, bar_q, dc * 64, h, sq.q_start + q0);
         for (int j = jbeg; j < jend; ++j) {
           const int n = j - jbeg, slot = n % C::NSLOT;
           const uint32_t ph = (n / C::NSLOT) & 1;
           mbar_wait_wg(&k_empty[slot], ph ^ 1);
-          mbar_arrive_expect_tx(&k_full[slot], C::TILE_BYTES);
+          mbar_arrive_expect_tx(&k_full[slot], C::QK_BYTES);
 #pragma unroll
-          for (int dc = 0; dc < D / 64; ++dc)
-            tma_load_3d(smem_k + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_k, &k_full[slot], dc * 64, hk, sq.k_start + j * 128);
+          for (int dc = 0; dc < DQK / 64; ++dc)
+            tma_load_3d(smem_k + slot * C::QK_BYTES + dc * (128 * 128), &tmap_k, &k_full[slot], dc * 64, hk, sq.k_start + j * 128);
           mbar_wait_wg(&v_empty[slot], ph ^ 1);
           uint64_t* vbar = (j * 128 + 128 > sq.Sk) ? v_land : &v_full[slot];
-          mbar_arrive_expect_tx(vbar, C::TILE_BYTES);
+          mbar_arrive_expect_tx(vbar, C::V_BYTES);
 #pragma unroll
-          for (int dc = 0; dc < D / 64; ++dc)
-            tma_load_3d(smem_v + slot * C::TILE_BYTES + dc * (128 * 128), &tmap_v, vbar, dc * 64, hk, sq.k_start + j * 128);
+          for (int dc = 0; dc < DV / 64; ++dc)
+            tma_load_3d(smem_v + slot * C::V_BYTES + dc * (128 * 128), &tmap_v, vbar, dc * 64, hk, sq.k_start + j * 128);
         }
       }
       __syncwarp();
@@ -208,7 +218,7 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       if (k_last + 128 > sq.Sk) {
         const int slot = (jl - jbeg) % C::NSLOT;
         mbar_wait_wg(v_land, 0);
-        zero_tile_rows(smem_v + slot * C::TILE_BYTES, 128, D / 64, sq.Sk - k_last, lane);
+        zero_tile_rows(smem_v + slot * C::V_BYTES, 128, DV / 64, sq.Sk - k_last, lane);
         if (lane == 0) mbar_arrive(&v_full[slot]);
       }
     }
@@ -230,9 +240,9 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const float scale_eff = capped ? kLog2e : p.scale * kLog2e;  // log2-domain multiplier of the (capped) score
     const float cap_in = capped ? p.scale / p.softcap : 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-    float o[D / 2];
+    float o[DV / 2];
 #pragma unroll
-    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
     const uint32_t q_addr = smem_u32(smem_q) + cw * (64 * 128);
     if (jend > jbeg) mbar_wait_wg(bar_q, 0);
     for (int j = jbeg; j < jend; ++j) {
@@ -241,10 +251,10 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       const int k0 = j * 128;
       float s[64];
       mbar_wait_wg(&k_full[slot], ph);
-      const uint32_t k_addr = smem_u32(smem_k + slot * C::TILE_BYTES);
+      const uint32_t k_addr = smem_u32(smem_k + slot * C::QK_BYTES);
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk)
+      for (int kk = 0; kk < DQK / 16; ++kk)
         wgmma_bf16_ss<128, 0, 0>(s, desc_kmajor(q_addr, 128 * 128, kk), desc_kmajor(k_addr, 128 * 128, kk), kk != 0);
       wgmma_commit();
       wgmma_wait<0>();
@@ -287,7 +297,7 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         l[r] += sum;  // partial over this thread's columns; the quad is summed once at the end
       }
 #pragma unroll
-      for (int jj = 0; jj < D / 8; ++jj) {
+      for (int jj = 0; jj < DV / 8; ++jj) {
         o[4 * jj + 0] *= alpha[0]; o[4 * jj + 1] *= alpha[0];
         o[4 * jj + 2] *= alpha[1]; o[4 * jj + 3] *= alpha[1];
       }
@@ -295,11 +305,11 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 #pragma unroll
       for (int ks = 0; ks < 8; ++ks) pack_a_frag(s, ks, pa[ks]);
       mbar_wait_wg(&v_full[slot], ph);
-      const uint32_t v_addr = smem_u32(smem_v + slot * C::TILE_BYTES);
+      const uint32_t v_addr = smem_u32(smem_v + slot * C::V_BYTES);
       wgmma_fence_regs(o);
       wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) wgmma_bf16_rs<D, 1>(o, pa[ks], desc_mnmajor(v_addr, 128 * 128, ks), 1);
+      for (int ks = 0; ks < 8; ++ks) wgmma_bf16_rs<DV, 1>(o, pa[ks], desc_mnmajor(v_addr, 128 * 128, ks), 1);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(o);
@@ -327,9 +337,9 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       const float inv_l = (lr > 0.f) ? o_scale / lr : 0.f;
       const int qi = q0 + row_l + 8 * r;
       if (qi < sq.Sq) {
-        __nv_bfloat16* dst = p.out + (static_cast<long long>(sq.q_start + qi) * p.Hq + h) * D + cq;
+        __nv_bfloat16* dst = p.out + (static_cast<long long>(sq.q_start + qi) * p.Hq + h) * DV + cq;
 #pragma unroll
-        for (int jj = 0; jj < D / 8; ++jj)
+        for (int jj = 0; jj < DV / 8; ++jj)
           *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * r] * inv_l, o[4 * jj + 2 * r + 1] * inv_l);
         if ((lane & 3) == 0 && p.lse != nullptr)
           p.lse[sq.lse_base + static_cast<long long>(h) * p.lse_hs + qi] = (lr > 0.f) ? (m_safe + log2f(lr)) * kLn2 : -INFINITY;
@@ -341,44 +351,52 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 // ======================================================================================================
 // backward
 // ======================================================================================================
-constexpr int BWD_NST = 4;  // streamed half-tile ring depth
-
-template <int D, bool DKV>
+template <int DQK, int DV, bool DKV>
 struct BwdCfg {
-  static constexpr int RES_BYTES = 128 * D * 2;       // one resident tile
-  static constexpr int STR_BYTES = 64 * D * 2;        // one streamed half-tile
-  static constexpr int VEC_BYTES = DKV ? BWD_NST * 2 * 64 * 4 : 0;
-  static constexpr int SMEM_BYTES = 2 * RES_BYTES + BWD_NST * 2 * STR_BYTES + VEC_BYTES + 1024 + 256;
+  // Streamed tile height SR and ring depth NST.  At (192, 128) the dK/dV consumers hold dK (96 registers) and dV (64): with
+  // 64-row streamed tiles S^T, dP^T and their bf16 operands would take another 96, so they stream 32-row tiles (m64n32 S^T
+  // and dP^T).  Four 64-row stages of Q + dO (dK/dV) or K + V (dQ) exceed shared memory at DQK = 192: dQ keeps three.
+  static constexpr int SR = (DQK == 192 && DKV) ? 32 : 64;
+  static constexpr int NST = DQK == 192 ? (DKV ? 6 : 3) : 4;
+  static constexpr int R1_BYTES = 128 * DQK * 2;  // resident K (DKV) / Q (DQ)
+  static constexpr int R2_BYTES = 128 * DV * 2;   // resident V (DKV) / dO (DQ)
+  static constexpr int S1_BYTES = SR * DQK * 2;   // streamed Q (DKV) / K (DQ)
+  static constexpr int S2_BYTES = SR * DV * 2;    // streamed dO (DKV) / V (DQ)
+  static constexpr int STAGE_BYTES = S1_BYTES + S2_BYTES;
+  static constexpr int VEC_BYTES = DKV ? NST * 2 * SR * 4 : 0;
+  static constexpr int SMEM_BYTES = R1_BYTES + R2_BYTES + NST * STAGE_BYTES + VEC_BYTES + 1024 + 256;
   // per-thread register budgets (setmaxnreg; 2 x 128 x CONSUMER + 128 x PRODUCER <= 64 K).  The D = 128 consumers hold
   // two 64 x 128 fp32 accumulators, S, dP and the bf16 A operands with wgmma in flight: below 240 ptxas serialises them
   // (C7512).  The D = 64 producer spills at 24.
-  static constexpr int CONSUMER_REGS = D == 128 ? 240 : 232;
-  static constexpr int PRODUCER_REGS = D == 128 ? 24 : 40;
+  static constexpr int CONSUMER_REGS = DQK == 64 ? 232 : 240;
+  static constexpr int PRODUCER_REGS = DQK == 64 ? 40 : 24;
 };
 
 // Two kernels from one template (no atomics, deterministic):
-//   DKV: CTA owns a 128-key tile of one kv head (64 keys per consumer warpgroup), keeps K,V resident, streams 64-row Q/dO
-//        half-tiles of every query head of the group: S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T (registers, bf16 A operands)
+//   DKV: CTA owns a 128-key tile of one kv head (64 keys per consumer warpgroup), keeps K,V resident, streams SR-row Q/dO
+//        tiles of every query head of the group: S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T (registers, bf16 A operands)
 //        -> dV += P^T dO, dK += dS^T Q accumulated in registers over the whole loop.
-//   DQ : CTA owns a 128-row query tile of one head, keeps Q,dO resident, streams 64-key K/V half-tiles:
+//   DQ : CTA owns a 128-row query tile of one head, keeps Q,dO resident, streams SR-key K/V tiles:
 //        S = Q K^T, dP = dO V^T -> dS -> dQ += dS K.
-template <int D, bool DKV>
+// S and dS reduce over DQK (Q, K), dP over DV (V, dO).
+template <int DQK, int DV, bool DKV>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_constant__ CUtensorMap tmap_r2,
                       const __grid_constant__ CUtensorMap tmap_s1, const __grid_constant__ CUtensorMap tmap_s2, const FaParams p) {
-  // DKV: r1 = K, r2 = V (128-row boxes), s1 = Q, s2 = dO (64-row boxes).   DQ: r1 = Q, r2 = dO, s1 = K, s2 = V.
-  using C = BwdCfg<D, DKV>;
+  // DKV: r1 = K, r2 = V (128-row boxes), s1 = Q, s2 = dO (SR-row boxes).   DQ: r1 = Q, r2 = dO, s1 = K, s2 = V.
+  using C = BwdCfg<DQK, DV, DKV>;
+  constexpr int SR = C::SR, NST = C::NST;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_r1 = smem;
-  uint8_t* smem_r2 = smem_r1 + C::RES_BYTES;
-  uint8_t* smem_s = smem_r2 + C::RES_BYTES;                      // [NST][s1 | s2]
-  float* smem_vec = reinterpret_cast<float*>(smem_s + BWD_NST * 2 * C::STR_BYTES);  // DKV: [NST][lse2(64) | delta(64)]
+  uint8_t* smem_r2 = smem_r1 + C::R1_BYTES;
+  uint8_t* smem_s = smem_r2 + C::R2_BYTES;                      // [NST][s1 | s2]
+  float* smem_vec = reinterpret_cast<float*>(smem_s + NST * C::STAGE_BYTES);  // DKV: [NST][lse2(SR) | delta(SR)]
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(smem_vec) + C::VEC_BYTES);
-  uint64_t* r_full = bars;          // 1
-  uint64_t* st_full = bars + 1;     // [NST]
-  uint64_t* st_empty = bars + 5;    // [NST]
-  uint64_t* st_land = bars + 9;     // 1: a streamed half-tile past the end of the sequence, zeroed there before st_full
+  uint64_t* r_full = bars;                  // 1
+  uint64_t* st_full = bars + 1;             // [NST]
+  uint64_t* st_empty = bars + 1 + NST;      // [NST]
+  uint64_t* st_land = bars + 1 + 2 * NST;   // 1: a streamed tile past the end of the sequence, zeroed there before st_full
 
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const int tiles = ((DKV ? p.Sk : p.Sq) + 127) / 128;
@@ -394,20 +412,20 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
   const int head = bi.head;         // DKV: kv head; DQ: query head
   const int hk = DKV ? head : head / g;
 
-  // streamed half-tile range [clo, chi) in units of 64 rows
+  // streamed tile range [clo, chi) in units of SR rows
   int clo = 0, chi = 0;
   if constexpr (DKV) {
     const int qa = p.wr < 0 ? 0 : max(0, r0 - sq.off - p.wr);                         // first query seeing key r0
     const int qb = p.wl < 0 ? sq.Sq - 1 : min(sq.Sq - 1, r0 + 127 - sq.off + p.wl);    // last query seeing key r0+127
-    if (qb >= qa) { clo = qa / 64; chi = qb / 64 + 1; }
+    if (qb >= qa) { clo = qa / SR; chi = qb / SR + 1; }
   } else {
     const int qb = min(r0 + 127, sq.Sq - 1);
     const int ka = p.wl < 0 ? 0 : max(0, r0 + sq.off - p.wl);
     const int kb = p.wr < 0 ? sq.Sk - 1 : min(sq.Sk - 1, qb + sq.off + p.wr);
-    if (kb >= ka) { clo = ka / 64; chi = kb / 64 + 1; }
+    if (kb >= ka) { clo = ka / SR; chi = kb / SR + 1; }
   }
   const int nc = chi - clo;
-  const int T = DKV ? g * nc : nc;  // streamed half-tiles processed by this CTA
+  const int T = DKV ? g * nc : nc;  // streamed tiles processed by this CTA
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_r1);
@@ -416,7 +434,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
     tma_prefetch_desc(&tmap_s2);
     mbar_init(r_full, 1);
     mbar_init(st_land, 1);
-    for (int i = 0; i < BWD_NST; ++i) { mbar_init(&st_full[i], DKV ? 2 : 1); mbar_init(&st_empty[i], FA_CONSUMERS); }
+    for (int i = 0; i < NST; ++i) { mbar_init(&st_full[i], DKV ? 2 : 1); mbar_init(&st_empty[i], FA_CONSUMERS); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -428,58 +446,59 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
     // ================= producer (warp 0): TMA tiles (+ lse / delta vectors in DKV mode) =================
     if (warp == 0 && T > 0) {
       if (elect_one()) {
-        mbar_arrive_expect_tx(r_full, 2 * C::RES_BYTES);
+        mbar_arrive_expect_tx(r_full, C::R1_BYTES + C::R2_BYTES);
         const int rrow = (DKV ? sq.k_start : sq.q_start) + r0;
 #pragma unroll
-        for (int dc = 0; dc < D / 64; ++dc) {
+        for (int dc = 0; dc < DQK / 64; ++dc) {
           tma_load_3d(smem_r1 + dc * (128 * 128), &tmap_r1, r_full, dc * 64, head, rrow);
-          tma_load_3d(smem_r2 + dc * (128 * 128), &tmap_r2, r_full, dc * 64, head, rrow);
+          if (dc < DV / 64) tma_load_3d(smem_r2 + dc * (128 * 128), &tmap_r2, r_full, dc * 64, head, rrow);
         }
       }
       __syncwarp();
       const int s_len = DKV ? sq.Sq : sq.Sk;
       int n_land = 0;
       for (int t = 0; t < T; ++t) {
-        const int st = t % BWD_NST;
+        const int st = t % NST;
         const int hs = DKV ? head * g + t / nc : hk;   // head of the streamed operand
-        const int c0 = (clo + (DKV ? t % nc : t)) * 64;  // first streamed row, sequence-local
-        const bool partial = c0 + 64 > s_len;
+        const int c0 = (clo + (DKV ? t % nc : t)) * SR;  // first streamed row, sequence-local
+        const bool partial = c0 + SR > s_len;
         uint64_t* bar = partial ? st_land : &st_full[st];
-        mbar_wait_wg(&st_empty[st], ((t / BWD_NST) & 1) ^ 1);
+        mbar_wait_wg(&st_empty[st], ((t / NST) & 1) ^ 1);
         if (elect_one()) {
-          mbar_arrive_expect_tx(bar, 2 * C::STR_BYTES);
+          mbar_arrive_expect_tx(bar, C::STAGE_BYTES);
           const int srow = (DKV ? sq.q_start : sq.k_start) + c0;
-          uint8_t* dst = smem_s + st * 2 * C::STR_BYTES;
+          uint8_t* dst = smem_s + st * C::STAGE_BYTES;
 #pragma unroll
-          for (int dc = 0; dc < D / 64; ++dc) {
-            tma_load_3d(dst + dc * (64 * 128), &tmap_s1, bar, dc * 64, hs, srow);
-            tma_load_3d(dst + C::STR_BYTES + dc * (64 * 128), &tmap_s2, bar, dc * 64, hs, srow);
+          for (int dc = 0; dc < DQK / 64; ++dc) {
+            tma_load_3d(dst + dc * (SR * 128), &tmap_s1, bar, dc * 64, hs, srow);
+            if (dc < DV / 64) tma_load_3d(dst + C::S1_BYTES + dc * (SR * 128), &tmap_s2, bar, dc * 64, hs, srow);
           }
         }
         if (partial) {
           // DKV: Q and dO rows past Sq (both feed a second GEMM).  DQ: K rows past Sk; its V rows only reach dP, which the
-          // mask selects away
+          // mask selects away.  The stage's boxes are contiguous: Q (K) boxes, then dO (V) boxes
           __syncwarp();
           mbar_wait_wg(st_land, n_land & 1);
           ++n_land;
-          zero_tile_rows(smem_s + st * 2 * C::STR_BYTES, 64, DKV ? 2 * (D / 64) : D / 64, s_len - c0, lane);
+          zero_tile_rows(smem_s + st * C::STAGE_BYTES, SR, DKV ? DQK / 64 + DV / 64 : DQK / 64, s_len - c0, lane);
           if (lane == 0) mbar_arrive(&st_full[st]);
         }
         if constexpr (DKV) {
-          // per-query statistics of this half-tile: lse in the log2 domain (+inf -> P = 0 for rows outside the sequence)
-          float* vec = smem_vec + st * 128;
+          // per-query statistics of this tile: lse in the log2 domain (+inf -> P = 0 for rows outside the sequence)
+          constexpr int PER_LANE = SR / 32;
+          float* vec = smem_vec + st * (2 * SR);
           const long long base = sq.lse_base + static_cast<long long>(hs) * p.lse_hs;
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int q = c0 + lane * 2 + e;
+          for (int e = 0; e < PER_LANE; ++e) {
+            const int q = c0 + lane * PER_LANE + e;
             float l2 = INFINITY, dl = 0.f;
             if (q < sq.Sq) {
               const float lv = p.lse[base + q];
               l2 = (lv == -INFINITY) ? INFINITY : lv * kLog2e;
               dl = p.delta[base + q];
             }
-            vec[lane * 2 + e] = l2;
-            vec[64 + lane * 2 + e] = dl;
+            vec[lane * PER_LANE + e] = l2;
+            vec[SR + lane * PER_LANE + e] = dl;
           }
           __syncwarp();
           if (lane == 0) mbar_arrive(&st_full[st]);
@@ -509,46 +528,50 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
         }
       }
     }
-    float acc1[D / 2], acc2[D / 2];  // DKV: dV, dK.  DQ: dQ, unused
+    constexpr int ACC1 = DKV ? DV / 2 : DQK / 2;
+    float acc1[ACC1], acc2[DQK / 2];  // DKV: dV, dK.  DQ: dQ, unused
 #pragma unroll
-    for (int i = 0; i < D / 2; ++i) { acc1[i] = 0.f; acc2[i] = 0.f; }
+    for (int i = 0; i < DQK / 2; ++i) {
+      if (i < ACC1) acc1[i] = 0.f;
+      acc2[i] = 0.f;
+    }
     const uint32_t r1_addr = smem_u32(smem_r1) + cw * (64 * 128), r2_addr = smem_u32(smem_r2) + cw * (64 * 128);
-    // Commit groups per half-tile, in issue order: S, dP, [dV,] dK / dQ.  The exp of P runs while dP is on the tensor
-    // cores and dS is formed while dV runs.  The half-tile's groups all retire before the next one starts: groups still in
+    // Commit groups per streamed tile, in issue order: S, dP, [dV,] dK / dQ.  The exp of P runs while dP is on the tensor
+    // cores and dS is formed while dV runs.  The tile's groups all retire before the next one starts: groups still in
     // flight across the loop's back edge make ptxas serialise every wgmma (C7515).
     if (T > 0) mbar_wait_flag(r_full, 0, stuck);
     for (int t = 0; t < T; ++t) {
-      const int st = t % BWD_NST;
-      const int c0 = (clo + (DKV ? t % nc : t)) * 64;  // first streamed row of this half-tile
-      mbar_wait_flag(&st_full[st], (t / BWD_NST) & 1, stuck);
-      const uint32_t s1_addr = smem_u32(smem_s + st * 2 * C::STR_BYTES), s2_addr = s1_addr + C::STR_BYTES;
-      float s[32], dp[32];          // S (then P times the soft-cap derivative), dP
-      uint32_t pf[4][4], df[4][4];  // P and dS in bf16: the A operands of the second GEMMs
+      const int st = t % NST;
+      const int c0 = (clo + (DKV ? t % nc : t)) * SR;  // first streamed row of this tile
+      mbar_wait_flag(&st_full[st], (t / NST) & 1, stuck);
+      const uint32_t s1_addr = smem_u32(smem_s + st * C::STAGE_BYTES), s2_addr = s1_addr + C::S1_BYTES;
+      float s[SR / 2], dp[SR / 2];            // S (then P times the soft-cap derivative), dP
+      uint32_t pf[SR / 16][4], df[SR / 16][4];  // P and dS in bf16: the A operands of the second GEMMs
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk)
-        wgmma_bf16_ss<64, 0, 0>(s, desc_kmajor(r1_addr, 128 * 128, kk), desc_kmajor(s1_addr, 64 * 128, kk), kk != 0);
+      for (int kk = 0; kk < DQK / 16; ++kk)
+        wgmma_bf16_ss<SR, 0, 0>(s, desc_kmajor(r1_addr, 128 * 128, kk), desc_kmajor(s1_addr, SR * 128, kk), kk != 0);
       wgmma_commit();
 #pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk)
-        wgmma_bf16_ss<64, 0, 0>(dp, desc_kmajor(r2_addr, 128 * 128, kk), desc_kmajor(s2_addr, 64 * 128, kk), kk != 0);
+      for (int kk = 0; kk < DV / 16; ++kk)
+        wgmma_bf16_ss<SR, 0, 0>(dp, desc_kmajor(r2_addr, 128 * 128, kk), desc_kmajor(s2_addr, SR * 128, kk), kk != 0);
       wgmma_commit();
       wgmma_wait<1>();  // S
       wgmma_fence_regs(s);
-      const float* vec = smem_vec + st * 128;
+      const float* vec = smem_vec + st * (2 * SR);
       int vlo[2], vhi[2];  // visible streamed columns [vlo, vhi] (relative to c0) of this thread's two rows
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int ri = r0 + row_l + 8 * r;  // sequence-local key (DKV) / query (DQ) index
         if constexpr (DKV) {  // row = key ri, column = query c0 + c
           vlo[r] = p.wr < 0 ? 0 : ri - sq.off - p.wr - c0;
-          vhi[r] = p.wl < 0 ? 63 : ri - sq.off + p.wl - c0;
+          vhi[r] = p.wl < 0 ? SR - 1 : ri - sq.off + p.wl - c0;
         } else {              // row = query ri, column = key c0 + c
           vlo[r] = p.wl < 0 ? 0 : ri + sq.off - p.wl - c0;
           vhi[r] = min(sq.Sk - 1, p.wr < 0 ? sq.Sk - 1 : ri + sq.off + p.wr) - c0;
         }
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
+        for (int jj = 0; jj < SR / 8; ++jj) {
           float pv[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
@@ -574,7 +597,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
         wgmma_fence_regs(acc1);
         wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc1, pf[ks], desc_mnmajor(s2_addr, 64 * 128, ks), 1);  // dV += P^T dO
+        for (int ks = 0; ks < SR / 16; ++ks) wgmma_bf16_rs<DV, 1>(acc1, pf[ks], desc_mnmajor(s2_addr, SR * 128, ks), 1);  // dV += P^T dO
         wgmma_commit();
       }
       wgmma_wait<DKV ? 1 : 0>();  // dP
@@ -582,13 +605,13 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
+        for (int jj = 0; jj < SR / 8; ++jj) {
           float ds[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int c = 8 * jj + cq + e;
             const int i = 4 * jj + 2 * r + e;
-            const float dl = DKV ? vec[64 + c] : my_delta[r];
+            const float dl = DKV ? vec[SR + c] : my_delta[r];
             // dP may be NaN at masked columns (DQ: V rows past the end of the sequence), where dS must be exactly 0
             const bool vis = (c >= vlo[r]) && (c <= vhi[r]);
             ds[e] = vis ? s[i] * (dp[i] - dl) : 0.f;
@@ -596,12 +619,12 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
           df[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(ds[0], ds[1]);
         }
       }
-      float(&acc_ds)[D / 2] = DKV ? acc2 : acc1;
+      float(&acc_ds)[DQK / 2] = pick<DKV>(acc2, acc1);
       wgmma_fence_regs(acc_ds);
       wgmma_fence();
       // DKV: dK += dS^T Q.  DQ: dQ += dS K
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) wgmma_bf16_rs<D, 1>(acc_ds, df[ks], desc_mnmajor(s1_addr, 64 * 128, ks), 1);
+      for (int ks = 0; ks < SR / 16; ++ks) wgmma_bf16_rs<DQK, 1>(acc_ds, df[ks], desc_mnmajor(s1_addr, SR * 128, ks), 1);
       wgmma_commit();
       wgmma_wait<0>();
       if (signal) mbar_arrive(&st_empty[st]);
@@ -614,18 +637,19 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
       const int ri = r0 + row_l + 8 * r;
       if (ri >= (DKV ? sq.Sk : sq.Sq)) continue;
       if constexpr (DKV) {
-        __nv_bfloat16* dv = p.dv + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * D + cq;
-        __nv_bfloat16* dk = p.dk + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * D + cq;
+        __nv_bfloat16* dv = p.dv + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * DV + cq;
+        __nv_bfloat16* dk = p.dk + (static_cast<long long>(sq.k_start + ri) * p.Hk + head) * DQK + cq;
 #pragma unroll
-        for (int jj = 0; jj < D / 8; ++jj) {
-          *reinterpret_cast<uint32_t*>(dv + 8 * jj) = pack_bf16x2(acc1[4 * jj + 2 * r], acc1[4 * jj + 2 * r + 1]);
+        for (int jj = 0; jj < DQK / 8; ++jj) {
+          if (jj < DV / 8)
+            *reinterpret_cast<uint32_t*>(dv + 8 * jj) = pack_bf16x2(acc1[4 * jj + 2 * r], acc1[4 * jj + 2 * r + 1]);
           *reinterpret_cast<uint32_t*>(dk + 8 * jj) =
               pack_bf16x2(acc2[4 * jj + 2 * r] * p.scale, acc2[4 * jj + 2 * r + 1] * p.scale);
         }
       } else {
-        __nv_bfloat16* dq = p.dq + (static_cast<long long>(sq.q_start + ri) * p.Hq + head) * D + cq;
+        __nv_bfloat16* dq = p.dq + (static_cast<long long>(sq.q_start + ri) * p.Hq + head) * DQK + cq;
 #pragma unroll
-        for (int jj = 0; jj < D / 8; ++jj)
+        for (int jj = 0; jj < DQK / 8; ++jj)
           *reinterpret_cast<uint32_t*>(dq + 8 * jj) = pack_bf16x2(acc1[4 * jj + 2 * r] * p.scale, acc1[4 * jj + 2 * r + 1] * p.scale);
       }
     }
@@ -633,19 +657,19 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
   if (stuck) __trap();
 }
 
-// delta[b, h, q] = sum_d dO[q, h, d] * O[q, h, d]   (D/8 lanes per (row, head), 16-byte loads)
-template <int D>
+// delta[b, h, q] = sum_d dO[q, h, d] * O[q, h, d] over the DV value columns   (DV/8 lanes per (row, head), 16-byte loads)
+template <int DV>
 __global__ void flash_attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ dout,
                                         float* __restrict__ delta, const int* __restrict__ cu_q, int B, int Sq, int Hq,
                                         long long total_rows, long long lse_bs, long long lse_hs) {
-  constexpr int LANES = D / 8;  // lanes cooperating on one (row, head)
+  constexpr int LANES = DV / 8;  // lanes cooperating on one (row, head)
   const long long gt = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long item = gt / LANES;
   const int sub = static_cast<int>(gt % LANES);
   const bool ok = item < total_rows * Hq;
   float acc = 0.f;
   if (ok) {
-    const uint4 a = *reinterpret_cast<const uint4*>(o + item * D + sub * 8), c = *reinterpret_cast<const uint4*>(dout + item * D + sub * 8);
+    const uint4 a = *reinterpret_cast<const uint4*>(o + item * DV + sub * 8), c = *reinterpret_cast<const uint4*>(dout + item * DV + sub * 8);
     const float2 a0 = unpack_bf16x2(a.x), a1 = unpack_bf16x2(a.y), a2 = unpack_bf16x2(a.z), a3 = unpack_bf16x2(a.w);
     const float2 c0 = unpack_bf16x2(c.x), c1 = unpack_bf16x2(c.y), c2 = unpack_bf16x2(c.z), c3 = unpack_bf16x2(c.w);
     acc = a0.x * c0.x + a0.y * c0.y + a1.x * c1.x + a1.y * c1.y + a2.x * c2.x + a2.y * c2.y + a3.x * c3.x + a3.y * c3.y;
@@ -732,17 +756,17 @@ FaParams make_params(const FlashAttnArgs& a) {
   return p;
 }
 
-template <int D>
+template <int DQK, int DV>
 void launch_fwd(const FlashAttnArgs& a, cudaStream_t stream) {
-  using C = FwdCfg<D>;
-  auto kern = flash_attn_fwd_kernel<D>;
+  using C = FwdCfg<DQK, DV>;
+  auto kern = flash_attn_fwd_kernel<DQK, DV>;
   static bool configured = false;
   if (!configured) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     configured = true;
   }
-  const CUtensorMap tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 128), tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 128),
-                    tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 128);
+  const CUtensorMap tq = make_tmap_rhd(a.q, a.total_q, a.Hq, DQK, 128), tk = make_tmap_rhd(a.k, a.total_k, a.Hk, DQK, 128),
+                    tv = make_tmap_rhd(a.v, a.total_k, a.Hk, DV, 128);
   FaParams p = make_params(a);
   p.out = static_cast<__nv_bfloat16*>(a.out);
   p.lse = a.lse;
@@ -750,16 +774,16 @@ void launch_fwd(const FlashAttnArgs& a, cudaStream_t stream) {
   check_launch("the forward kernel");
 }
 
-template <int D>
+template <int DV>
 void launch_delta(const FlashAttnArgs& a, cudaStream_t stream) {
-  const long long threads = a.total_q * a.Hq * (D / 8);
-  flash_attn_delta_kernel<D><<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(
+  const long long threads = a.total_q * a.Hq * (DV / 8);
+  flash_attn_delta_kernel<DV><<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(a.out), static_cast<const __nv_bfloat16*>(a.dout), a.delta, a.cu_q, a.B, a.Sq, a.Hq,
       a.total_q, static_cast<long long>(a.Hq) * a.Sq, a.cu_q != nullptr ? a.total_q : a.Sq);
   check_launch("the delta kernel");
 }
 
-template <int D>
+template <int DQK, int DV>
 void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
   FaParams p = make_params(a);
   p.lse = a.lse;
@@ -768,28 +792,28 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
   p.dk = static_cast<__nv_bfloat16*>(a.dk);
   p.dv = static_cast<__nv_bfloat16*>(a.dv);
   if (a.Sk > 0) {
-    using C = BwdCfg<D, true>;
-    auto kern = flash_attn_bwd_kernel<D, true>;
+    using C = BwdCfg<DQK, DV, true>;
+    auto kern = flash_attn_bwd_kernel<DQK, DV, true>;
     static bool configured = false;
     if (!configured) {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
       configured = true;
     }
-    const CUtensorMap tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 128), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 128),
-                      tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 64), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, D, 64);
+    const CUtensorMap tk = make_tmap_rhd(a.k, a.total_k, a.Hk, DQK, 128), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, DV, 128),
+                      tq = make_tmap_rhd(a.q, a.total_q, a.Hq, DQK, C::SR), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, DV, C::SR);
     kern<<<grid_1d(a.Sk, a.Hk, a.B), FA_THREADS, C::SMEM_BYTES, stream>>>(tk, tv, tq, tdo, p);
     check_launch("the dK/dV kernel");
   }
   if (a.Sq > 0) {
-    using C = BwdCfg<D, false>;
-    auto kern = flash_attn_bwd_kernel<D, false>;
+    using C = BwdCfg<DQK, DV, false>;
+    auto kern = flash_attn_bwd_kernel<DQK, DV, false>;
     static bool configured = false;
     if (!configured) {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
       configured = true;
     }
-    const CUtensorMap tq = make_tmap_rhd(a.q, a.total_q, a.Hq, D, 128), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, D, 128),
-                      tk = make_tmap_rhd(a.k, a.total_k, a.Hk, D, 64), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, D, 64);
+    const CUtensorMap tq = make_tmap_rhd(a.q, a.total_q, a.Hq, DQK, 128), tdo = make_tmap_rhd(a.dout, a.total_q, a.Hq, DV, 128),
+                      tk = make_tmap_rhd(a.k, a.total_k, a.Hk, DQK, C::SR), tv = make_tmap_rhd(a.v, a.total_k, a.Hk, DV, C::SR);
     kern<<<grid_1d(a.Sq, a.Hq, a.B), FA_THREADS, C::SMEM_BYTES, stream>>>(tq, tdo, tk, tv, p);
     check_launch("the dQ kernel");
   }
@@ -797,7 +821,10 @@ void launch_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
 
 void check_args(const FlashAttnArgs& a) {
   if (a.Hq % a.Hk != 0) throw std::runtime_error("d9d flash_attn: Hq must be a multiple of Hk");
-  if (a.D != 64 && a.D != 128) throw std::runtime_error("d9d flash_attn: head_dim must be 64 or 128");
+  const bool dims_ok = (a.Dqk == 64 && a.Dv == 64) || (a.Dqk == 128 && a.Dv == 128) || (a.Dqk == 192 && a.Dv == 128);
+  if (!dims_ok)
+    throw std::runtime_error("d9d flash_attn: (qk, v) head dims must be (64, 64), (128, 128) or (192, 128), got (" +
+                             std::to_string(a.Dqk) + ", " + std::to_string(a.Dv) + ")");
   if ((a.cu_q == nullptr) != (a.cu_k == nullptr)) throw std::runtime_error("d9d flash_attn: cu_seqlens_q and cu_seqlens_k go together");
 }
 
@@ -807,16 +834,17 @@ void flash_attn_fwd(const FlashAttnArgs& a, int variant, cudaStream_t stream) {
   if (a.B == 0 || a.Hq == 0 || a.total_q == 0) return;
   check_args(a);
   (void)variant;
-  if (a.cu_q != nullptr) zero_outside(a.out, nullptr, a.lse, a.cu_q, a.B, a.total_q, a.Hq * a.D, a.Hq, stream);
+  if (a.cu_q != nullptr) zero_outside(a.out, nullptr, a.lse, a.cu_q, a.B, a.total_q, a.Hq * a.Dv, a.Hq, stream);
   if (a.Sq == 0) return;
-  if (a.D == 64) launch_fwd<64>(a, stream);
-  else launch_fwd<128>(a, stream);
+  if (a.Dqk == 64) launch_fwd<64, 64>(a, stream);
+  else if (a.Dqk == 128) launch_fwd<128, 128>(a, stream);
+  else launch_fwd<192, 128>(a, stream);
 }
 
 void flash_attn_bwd_delta(const FlashAttnArgs& a, cudaStream_t stream) {
   if (a.B == 0 || a.Hq == 0 || a.total_q == 0) return;
   check_args(a);
-  if (a.D == 64) launch_delta<64>(a, stream);
+  if (a.Dv == 64) launch_delta<64>(a, stream);
   else launch_delta<128>(a, stream);
 }
 
@@ -824,16 +852,22 @@ void flash_attn_bwd(const FlashAttnArgs& a, cudaStream_t stream) {
   if (a.B == 0 || a.Hq == 0 || a.total_q == 0) return;
   check_args(a);
   if (a.total_k == 0) {  // no key anywhere: dq = 0
-    if (cudaMemsetAsync(a.dq, 0, static_cast<size_t>(a.total_q) * a.Hq * a.D * 2, stream) != cudaSuccess)
+    if (cudaMemsetAsync(a.dq, 0, static_cast<size_t>(a.total_q) * a.Hq * a.Dqk * 2, stream) != cudaSuccess)
       throw std::runtime_error("d9d flash_attn: cudaMemsetAsync failed");
     return;
   }
   if (a.cu_q != nullptr) {
-    zero_outside(a.dq, nullptr, nullptr, a.cu_q, a.B, a.total_q, a.Hq * a.D, 0, stream);
-    zero_outside(a.dk, a.dv, nullptr, a.cu_k, a.B, a.total_k, a.Hk * a.D, 0, stream);
+    zero_outside(a.dq, nullptr, nullptr, a.cu_q, a.B, a.total_q, a.Hq * a.Dqk, 0, stream);
+    if (a.Dqk == a.Dv) {
+      zero_outside(a.dk, a.dv, nullptr, a.cu_k, a.B, a.total_k, a.Hk * a.Dqk, 0, stream);
+    } else {  // dk and dv rows differ in width
+      zero_outside(a.dk, nullptr, nullptr, a.cu_k, a.B, a.total_k, a.Hk * a.Dqk, 0, stream);
+      zero_outside(a.dv, nullptr, nullptr, a.cu_k, a.B, a.total_k, a.Hk * a.Dv, 0, stream);
+    }
   }
-  if (a.D == 64) launch_bwd<64>(a, stream);
-  else launch_bwd<128>(a, stream);
+  if (a.Dqk == 64) launch_bwd<64, 64>(a, stream);
+  else if (a.Dqk == 128) launch_bwd<128, 128>(a, stream);
+  else launch_bwd<192, 128>(a, stream);
 }
 
 }  // namespace d9d
