@@ -1,4 +1,4 @@
-"""Native wgmma flash attention (forward, both P variants, and backward) vs PyTorch SDPA on cuDNN, flagship shapes; then
+"""Native wgmma flash attention (forward and backward) vs PyTorch SDPA on cuDNN, flagship shapes; then
 multi-head latent attention rows (qk head dim 192, v head dim 128): native, the SDPA path on V zero-padded to 192 (default
 backend selection, what non-native callers get) and cuDNN on the padded tensors.
 
@@ -47,13 +47,9 @@ for (B, S, Hq, Hk, D, causal) in shapes:
     flops = 4.0 * B * Hq * S * S * D * (0.5 if causal else 1.0)
     wr = 0 if causal else -1
     row = {"B": B, "S": S, "Hq": Hq, "Hk": Hk, "D": D, "causal": causal}
-    for variant, name in ((0, "native_fwd"),):
-        try:
-            t = timeit(lambda: ops.flash_attn_fwd(q, k, v, D ** -0.5, -1, wr, 0.0, None, None, None, 0, 0, variant))
-            row[name + "_ms"], row[name + "_tflops"] = t, flops / t / 1e9
-        except Exception as exc:  # noqa: BLE001
-            row[name + "_error"] = str(exc)[:200]
-    out, lse = ops.flash_attn_fwd(q, k, v, D ** -0.5, -1, wr, 0.0, None, None, None, 0, 0, 0)
+    t = timeit(lambda: ops.flash_attn_fwd(q, k, v, D ** -0.5, -1, wr, 0.0, None, None, None, 0, 0))
+    row["native_fwd_ms"], row["native_fwd_tflops"] = t, flops / t / 1e9
+    out, lse = ops.flash_attn_fwd(q, k, v, D ** -0.5, -1, wr, 0.0, None, None, None, 0, 0)
     t = timeit(lambda: ops.flash_attn_bwd(do, q, k, v, out, lse, D ** -0.5, -1, wr, 0.0, None, None, 0, 0, None))
     row["native_bwd_ms"], row["native_bwd_tflops"] = t, 2.5 * flops / t / 1e9
     qh, kh, vh = (x.transpose(1, 2).detach().requires_grad_() for x in (q, k, v))
@@ -84,8 +80,8 @@ for (B, S, H, causal) in mla_shapes:
     def put(name, t, flops):
         row[name + "_ms"], row[name + "_tflops"] = t, flops / t / 1e9
 
-    put("native_fwd", timeit(lambda: ops.flash_attn_fwd(q, k, v, sc, -1, wr, 0.0, None, None, None, 0, 0, 0)), fwd_flops)
-    out, lse = ops.flash_attn_fwd(q, k, v, sc, -1, wr, 0.0, None, None, None, 0, 0, 0)
+    put("native_fwd", timeit(lambda: ops.flash_attn_fwd(q, k, v, sc, -1, wr, 0.0, None, None, None, 0, 0)), fwd_flops)
+    out, lse = ops.flash_attn_fwd(q, k, v, sc, -1, wr, 0.0, None, None, None, 0, 0)
     put("native_bwd", timeit(lambda: ops.flash_attn_bwd(do, q, k, v, out, lse, sc, -1, wr, 0.0, None, None, 0, 0, None)), bwd_flops)
     qh, kh, vh = (x.transpose(1, 2).detach().requires_grad_() for x in (q, k, v))
     doh = do.transpose(1, 2)

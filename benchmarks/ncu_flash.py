@@ -13,6 +13,6 @@ q = torch.randn(B, S, Hq, D, device="cuda").bfloat16()
 k = torch.randn(B, S, Hk, D, device="cuda").bfloat16()
 v = torch.randn_like(k)
 for _ in range(2):
-    out, lse = ops.flash_attn_fwd(q, k, v, D ** -0.5, -1, 0, 0.0, None, None, None, 0, 0, 0)
+    out, lse = ops.flash_attn_fwd(q, k, v, D ** -0.5, -1, 0, 0.0, None, None, None, 0, 0)
     ops.flash_attn_bwd(torch.randn_like(q), q, k, v, out, lse, D ** -0.5, -1, 0, 0.0, None, None, 0, 0, None)
 torch.cuda.synchronize()

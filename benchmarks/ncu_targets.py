@@ -59,7 +59,7 @@ def main() -> None:
     q = torch.randn(B, S, Hq, D, **bf)
     kk = torch.randn(B, S, Hk, D, **bf)
     vv = torch.randn(B, S, Hk, D, **bf)
-    out, lse = ops.flash_attn_fwd(q, kk, vv, D ** -0.5, -1, 0, 0.0, None, None, None, 0, 0, 0)
+    out, lse = ops.flash_attn_fwd(q, kk, vv, D ** -0.5, -1, 0, 0.0, None, None, None, 0, 0)
     ops.flash_attn_bwd(torch.randn_like(q), q, kk, vv, out, lse, D ** -0.5, -1, 0, 0.0, None, None, 0, 0, None)
     # 10) fused q/k RMSNorm + RoPE, 11) router
     wqn = torch.ones(D, **bf)

@@ -50,7 +50,7 @@ def main() -> None:
     q = torch.randn(B, S, Hq, D, **bf)
     kk = torch.randn(B, S, Hk, D, **bf)
     vv = torch.randn(B, S, Hk, D, **bf)
-    out, lse = ops.flash_attn_fwd(q, kk, vv, D ** -0.5, -1, 0, 0.0, None, None, None, 0, 0, 0)
+    out, lse = ops.flash_attn_fwd(q, kk, vv, D ** -0.5, -1, 0, 0.0, None, None, None, 0, 0)
     ops.flash_attn_bwd(torch.randn_like(q), q, kk, vv, out, lse, D ** -0.5, -1, 0, 0.0, None, None, 0, 0, None)
     torch.cuda.synchronize()
 

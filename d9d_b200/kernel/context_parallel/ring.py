@@ -225,7 +225,7 @@ def _attend_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: fl
         from d9d_b200.kernel._native import native_ops
 
         out, lse = native_ops().flash_attn_fwd(q.contiguous(), k.contiguous(), v.contiguous(), scale, -1, 0 if mode == _CAUSAL else -1,
-                                               0.0, None, None, None, 0, 0, 0)
+                                               0.0, None, None, None, 0, 0)
         return out, lse
     from d9d_b200.kernel.flash_attn.function import attention_reference
 

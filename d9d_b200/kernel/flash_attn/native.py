@@ -44,7 +44,7 @@ class _NativeFlashAttention(torch.autograd.Function):
         ops = native_ops()
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         sink32 = sink.detach().float().contiguous() if sink is not None else None
-        out, lse = ops.flash_attn_fwd(q, k, v, scale, wl, wr, softcap, sink32, cu_q, cu_k, max_q, max_k, 0)
+        out, lse = ops.flash_attn_fwd(q, k, v, scale, wl, wr, softcap, sink32, cu_q, cu_k, max_q, max_k)
         ctx.save_for_backward(q, k, v, out, lse, sink, cu_q, cu_k)
         ctx.cfg = (scale, wl, wr, softcap, max_q, max_k)
         return out, lse

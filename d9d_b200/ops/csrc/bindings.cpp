@@ -553,14 +553,14 @@ static Tensor fa_stats_like(const d9d::FlashAttnArgs& a, const Tensor& q) {
 std::tuple<Tensor, Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, double scale, int64_t window_left,
                                           int64_t window_right, double softcap, const c10::optional<Tensor>& sink,
                                           const c10::optional<Tensor>& cu_q, const c10::optional<Tensor>& cu_k, int64_t max_q,
-                                          int64_t max_k, int64_t variant) {
+                                          int64_t max_k) {
   c10::cuda::CUDAGuard guard(q.device());
   d9d::FlashAttnArgs a = fa_args(q, k, v, scale, window_left, window_right, softcap, sink, cu_q, cu_k, max_q, max_k);
   Tensor out = at::empty(fa_out_shape(a, q), q.options());
   Tensor lse = fa_stats_like(a, q);
   a.out = out.data_ptr();
   a.lse = lse.data_ptr<float>();
-  d9d::flash_attn_fwd(a, static_cast<int>(variant), cur_stream());
+  d9d::flash_attn_fwd(a, cur_stream());
   return {out, lse};
 }
 
@@ -861,7 +861,7 @@ TORCH_LIBRARY(d9d_b200, m) {
   m.def("moe_gather(Tensor yp, Tensor? dpp, Tensor row_map, int T, int k) -> (Tensor, Tensor)");
   m.def("sumsq_accumulate_(Tensor x, Tensor(a!) out) -> ()");
   m.def("moe_zero_pad(Tensor(a!) xp, Tensor? pp, Tensor counts, Tensor seg_offsets) -> ()");
-  m.def("flash_attn_fwd(Tensor q, Tensor k, Tensor v, float scale, int window_left, int window_right, float softcap, Tensor? sink, Tensor? cu_q, Tensor? cu_k, int max_q, int max_k, int variant) -> (Tensor, Tensor)");
+  m.def("flash_attn_fwd(Tensor q, Tensor k, Tensor v, float scale, int window_left, int window_right, float softcap, Tensor? sink, Tensor? cu_q, Tensor? cu_k, int max_q, int max_k) -> (Tensor, Tensor)");
   m.def("flash_attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor out, Tensor lse, float scale, int window_left, int window_right, float softcap, Tensor? cu_q, Tensor? cu_k, int max_q, int max_k, Tensor? dlse) -> (Tensor, Tensor, Tensor, Tensor)");
   m.def("qk_norm_rope_fwd(Tensor q, Tensor k, Tensor wq, Tensor wk, Tensor cos_t, Tensor sin_t, float eps, bool zero_centered, "
         "int style) -> (Tensor, Tensor, Tensor)");

@@ -181,9 +181,7 @@ struct FlashAttnArgs {
   int window_left, window_right;
   float scale, softcap;
 };
-// variant: reserved and ignored (there is one forward: P stays in registers as the A operand of the PV wgmma, as P^T / dS^T
-// do in the backward kernels)
-void flash_attn_fwd(const FlashAttnArgs& a, int variant, cudaStream_t stream);
+void flash_attn_fwd(const FlashAttnArgs& a, cudaStream_t stream);
 // backward = delta pre-pass (delta[b,h,q] = sum_d dO*O, written to a.delta) followed by the dK/dV and dQ kernels (which read
 // a.delta; the caller may subtract d(lse) from it in between)
 void flash_attn_bwd_delta(const FlashAttnArgs& a, cudaStream_t stream);

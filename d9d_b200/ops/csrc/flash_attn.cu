@@ -830,10 +830,9 @@ void check_args(const FlashAttnArgs& a) {
 
 }  // namespace
 
-void flash_attn_fwd(const FlashAttnArgs& a, int variant, cudaStream_t stream) {
+void flash_attn_fwd(const FlashAttnArgs& a, cudaStream_t stream) {
   if (a.B == 0 || a.Hq == 0 || a.total_q == 0) return;
   check_args(a);
-  (void)variant;
   if (a.cu_q != nullptr) zero_outside(a.out, nullptr, a.lse, a.cu_q, a.B, a.total_q, a.Hq * a.Dv, a.Hq, stream);
   if (a.Sq == 0) return;
   if (a.Dqk == 64) launch_fwd<64, 64>(a, stream);

@@ -5,15 +5,18 @@ Visibility (``d9d_ops.h``): key k of a sequence sees query q iff q + off - wl <=
 negative wl / wr is unbounded.  Scores x = scale q.k, or cap tanh(scale q.k / cap) with a soft-cap; an optional per-head
 sink joins the softmax denominator.
 
+q and k have Dqk columns, v and out Dv (multi-head latent attention runs at (192, 128)); dq and dk have Dqk columns, dv Dv.
+Each sum over a head dim below runs over its own width.
+
 Error sources of the kernels, all taken from the tensors actually passed to them:
 
-* S = Q K^T accumulates over D in fp32:  |dx_ij| <= scale c_k(D) |q_i|.|k_j|;  fast tanh adds cap 2^-10.9,
+* S = Q K^T accumulates over Dqk in fp32:  |dx_ij| <= scale c_k(Dqk) |q_i|.|k_j|;  fast tanh adds cap 2^-10.9,
   and the log2-domain arithmetic / ex2 a few fp32 ulps of |x| and of the row max.  eps_i is the largest of these over the
   visible keys of row i; P_ij = exp(x_ij - lse_i) is then off by at most exp(2 eps_i) relatively (forward).
 * P (and dS) are rounded to bf16 before they enter the second GEMM, whose fp32 accumulation runs over Sk (forward, dQ) or
   g Sq (dK / dV, g = Hq / Hk).
-* The backward recomputes P from the forward's lse, so the lse bound joins eps_i there; dP = dO V^T accumulates over D;
-  Delta = dO.O - dlse is taken from the bf16 O the backward is given.
+* The backward recomputes P from the forward's lse, so the lse bound joins eps_i there; dP = dO V^T accumulates over
+  Dv; Delta = dO.O - dlse, also over Dv, is taken from the bf16 O the backward is given.
 * Every bf16 output is rounded once more (2^-8 relative).  Results below 2^-100 may flush to zero.
 """
 
@@ -57,14 +60,14 @@ def _group_sum(x: torch.Tensor, Hk: int) -> torch.Tensor:
 
 def sequence_reference(q, k, v, *, scale: float, wl: int = -1, wr: int = -1, softcap: float = 0.0, sink=None, out=None,
                        dout=None, dlse=None, chunk: int = 1024) -> dict[str, tuple[torch.Tensor, torch.Tensor]]:
-    """(reference, bound) per output for one sequence: q [Sq, Hq, D], k / v [Sk, Hk, D], sink [Hq] or None.
+    """(reference, bound) per output for one sequence: q [Sq, Hq, Dqk], k [Sk, Hk, Dqk], v [Sk, Hk, Dv], sink [Hq] or None.
 
-    Always ``out`` [Sq, Hq, D] and ``lse`` [Hq, Sq] (-inf where a row sees no key and there is no sink).  With ``dout``
+    Always ``out`` [Sq, Hq, Dv] and ``lse`` [Hq, Sq] (-inf where a row sees no key and there is no sink).  With ``dout``
     (and the bf16 ``out`` the backward is given, optional ``dlse`` [Hq, Sq]) also ``dq``, ``dk``, ``dv`` and, with a sink,
     ``dsink`` [Hq] (its fp32 sum over the whole batch is bounded by :func:`batch_reference`).  Rows are processed
     ``chunk`` queries at a time, so long sequences fit in memory."""
-    Sq, Hq, D = q.shape
-    Sk, Hk = k.shape[0], k.shape[1]
+    Sq, Hq, Dqk = q.shape
+    Sk, Hk, Dv = k.shape[0], k.shape[1], v.shape[2]
     dev = q.device
     kf, vf = _heads(k, Hq), _heads(v, Hq)
     kabs, vabs = kf.abs(), vf.abs()
@@ -74,16 +77,17 @@ def sequence_reference(q, k, v, *, scale: float, wl: int = -1, wr: int = -1, sof
     bwd = dout is not None
     res = {n: [] for n in ("out", "out_b", "lse", "lse_b", "dq", "dq_b")}
     if bwd:
-        dk, dk_b, dv, dv_b = (torch.zeros(Hq, Sk, D, dtype=torch.float64, device=dev) for _ in range(4))
+        dk, dk_b = (torch.zeros(Hq, Sk, Dqk, dtype=torch.float64, device=dev) for _ in range(2))
+        dv, dv_b = (torch.zeros(Hq, Sk, Dv, dtype=torch.float64, device=dev) for _ in range(2))
         dsink = torch.zeros(Hq, dtype=torch.float64, device=dev)
         dsink_b = torch.zeros(Hq, dtype=torch.float64, device=dev)
         dsink_abs = torch.zeros(Hq, dtype=torch.float64, device=dev)
     for i0 in range(0, Sq, chunk):
         i1 = min(Sq, i0 + chunk)
         keep = keep_all[i0:i1][None]                       # [1, n, Sk]
-        qf = q[i0:i1].double().permute(1, 0, 2)            # [Hq, n, D]
+        qf = q[i0:i1].double().permute(1, 0, 2)            # [Hq, n, Dqk]
         s = scale * (qf @ kf.transpose(1, 2))
-        s_err = scale * ck(D) * (qf.abs() @ kabs.transpose(1, 2))
+        s_err = scale * ck(Dqk) * (qf.abs() @ kabs.transpose(1, 2))
         if softcap:
             t = torch.tanh(s / softcap)
             x = softcap * t
@@ -117,13 +121,13 @@ def sequence_reference(q, k, v, *, scale: float, wl: int = -1, wr: int = -1, sof
         do = dout[i0:i1].double().permute(1, 0, 2)
         ob = out[i0:i1].double().permute(1, 0, 2)
         delta = (do * ob).sum(-1, keepdim=True)
-        delta_err = ck(D) * (do.abs() * ob.abs()).sum(-1, keepdim=True) + 2 * U_F32 * delta.abs()
+        delta_err = ck(Dv) * (do.abs() * ob.abs()).sum(-1, keepdim=True) + 2 * U_F32 * delta.abs()
         if dlse is not None:
             dl = dlse[:, i0:i1].double()[..., None]
             delta = delta - dl
             delta_err = delta_err + 2 * U_F32 * (delta.abs() + dl.abs())
         dp = do @ vf.transpose(1, 2)
-        dp_err = ck(D) * (do.abs() @ vabs.transpose(1, 2))
+        dp_err = ck(Dv) * (do.abs() @ vabs.transpose(1, 2))
         dpd = dp - delta
         eta_b = torch.expm1(eps + torch.where(torch.isfinite(lse), lse_b, 0.0)) + ULP_MATH  # P recomputed from the lse
         cap_d = (1 - t * t) if softcap else 1.0
@@ -163,19 +167,19 @@ def sequence_reference(q, k, v, *, scale: float, wl: int = -1, wr: int = -1, sof
 
 
 def batch_reference(q, k, v, cu_q: list[int], cu_k: list[int], **kw) -> dict[str, tuple[torch.Tensor, torch.Tensor]]:
-    """:func:`sequence_reference` over a packed batch: q [total_q, Hq, D], k / v [total_k, Hk, D], sequence b = rows
-    [cu_q[b], cu_q[b+1]) / [cu_k[b], cu_k[b+1]).  lse is [Hq, total_q].  Rows outside every sequence must be exactly 0
-    (lse: -inf).  ``out`` / ``dlse`` (packed like q / lse) are sliced per sequence."""
-    total_q, Hq, D = q.shape
-    total_k, Hk = k.shape[0], k.shape[1]
+    """:func:`sequence_reference` over a packed batch: q [total_q, Hq, Dqk], k [total_k, Hk, Dqk], v [total_k, Hk, Dv],
+    sequence b = rows [cu_q[b], cu_q[b+1]) / [cu_k[b], cu_k[b+1]).  lse is [Hq, total_q].  Rows outside every sequence must
+    be exactly 0 (lse: -inf).  ``out`` / ``dlse`` (packed like q / lse) are sliced per sequence."""
+    total_q, Hq, Dqk = q.shape
+    total_k, Hk, Dv = k.shape[0], k.shape[1], v.shape[2]
     dev = q.device
     z = lambda *shape: torch.zeros(*shape, dtype=torch.float64, device=dev)  # noqa: E731
     bwd = kw.get("dout") is not None
-    acc = {"out": [z(total_q, Hq, D), z(total_q, Hq, D)], "lse": [torch.full((Hq, total_q), -math.inf, dtype=torch.float64, device=dev),
-                                                                   z(Hq, total_q)]}
+    acc = {"out": [z(total_q, Hq, Dv), z(total_q, Hq, Dv)], "lse": [torch.full((Hq, total_q), -math.inf, dtype=torch.float64, device=dev),
+                                                                     z(Hq, total_q)]}
     if bwd:
-        acc.update(dq=[z(total_q, Hq, D), z(total_q, Hq, D)], dk=[z(total_k, Hk, D), z(total_k, Hk, D)],
-                   dv=[z(total_k, Hk, D), z(total_k, Hk, D)])
+        acc.update(dq=[z(total_q, Hq, Dqk), z(total_q, Hq, Dqk)], dk=[z(total_k, Hk, Dqk), z(total_k, Hk, Dqk)],
+                   dv=[z(total_k, Hk, Dv), z(total_k, Hk, Dv)])
         if kw.get("sink") is not None:
             acc.update(dsink=[z(Hq), z(Hq)], dsink_abs=[z(Hq), z(Hq)])
     for b in range(len(cu_q) - 1):
@@ -208,13 +212,13 @@ def batch_reference(q, k, v, cu_q: list[int], cu_k: list[int], **kw) -> dict[str
 
 
 def fixed_reference(q, k, v, **kw) -> dict[str, tuple[torch.Tensor, torch.Tensor]]:
-    """:func:`sequence_reference` over a fixed-length batch, q [B, Sq, Hq, D], k / v [B, Sk, Hk, D], lse / dlse
-    [B, Hq, Sq]: the batch is folded into the heads (head b Hq + h reads kv head b Hk + h // g), so that many short
-    sequences cost one call."""
-    B, Sq, Hq, D = q.shape
+    """:func:`sequence_reference` over a fixed-length batch, q [B, Sq, Hq, Dqk], k [B, Sk, Hk, Dqk], v [B, Sk, Hk, Dv],
+    lse / dlse [B, Hq, Sq]: the batch is folded into the heads (head b Hq + h reads kv head b Hk + h // g), so that many
+    short sequences cost one call."""
+    B, Sq, Hq = q.shape[:3]
     Sk, Hk = k.shape[1], k.shape[2]
-    fold = lambda x, S, H: x.permute(1, 0, 2, 3).reshape(S, B * H, D)  # noqa: E731
-    unfold = lambda x, S, H: x.reshape(S, B, H, D).permute(1, 0, 2, 3)  # noqa: E731
+    fold = lambda x, S, H: x.permute(1, 0, 2, 3).reshape(S, B * H, x.shape[-1])  # noqa: E731
+    unfold = lambda x, S, H: x.reshape(S, B, H, x.shape[-1]).permute(1, 0, 2, 3)  # noqa: E731
     kws = dict(kw)
     if kws.get("sink") is not None:
         kws["sink"] = kws["sink"].repeat(B)
@@ -254,18 +258,21 @@ def assert_lse_within(got, ref, bound, what: str = "lse") -> float:
     return r
 
 
-def make_inputs(Sq: int, Sk: int, Hq: int, Hk: int, D: int, *, scale: float, peak: float = 20.0, ramp: float = 8.0, B=None,
-                gen: torch.Generator | None = None, device="cpu"):
-    """bf16 (q, k, v, dout) as [S, H, D] (or [B, S, H, D]).  Scores reach about +-peak, so that soft-caps of 5 to 10 bend
-    them and P is far from uniform, and every row's score rises by about ``ramp`` from the first key to the last, so the
-    running max of the online softmax moves from one key tile to the next."""
+def make_inputs(Sq: int, Sk: int, Hq: int, Hk: int, Dqk: int, Dv: int | None = None, *, scale: float, peak: float = 20.0,
+                ramp: float = 8.0, B=None, gen: torch.Generator | None = None, device="cpu"):
+    """bf16 (q, k, v, dout) as [S, H, D] (or [B, S, H, D]): q / k with Dqk columns, v / dout with Dv (default Dqk).  Scores
+    reach about +-peak, so that soft-caps of 5 to 10 bend them and P is far from uniform, and every row's score rises by
+    about ``ramp`` from the first key to the last, so the running max of the online softmax moves from one key tile to the
+    next.  v / dout are the first Dv columns of the Dqk-wide draws, so a given seed yields the same q and k at every Dv."""
+    Dv = Dqk if Dv is None else Dv
     lead = () if B is None else (B,)
-    a = math.sqrt(peak / 3.0 / (scale * math.sqrt(D)))
-    q = torch.randn(*lead, Sq, Hq, D, generator=gen) * a
-    k = torch.randn(*lead, Sk, Hk, D, generator=gen) * a
-    v = torch.randn(*lead, Sk, Hk, D, generator=gen)
-    dout = torch.randn(*lead, Sq, Hq, D, generator=gen)
+    a = math.sqrt(peak / 3.0 / (scale * math.sqrt(Dqk)))
+    q = torch.randn(*lead, Sq, Hq, Dqk, generator=gen) * a
+    k = torch.randn(*lead, Sk, Hk, Dqk, generator=gen) * a
+    v = torch.randn(*lead, Sk, Hk, Dqk, generator=gen)
+    dout = torch.randn(*lead, Sq, Hq, Dqk, generator=gen)
     c = math.sqrt(ramp / scale)
     q[..., 0] += c
     k[..., 0] += c * (torch.arange(Sk) / max(Sk - 1, 1)).view(*((1,) * len(lead)), Sk, 1)
-    return tuple(t.bfloat16().to(device) for t in (q, k, v, dout))
+    q, k, v, dout = (t.bfloat16().to(device) for t in (q, k, v, dout))
+    return q, k, v[..., :Dv].contiguous(), dout[..., :Dv].contiguous()

@@ -1,6 +1,7 @@
 """Self-test of the fp64 reference / error bound that the flash attention kernel tests rely on: an fp32 emulation of the
 kernels' algorithm must pass it, and each fault a broken kernel could have must exceed it, at the shapes and inputs the
-GPU tests use."""
+GPU tests use: equal head dims 64 and 128, and separate qk and v head dims (192, 128), where a kernel has more ways to
+mix up the two widths."""
 
 import math
 
@@ -13,14 +14,27 @@ from tests.gemm_reference import err_ratio
 L2E = math.log2(math.e)
 
 
+def _pitch(x: torch.Tensor, pitch: int) -> torch.Tensor:
+    """[S, H, Dv] read as if its rows were ``pitch`` elements apart (past the end of the buffer: zeros)."""
+    S, H, Dv = x.shape
+    flat = torch.zeros(S * H * pitch, dtype=x.dtype)
+    flat[: x.numel()] = x.reshape(-1)
+    return flat.view(S, H, pitch)[..., :Dv]
+
+
 def emulate(q, k, v, *, scale, wl=-1, wr=-1, softcap=0.0, sink=None, dout=None, dlse=None, fault=None):
-    """fp32 emulation of one sequence through the kernels: 128-key tiles with an online softmax in the log2 domain, P
-    rounded to bf16 for O += P V, the sink folded into the max at the end; backward with P recomputed from the lse, Delta
-    from the bf16 O, dS rounded to bf16, fp32 accumulation of dQ / dK / dV.  ``fault`` injects one bug."""
-    Sq, Hq, D = q.shape
-    Sk, Hk = k.shape[0], k.shape[1]
+    """fp32 emulation of one sequence through the kernels with q / k [S, H, Dqk] and v / dout [S, H, Dv]: 128-key tiles
+    with an online softmax in the log2 domain, P rounded to bf16 for O += P V, the sink folded into the max at the end;
+    backward with P recomputed from the lse, Delta from the bf16 O over the Dv columns, dS rounded to bf16, fp32
+    accumulation of dQ / dK (Dqk columns) and dV (Dv columns).  ``fault`` injects one bug."""
+    Sq, Hq, Dqk = q.shape
+    Sk, Hk, Dv = k.shape[0], k.shape[1], v.shape[2]
     g = Hq // Hk
     hmap = torch.arange(Hq) % Hk if fault == "gqa_mod" else torch.arange(Hq) // g
+    if fault == "v_pitch":
+        v = _pitch(v, Dqk)
+    if fault == "do_pitch" and dout is not None:
+        dout = _pitch(dout, Dqk)
     qf = q.float().permute(1, 0, 2)
     kf, vf = k.float().permute(1, 0, 2)[hmap], v.float().permute(1, 0, 2)[hmap]
     keep = visible(Sq, Sk, wl + (fault == "left"), wr + (fault == "right"))
@@ -28,7 +42,7 @@ def emulate(q, k, v, *, scale, wl=-1, wr=-1, softcap=0.0, sink=None, dout=None, 
         keep &= torch.arange(Sk)[None] < torch.arange(Sq)[:, None] + (Sk - Sq)
     if fault == "last_key":
         keep[:, Sk - 1] = False
-    s = qf @ kf.transpose(1, 2)
+    s = qf[..., : Dqk - 64] @ kf[..., : Dqk - 64].transpose(1, 2) if fault == "no_rope" else qf @ kf.transpose(1, 2)
     if softcap:
         t = torch.tanh(s * (scale / softcap))
         x = softcap * t * L2E
@@ -37,7 +51,7 @@ def emulate(q, k, v, *, scale, wl=-1, wr=-1, softcap=0.0, sink=None, dout=None, 
     x = x.masked_fill(~keep, -math.inf)
     m = torch.full((Hq, Sq, 1), -math.inf)
     l = torch.zeros(Hq, Sq, 1)
-    o = torch.zeros(Hq, Sq, D)
+    o = torch.zeros(Hq, Sq, Dv)
     for j in range(0, Sk, 128):
         if fault == "skip_tile" and j == 128:
             continue
@@ -64,7 +78,8 @@ def emulate(q, k, v, *, scale, wl=-1, wr=-1, softcap=0.0, sink=None, dout=None, 
     if dout is None:
         return res
     do = dout.float().permute(1, 0, 2)
-    delta = (do * out.float()).sum(-1, keepdim=True)
+    n_delta = 64 if fault == "delta_64" else Dv
+    delta = (do[..., :n_delta] * out.float()[..., :n_delta]).sum(-1, keepdim=True)
     if dlse is not None and fault != "dlse_ignored":
         delta = delta - dlse.float()[..., None]
     lse2 = torch.where(lse == -math.inf, math.inf, lse * L2E)
@@ -75,35 +90,38 @@ def emulate(q, k, v, *, scale, wl=-1, wr=-1, softcap=0.0, sink=None, dout=None, 
         ds = ds * (1 - t * t)
     pb, dsb = p.bfloat16().float(), ds.bfloat16().float()
     dk_scale = 1.0 if fault == "dk_unscaled" else scale
-    dq = (scale * (dsb @ kf)).bfloat16()
+    dq = scale * (dsb @ kf)
     dk_h, dv_h = dsb.transpose(1, 2) @ qf, pb.transpose(1, 2) @ do
-    dk = torch.zeros(Hk, Sk, D).index_add_(0, hmap, dk_h) * dk_scale
-    dv = torch.zeros(Hk, Sk, D).index_add_(0, hmap, dv_h)
-    res.update(dq=dq.permute(1, 0, 2), dk=dk.bfloat16().permute(1, 0, 2), dv=dv.bfloat16().permute(1, 0, 2))
+    dk = torch.zeros(Hk, Sk, Dqk).index_add_(0, hmap, dk_h) * dk_scale
+    dv = torch.zeros(Hk, Sk, Dv).index_add_(0, hmap, dv_h)
+    if fault == "dq_partial":
+        dq[..., Dv:] = 0.0
+    if fault == "dk_partial":
+        dk[..., Dv:] = 0.0
+    res.update(dq=dq.bfloat16().permute(1, 0, 2), dk=dk.bfloat16().permute(1, 0, 2), dv=dv.bfloat16().permute(1, 0, 2))
     if sink is not None:
         ps = torch.where(lse == -math.inf, 0.0, torch.exp(sink.float().view(Hq, 1, 1) - lse))
         res["dsink"] = -(ps * delta).sum((1, 2))
     return res
 
 
-def _ratios(got, ref):
-    r = {}
-    for name, (want, bound) in ref.items():
-        r[name] = lse_err_ratio(got[name], want, bound) if name == "lse" else err_ratio(got[name], want, bound)
-    return r
-
-
-def _run(Sq, Sk, Hq, Hk, D, *, wl=-1, wr=-1, softcap=0.0, sink=None, with_dlse=False, fault=None, seed=0):
-    scale = 1.0 / math.sqrt(D)
+def _run(Sq, Sk, Hq, Hk, Dqk, Dv, *, wl=-1, wr=-1, softcap=0.0, sink=None, with_dlse=False, fault=None, seed=0):
+    scale = 1.0 / math.sqrt(Dqk)
     gen = torch.Generator().manual_seed(seed)
-    q, k, v, dout = make_inputs(Sq, Sk, Hq, Hk, D, scale=scale, gen=gen)
+    q, k, v, dout = make_inputs(Sq, Sk, Hq, Hk, Dqk, Dv, scale=scale, gen=gen)
     sink_t = None if sink is None else torch.tensor(sink, dtype=torch.float32)
     dlse = torch.randn(Hq, Sq, generator=gen) if with_dlse else None
     kw = dict(scale=scale, wl=wl, wr=wr, softcap=softcap, sink=sink_t)
     got = emulate(q, k, v, dout=dout, dlse=dlse, fault=fault, **kw)
     ref = batch_reference(q, k, v, [0, Sq], [0, Sk], out=got["out"], dout=dout, dlse=dlse, **kw)
-    return _ratios(got, ref)
+    r = {}
+    for name, (want, bound) in ref.items():
+        assert got[name].shape == want.shape, (name, got[name].shape, want.shape)
+        r[name] = lse_err_ratio(got[name], want, bound) if name == "lse" else err_ratio(got[name], want, bound)
+    return r
 
+
+MLA = (192, 128)  # (Dqk, Dv) of multi-head latent attention
 
 ACCEPT = [
     # Sq, Sk, Hq, Hk, D, wl, wr, softcap, sink, dlse
@@ -116,9 +134,12 @@ ACCEPT = [
 ]
 
 
+@pytest.mark.parametrize("dims", [None, MLA], ids=["D", "192-128"])
 @pytest.mark.parametrize("Sq,Sk,Hq,Hk,D,wl,wr,softcap,sink,dlse", ACCEPT)
-def test_accepts_kernel_emulation(Sq, Sk, Hq, Hk, D, wl, wr, softcap, sink, dlse):
-    r = _run(Sq, Sk, Hq, Hk, D, wl=wl, wr=wr, softcap=softcap, sink=sink, with_dlse=dlse)
+def test_accepts_kernel_emulation(Sq, Sk, Hq, Hk, D, wl, wr, softcap, sink, dlse, dims):
+    """Each case at its listed head dim D = Dqk = Dv, and at (192, 128)."""
+    Dqk, Dv = dims or (D, D)
+    r = _run(Sq, Sk, Hq, Hk, Dqk, Dv, wl=wl, wr=wr, softcap=softcap, sink=sink, with_dlse=dlse)
     assert all(x <= 1.0 for x in r.values()), r
 
 
@@ -135,14 +156,35 @@ FAULTS = [
     ("no_rescale", dict()),
     ("gqa_mod", dict()),
 ]
+UNEQUAL_DIMS_FAULTS = [
+    ("no_rope", dict()),          # S without the last 64-column box of Q and K
+    ("v_pitch", dict()),          # V read at the Dqk row pitch
+    ("do_pitch", dict()),         # dO read at the Dqk row pitch
+    ("delta_64", dict()),         # Delta summed over the first 64 of the Dv columns
+    ("dk_partial", dict()),       # dK written for the first Dv columns only
+    ("dq_partial", dict()),       # dQ written for the first Dv columns only
+]
+FAULT_CASES = ([(f, kw, (D, D)) for D in (64, 128) for f, kw in FAULTS]
+               + [(f, kw, MLA) for f, kw in UNEQUAL_DIMS_FAULTS + FAULTS])
 
 
-@pytest.mark.parametrize("D", [64, 128])
-@pytest.mark.parametrize("fault,kw", FAULTS, ids=[f for f, _ in FAULTS])
-def test_rejects_fault(fault, kw, D):
-    assert max(_run(257, 257, 4, 2, D, **kw).values()) <= 1.0  # the same case without the fault passes
-    r = _run(257, 257, 4, 2, D, fault=fault, **kw)
+@pytest.mark.parametrize("fault,kw,dims", FAULT_CASES,
+                         ids=[f"{f}-{dqk}" if dqk == dv else f"{f}-{dqk}-{dv}" for f, _, (dqk, dv) in FAULT_CASES])
+def test_rejects_fault(fault, kw, dims):
+    assert max(_run(257, 257, 4, 2, *dims, **kw).values()) <= 1.0  # the same case without the fault passes
+    r = _run(257, 257, 4, 2, *dims, fault=fault, **kw)
     assert max(r.values()) > 1.0, r
+
+
+def test_reference_shapes_follow_each_head_dim():
+    """out / dv take the v head dim, dq / dk the qk head dim, packed and fixed-length alike."""
+    gen = torch.Generator().manual_seed(1)
+    q, k, v, dout = make_inputs(20, 24, 4, 2, *MLA, scale=0.1, B=2, gen=gen)
+    assert v.shape == (2, 24, 2, 128) and dout.shape == (2, 20, 4, 128)
+    out = torch.zeros(2, 20, 4, 128).bfloat16()
+    f = fixed_reference(q, k, v, scale=0.1, wr=0, out=out, dout=dout)
+    assert f["out"][0].shape == (2, 20, 4, 128) and f["dv"][0].shape == (2, 24, 2, 128)
+    assert f["dq"][0].shape == (2, 20, 4, 192) and f["dk"][0].shape == (2, 24, 2, 192)
 
 
 def test_fixed_batch_folds_into_heads():
