@@ -81,7 +81,8 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
                : "memory");
 }
 
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+// bar: shared-window address of the mbarrier
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
       "{\n\t"
@@ -90,9 +91,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       "selp.b32 %0, 1, 0, P;\n\t"
       "}\n"
       : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
+      : "r"(bar), "r"(parity)
       : "memory");
   return ok != 0;
+}
+
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+  return mbar_try_wait(smem_u32(bar), parity);
 }
 
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
@@ -128,7 +133,7 @@ __device__ __forceinline__ void mbar_wait_wg(uint64_t* bar, uint32_t parity) {
 // Same wait for warps that raised their register budget with setmaxnreg.inc: a trap anywhere in such a region makes ptxas
 // allocate all of it under the launch bound's cap (168 registers at 384 threads), with spills and serialised wgmma.  A
 // timeout sets `stuck` and every later wait returns at once; the caller traps after the region ends.
-__device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, bool& stuck) {
+__device__ __forceinline__ void mbar_wait_flag(uint32_t bar, uint32_t parity, bool& stuck) {
 #if D9D_WATCHDOG
   uint32_t spins = 0;
   while (!stuck && !mbar_try_wait(bar, parity)) {
@@ -138,6 +143,10 @@ __device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, b
   while (!mbar_try_wait(bar, parity)) {
   }
 #endif
+}
+
+__device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, bool& stuck) {
+  mbar_wait_flag(smem_u32(bar), parity, stuck);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -296,14 +305,17 @@ __device__ __forceinline__ void tma_load_3d_multicast(void* smem_dst, const void
       : "memory");
 }
 
-// arrive on the mbarrier at this shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+// arrive on the mbarrier at this shared-window address in CTA `cta` of the cluster.  The arrival has the default
+// .release.cta semantics: it frees a stage whose only readers were this CTA's wgmma (complete once wgmma.wait_group
+// returns) for the next TMA write.  A .release.cluster arrival compiles to MEMBAR.ALL.GPU in front of the arrive (ptxas,
+// sm_90a), which stalled the consumer warp that issues the next k-block's wgmma, twice per k-block.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
       ".reg .b32 remote;\n\t"
       "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t"
+      "}\n" ::"r"(bar),
       "r"(cta)
       : "memory");
 }

@@ -341,11 +341,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     uint32_t phase = 0;
     uint32_t epi_chunk = 0;  // running count of staged chunks (selects the staging buffer)
     float acc[BLOCK_N / 2];
+    // Shared-window address of the stage ring, pinned in a register.  In a cluster kernel a shared address carries the
+    // CTA's id, and ptxas rebuilt it from SR_CgaCtaId before every k-block's barrier wait and first wgmma instead of
+    // keeping it live.
+    uint32_t ring;
+    asm volatile("mov.b32 %0, %1;\n" : "=r"(ring) : "r"(smem_u32(smem)));
+    const uint32_t ring_b = ring + static_cast<uint32_t>(smem_b - smem);
+    const uint32_t ring_full = ring + static_cast<uint32_t>(reinterpret_cast<uint8_t*>(full_bar) - smem);
+    const uint32_t ring_empty = ring + static_cast<uint32_t>(reinterpret_cast<uint8_t*>(empty_bar) - smem);
     auto release = [&](int s) {  // one thread per consumer warpgroup frees the stage (in both CTAs of a pair)
       if (wq == 0 && lane == 0) {
         if constexpr (CTAS == 2) {
-          mbar_arrive_cluster(&empty_bar[s], 0);
-          mbar_arrive_cluster(&empty_bar[s], 1);
+          mbar_arrive_cluster(ring_empty + s * 8, 0);
+          mbar_arrive_cluster(ring_empty + s * 8, 1);
         } else {
           mbar_arrive(&empty_bar[s]);
         }
@@ -361,9 +369,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       wgmma_fence_regs(acc);
       int prev = -1;
       for (int kb = 0; kb < t.k_blocks; ++kb) {
-        mbar_wait_flag(&full_bar[stage], phase, stuck);
-        const uint32_t a_addr = smem_u32(smem_a + stage * C::A_STAGE_BYTES);
-        const uint32_t b_addr = smem_u32(smem_b + stage * C::B_STAGE_BYTES);
+        mbar_wait_flag(ring_full + stage * 8, phase, stuck);
+        const uint32_t a_addr = ring + stage * C::A_STAGE_BYTES;
+        const uint32_t b_addr = ring_b + stage * C::B_STAGE_BYTES;
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
