@@ -1,4 +1,5 @@
-"""Fused MoE routing: fp32 softmax over experts + top-k (+ selection bias, + renormalisation) and its backward."""
+"""Fused MoE routing: fp32 softmax or sigmoid scores + top-k (+ selection bias, + group-limited selection, + renormalisation,
++ scaling) and its backward."""
 
 from __future__ import annotations
 
@@ -26,17 +27,23 @@ def route_topk_reference(logits: torch.Tensor, top_k: int, renormalize: bool, ex
 
 class _RouteTopK(Function):
     @staticmethod
-    def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None):
-        idx, probs = native_ops().router_topk_fwd(logits, expert_bias, top_k, renormalize)
+    def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None,
+                score_function: str, num_groups: int, topk_groups: int, scaling_factor: float):
+        idx, probs = native_ops().router_topk_fwd(logits, expert_bias, top_k, renormalize, score_function, num_groups,
+                                                  topk_groups, scaling_factor)
         ctx.save_for_backward(logits, idx)
         ctx.renormalize = renormalize
+        ctx.score_function = score_function
+        ctx.scaling_factor = scaling_factor
         ctx.mark_non_differentiable(idx)
         return idx, probs
 
     @staticmethod
     def backward(ctx: Any, _didx: torch.Tensor, dprobs: torch.Tensor):  # type: ignore[override]
         logits, idx = ctx.saved_tensors
-        return native_ops().router_topk_bwd(logits, idx, dprobs.float().contiguous(), ctx.renormalize), None, None, None
+        dlogits = native_ops().router_topk_bwd(logits, idx, dprobs.float().contiguous(), ctx.renormalize, ctx.score_function,
+                                               ctx.scaling_factor)
+        return dlogits, None, None, None, None, None, None, None
 
 
 def route_topk_general(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None,
@@ -77,18 +84,27 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
                score_function: str = "softmax", num_groups: int = 1, topk_groups: int = 1, scaling_factor: float = 1.0):
     """``logits [..., E]`` -> ``(indices [..., k] int64, probabilities [..., k] fp32)``.
 
-    Plain softmax top-k (the Qwen3 / Mixtral router) runs on the fused CUDA kernel; the DeepSeek variants (sigmoid scores,
-    group-limited selection, weight scaling) are ``[tokens, experts]``-sized element-wise work and use the PyTorch
-    definition on every device.
+    bf16 CUDA logits with ``E <= 1024``, ``k <= min(32, E)`` and at most 32 expert groups run on the fused CUDA kernel,
+    whatever the routing options (softmax or sigmoid scores, bias, group-limited selection, renormalisation, scaling).
+    Other inputs use the PyTorch definitions: ``route_topk_reference`` for plain softmax top-k, ``route_topk_general``
+    for the DeepSeek variants.
     """
-    if score_function != "softmax" or num_groups > 1 or scaling_factor != 1.0:
-        return route_topk_general(logits, top_k, renormalize, expert_bias, score_function, num_groups, topk_groups, scaling_factor)
-    if on_gpu(logits) and logits.dtype == torch.bfloat16 and logits.shape[-1] <= 1024 and top_k <= 32:
-        flat = logits.reshape(-1, logits.shape[-1])
+    num_experts = logits.shape[-1]
+    if num_groups > 1 and (num_experts % num_groups != 0 or not 0 < topk_groups <= num_groups):
+        raise ValueError("experts must split evenly into groups and 0 < topk_groups <= num_groups")
+    if score_function not in ("softmax", "sigmoid"):
+        raise ValueError(f"unknown router score function {score_function!r}")
+    if (on_gpu(logits) and logits.dtype == torch.bfloat16 and num_experts <= 1024 and top_k <= min(32, num_experts)
+            and num_groups <= 32):
+        flat = logits.reshape(logits.shape[:-1].numel(), num_experts)  # also when there are no tokens
         if not flat.is_contiguous():
             flat = flat.contiguous()
-        idx, probs = _RouteTopK.apply(flat, top_k, renormalize, None if expert_bias is None else expert_bias.float().contiguous())
+        groups = (num_groups, topk_groups) if num_groups > 1 else (1, 1)
+        idx, probs = _RouteTopK.apply(flat, top_k, renormalize, None if expert_bias is None else expert_bias.float().contiguous(),
+                                      score_function, *groups, float(scaling_factor))
         return idx.view(*logits.shape[:-1], top_k), probs.view(*logits.shape[:-1], top_k)
+    if score_function != "softmax" or num_groups > 1 or scaling_factor != 1.0:
+        return route_topk_general(logits, top_k, renormalize, expert_bias, score_function, num_groups, topk_groups, scaling_factor)
     return route_topk_reference(logits, top_k, renormalize, expert_bias)
 
 

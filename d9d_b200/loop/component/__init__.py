@@ -3,6 +3,7 @@
 from .batch_maths import BatchMaths
 from .checkpointer import StateCheckpointer
 from .data_loader_factory import DataLoaderFactory, IteratorBatchGroup, StatefulDataLoaderDataParallelAware
+from .expert_bias_balancer import ExpertBiasBalancer
 from .garbage_collector import ManualGarbageCollector
 from .gradient_clipper import GradientClipper
 from .gradient_manager import GradientManager
@@ -21,6 +22,7 @@ __all__ = [
     "STATE_LOSS_WEIGHT",
     "BatchMaths",
     "DataLoaderFactory",
+    "ExpertBiasBalancer",
     "ForwardResult",
     "GradientClipper",
     "GradientManager",

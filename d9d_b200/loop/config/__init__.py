@@ -5,6 +5,7 @@ from .config import (
     CheckpointingConfig,
     DataLoadingConfig,
     DeterminismConfig,
+    ExpertBiasBalancingConfig,
     GarbageCollectionConfig,
     GradientClippingConfig,
     GradientManagerConfig,
@@ -24,6 +25,7 @@ __all__ = [
     "CheckpointingConfig",
     "DataLoadingConfig",
     "DeterminismConfig",
+    "ExpertBiasBalancingConfig",
     "GarbageCollectionConfig",
     "GradientClippingConfig",
     "GradientManagerConfig",

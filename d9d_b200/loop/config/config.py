@@ -85,6 +85,14 @@ class GradientManagerConfig(BaseModel):
     fold_scaling_into_optimizer: bool = True
 
 
+class ExpertBiasBalancingConfig(BaseModel):
+    """Auxiliary-loss-free load balancing (DeepSeek-V3): after every optimizer step each expert bias of the model's MoE
+    routers moves by ``update_rate`` toward balance, ``b_e += update_rate * sign(mean(c) - c_e)``, ``c_e`` counting the
+    step's selections of expert ``e`` over every rank of the pipeline stage."""
+
+    update_rate: float
+
+
 class TimeoutConfig(BaseModel):
     init_timeout: int = 10000
     step_timeout: int = 100
@@ -104,6 +112,7 @@ class TrainerConfig(BaseModel):
     profiling: ProfilingConfig | None
     gradient_manager: GradientManagerConfig
     timeout: TimeoutConfig = TimeoutConfig()
+    expert_bias_balancing: ExpertBiasBalancingConfig | None = None  # None: expert biases stay as loaded
 
 
 class InferenceConfig(BaseModel):

@@ -78,6 +78,8 @@ class TrainingConfigurator:
                                    additional_hparams=hparams),
             exporter=parts.ModelStageExporter(model_provider=self._model_provider, dist_context=ctx, modules=modules),
             garbage_collector=house.gc, checkpointer=house.checkpointer, profiler=house.profiler, timeout_manager=base.timeout,
+            expert_bias_balancer=parts.ExpertBiasBalancer(dist_context=ctx, tracked_modules=modules, config=cfg.expert_bias_balancing)
+            if cfg.expert_bias_balancing is not None else None,
         )
 
     def configure(self) -> "Trainer":
@@ -89,7 +91,7 @@ class Trainer:
 
     One iteration == one optimizer step: forward/backward over the accumulation group (gradient buckets all-reduce
     on the side stream as they fill), metric sync kicked off asynchronously, gradient wait + ``1/sum(w)`` scaling,
-    clipping, optimizer, LR scheduler, logging, ``zero_grad``, housekeeping, post-step checkpoint.
+    clipping, optimizer, expert-bias balancing (when configured), LR scheduler, logging, ``zero_grad``, housekeeping, post-step checkpoint.
     """
 
     def __init__(self, state: TrainJobState):
@@ -124,6 +126,8 @@ class Trainer:
             for batch_group in s.data_loader:
                 run.set_step(s.stepper.current_step)
                 s.event_bus.trigger(events.EVENT_TRAIN_STEP_PRE, step_ctx)
+                if s.expert_bias_balancer is not None:
+                    s.expert_bias_balancer.reset_counters()
                 with s.event_bus.bounded(events.EVENT_TRAIN_FORWARD_BACKWARD_PRE, events.EVENT_TRAIN_FORWARD_BACKWARD_POST, step_ctx):
                     for batch in batch_group:
                         result = s.task_operator.forward_backward(batch)
@@ -134,6 +138,8 @@ class Trainer:
                 s.gradient_clipper.clip_and_log(run)
                 with s.event_bus.bounded(events.EVENT_TRAIN_OPTIMIZER_STEP_PRE, events.EVENT_TRAIN_OPTIMIZER_STEP_POST, step_ctx):
                     s.optimizer.step()
+                if s.expert_bias_balancer is not None:
+                    s.expert_bias_balancer.update()
                 s.lr_scheduler.step()
                 s.logger.log(run, loss_value=s.gradient_manager.compute_global_loss())
                 s.gradient_manager.zero_grad()

@@ -1,7 +1,8 @@
 """Aggregated job state (everything the loops need + what gets checkpointed).
 
 Checkpoint key tree (reference ``d9d/loop/state.py:64-118``): ``stepper``, ``tracked_modules``, ``data_loader`` and,
-for training, ``logger``, ``task``, ``metrics``, ``optimizer``, ``lr_scheduler``.
+for training, ``logger``, ``task``, ``metrics``, ``optimizer``, ``lr_scheduler`` (+ ``expert_bias_balancer`` when expert-bias
+balancing is on).
 """
 
 from __future__ import annotations
@@ -16,6 +17,7 @@ from d9d_b200.core.dist_context import DistributedContext
 from d9d_b200.core.protocol import LRSchedulerProtocol, OptimizerProtocol
 from d9d_b200.loop.component import (
     BatchMaths,
+    ExpertBiasBalancer,
     GradientClipper,
     GradientManager,
     InferenceTaskOperator,
@@ -36,16 +38,17 @@ from d9d_b200.metric.impl.container import ComposeMetric
 
 class _CheckpointedFields(Stateful):
     """``state_dict`` / ``load_state_dict`` derived from ``CHECKPOINTED``: the names of the fields that are Stateful and
-    belong in a job checkpoint (subclasses extend the tuple)."""
+    belong in a job checkpoint (subclasses extend the tuple).  Optional fields that are ``None`` are left out."""
 
     CHECKPOINTED: tuple[str, ...] = ()
 
     def state_dict(self) -> dict[str, Any]:
-        return {name: getattr(self, name).state_dict() for name in self.CHECKPOINTED}
+        return {name: getattr(self, name).state_dict() for name in self.CHECKPOINTED if getattr(self, name) is not None}
 
     def load_state_dict(self, state_dict: dict[str, Any]) -> None:
         for name in self.CHECKPOINTED:
-            getattr(self, name).load_state_dict(state_dict[name])
+            if getattr(self, name) is not None:
+                getattr(self, name).load_state_dict(state_dict[name])
 
 
 @dataclasses.dataclass(kw_only=True)
@@ -68,7 +71,7 @@ class JobState(_CheckpointedFields):
 
 @dataclasses.dataclass(kw_only=True)
 class TrainJobState(JobState):
-    CHECKPOINTED = (*JobState.CHECKPOINTED, "logger", "task", "metrics", "optimizer", "lr_scheduler")
+    CHECKPOINTED = (*JobState.CHECKPOINTED, "logger", "task", "metrics", "optimizer", "lr_scheduler", "expert_bias_balancer")
 
     task: TrainTask
     task_operator: TrainTaskOperator
@@ -79,6 +82,7 @@ class TrainJobState(JobState):
     gradient_manager: GradientManager
     gradient_clipper: GradientClipper
     exporter: ModelStageExporter
+    expert_bias_balancer: ExpertBiasBalancer | None = None
 
 
 @dataclasses.dataclass(kw_only=True)

@@ -1,5 +1,6 @@
 """Mixture-of-Experts building blocks."""
 
+from .balancing import update_expert_bias
 from .grouped_experts import GroupedSwiGLU
 from .grouped_linear import GroupedLinear
 from .layer import MoELayer
@@ -15,4 +16,5 @@ __all__ = [
     "SharedExpertParameters",
     "SharedSwiGLU",
     "TopKRouter",
+    "update_expert_bias",
 ]

@@ -638,9 +638,17 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> qk_norm_rope_bwd(const Tensor& dq_out
 }
 
 // ------------------------------------------------------------------ MoE router
-std::tuple<Tensor, Tensor> router_topk_fwd(const Tensor& logits, const c10::optional<Tensor>& bias, int64_t k, bool renorm) {
+static bool router_sigmoid(c10::string_view score_function) {
+  TORCH_CHECK(score_function == "softmax" || score_function == "sigmoid", "router: unknown score function ", score_function);
+  return score_function == "sigmoid";
+}
+
+std::tuple<Tensor, Tensor> router_topk_fwd(const Tensor& logits, const c10::optional<Tensor>& bias, int64_t k, bool renorm,
+                                           c10::string_view score_function, int64_t num_groups, int64_t topk_groups,
+                                           double scaling_factor) {
   CHECK_CUDA_CONTIG(logits);
   TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && logits.dim() == 2);
+  const bool sigmoid = router_sigmoid(score_function);
   c10::cuda::CUDAGuard guard(logits.device());
   const int64_t T = logits.size(0), E = logits.size(1);
   const float* b = nullptr;
@@ -650,19 +658,23 @@ std::tuple<Tensor, Tensor> router_topk_fwd(const Tensor& logits, const c10::opti
   }
   Tensor idx = at::empty({T, k}, logits.options().dtype(at::kLong));
   Tensor probs = at::empty({T, k}, logits.options().dtype(at::kFloat));
-  d9d::router_topk_fwd(logits.data_ptr(), b, T, static_cast<int>(E), static_cast<int>(k), renorm,
+  d9d::router_topk_fwd(logits.data_ptr(), b, T, static_cast<int>(E), static_cast<int>(k), renorm, sigmoid,
+                       static_cast<int>(num_groups), static_cast<int>(topk_groups), static_cast<float>(scaling_factor),
                        reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), probs.data_ptr<float>(), cur_stream());
   return {idx, probs};
 }
 
-Tensor router_topk_bwd(const Tensor& logits, const Tensor& idx, const Tensor& dprobs, bool renorm) {
+Tensor router_topk_bwd(const Tensor& logits, const Tensor& idx, const Tensor& dprobs, bool renorm, c10::string_view score_function,
+                       double scaling_factor) {
   CHECK_CUDA_CONTIG(logits); CHECK_CUDA_CONTIG(idx); CHECK_CUDA_CONTIG(dprobs);
   TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && idx.scalar_type() == at::kLong && dprobs.scalar_type() == at::kFloat);
+  const bool sigmoid = router_sigmoid(score_function);
   c10::cuda::CUDAGuard guard(logits.device());
   const int64_t T = logits.size(0), E = logits.size(1), k = idx.size(1);
   Tensor out = at::empty_like(logits);
   d9d::router_topk_bwd(logits.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dprobs.data_ptr<float>(), T,
-                       static_cast<int>(E), static_cast<int>(k), renorm, out.data_ptr(), cur_stream());
+                       static_cast<int>(E), static_cast<int>(k), renorm, sigmoid, static_cast<float>(scaling_factor),
+                       out.data_ptr(), cur_stream());
   return out;
 }
 
@@ -867,8 +879,9 @@ TORCH_LIBRARY(d9d_b200, m) {
         "int style) -> (Tensor, Tensor, Tensor)");
   m.def("qk_norm_rope_bwd(Tensor dq_out, Tensor dk_out, Tensor q, Tensor k, Tensor wq, Tensor wk, Tensor cos_t, Tensor sin_t, "
         "Tensor inv_rms, bool zero_centered, int style) -> (Tensor, Tensor, Tensor, Tensor)");
-  m.def("router_topk_fwd(Tensor logits, Tensor? bias, int k, bool renorm) -> (Tensor, Tensor)");
-  m.def("router_topk_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm) -> Tensor");
+  m.def("router_topk_fwd(Tensor logits, Tensor? bias, int k, bool renorm, str score_function, int num_groups, int topk_groups, "
+        "float scaling_factor) -> (Tensor, Tensor)");
+  m.def("router_topk_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm, str score_function, float scaling_factor) -> Tensor");
   m.def("gemm_ag_a(int[] a_peer_ptrs, int rows_local, int lda, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int block_n=0) -> ()");
   m.def("gemm_wait_a(Tensor a, Tensor flags, int rank, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int spare_sms=0, "
         "int block_n=0) -> ()");

@@ -199,11 +199,13 @@ void qk_norm_rope_bwd(const void* dq_out, const void* dk_out, const void* q, con
                       float* dw_partial, float* dwq, float* dwk, cudaStream_t s);
 
 // ------------------------------------------------------------------ MoE router -----------------------------
-// logits [T, E] bf16 -> softmax (fp32) -> top-k by (prob + bias) -> idx [T, k] int64, probs [T, k] fp32 (renormalised)
-void router_topk_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, long long* idx,
-                     float* probs, cudaStream_t stream);
+// logits [T, E] bf16 -> scores (fp32 softmax, or sigmoid) -> top-k by (score + bias), optionally only among the
+// topk_groups best of num_groups expert groups (group score: sum of its two best keys; dropped experts get key 0) ->
+// idx [T, k] int64, probs [T, k] fp32 = scale * score (renormalised over the k when renorm)
+void router_topk_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
+                     int num_groups, int topk_groups, float scale, long long* idx, float* probs, cudaStream_t stream);
 void router_topk_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                     bool renorm, void* dlogits, cudaStream_t stream);
+                     bool renorm, bool sigmoid, float scale, void* dlogits, cudaStream_t stream);
 
 // ------------------------------------------------------------------ expert-parallel exchange over NVLink ----
 // peer_base: device array [world] of symmetric-arena base pointers; off_* are byte offsets of regions inside the arena.
