@@ -222,6 +222,18 @@ __device__ __forceinline__ void named_barrier_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
 }
 
+// arrive on a named barrier without waiting for it (the threads that bar.sync it wait for these arrivals)
+__device__ __forceinline__ void named_barrier_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
+}
+
+// two floats from an 8-byte aligned shared-memory address (a 32-bit shared-window address, as smem_u32 returns)
+__device__ __forceinline__ float2 lds_f32x2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];\n" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+
 // ----------------------------------------------------------------------------------------------
 // numeric helpers
 // ----------------------------------------------------------------------------------------------

@@ -17,6 +17,7 @@
 // Reference parity: d9d/kernel/flash_attn/function.py:72-178 (fwd/bwd, sink gradient), :181-305 (varlen).
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 #include "gemm_host.cuh"
 
@@ -484,21 +485,24 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
           if (lane == 0) mbar_arrive(&st_full[st]);
         }
         if constexpr (DKV) {
-          // per-query statistics of this tile: lse in the log2 domain (+inf -> P = 0 for rows outside the sequence)
+          // per-query statistics of this tile: lse in the log2 domain (+inf -> P = 0 for rows outside the sequence).
+          // Column c = 8 jj + 2 quad + e of a consumer fragment goes to quad * SR/4 + 2 jj + e: the two columns a consumer
+          // thread reads per jj are one 8-byte shared load
           constexpr int PER_LANE = SR / 32;
           float* vec = smem_vec + st * (2 * SR);
           const long long base = sq.lse_base + static_cast<long long>(hs) * p.lse_hs;
 #pragma unroll
           for (int e = 0; e < PER_LANE; ++e) {
-            const int q = c0 + lane * PER_LANE + e;
+            const int c = lane * PER_LANE + e, q = c0 + c;
+            const int pos = ((c >> 1) & 3) * (SR / 4) + (c >> 3) * 2 + (c & 1);
             float l2 = INFINITY, dl = 0.f;
             if (q < sq.Sq) {
               const float lv = p.lse[base + q];
               l2 = (lv == -INFINITY) ? INFINITY : lv * kLog2e;
               dl = p.delta[base + q];
             }
-            vec[lane * PER_LANE + e] = l2;
-            vec[SR + lane * PER_LANE + e] = dl;
+            vec[pos] = l2;
+            vec[SR + pos] = dl;
           }
           __syncwarp();
           if (lane == 0) mbar_arrive(&st_full[st]);
@@ -539,7 +543,16 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
     // Commit groups per streamed tile, in issue order: S, dP, [dV,] dK / dQ.  The exp of P runs while dP is on the tensor
     // cores and dS is formed while dV runs.  The tile's groups all retire before the next one starts: groups still in
     // flight across the loop's back edge make ptxas serialise every wgmma (C7515).
-    if (T > 0) mbar_wait_flag(r_full, 0, stuck);
+    // DKV: the two consumer warpgroups take turns to issue S and dP (named barriers 1 + cw, FA3's warpgroup ping-pong), so
+    // that the tensor cores run one warpgroup's GEMMs while the other computes P and dS, instead of both doing their math
+    // at once.  Warpgroup 1 opens the first turn for warpgroup 0 and skips its last hand-over: no arrival is left pending.
+    // DQ has no dV GEMM to cover the other warpgroup's math and ran 1-5 % slower with the turns (H100): it takes none.
+    if (T > 0) {
+      if (DKV && cw == 1) named_barrier_arrive(1, 256);
+      mbar_wait_flag(r_full, 0, stuck);
+    }
+    // this thread's lse2 / delta columns 8 jj + cq + {0, 1} of a DKV stage: 8 bytes at vec_lane + 8 jj (see the producer)
+    const uint32_t vec_lane = smem_u32(smem_vec) + (lane & 3) * (SR / 4) * 4;
     for (int t = 0; t < T; ++t) {
       const int st = t % NST;
       const int c0 = (clo + (DKV ? t % nc : t)) * SR;  // first streamed row of this tile
@@ -547,6 +560,7 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
       const uint32_t s1_addr = smem_u32(smem_s + st * C::STAGE_BYTES), s2_addr = s1_addr + C::S1_BYTES;
       float s[SR / 2], dp[SR / 2];            // S (then P times the soft-cap derivative), dP
       uint32_t pf[SR / 16][4], df[SR / 16][4];  // P and dS in bf16: the A operands of the second GEMMs
+      if constexpr (DKV) named_barrier_sync(1 + cw, 256);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < DQK / 16; ++kk)
@@ -556,9 +570,8 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
       for (int kk = 0; kk < DV / 16; ++kk)
         wgmma_bf16_ss<SR, 0, 0>(dp, desc_kmajor(r2_addr, 128 * 128, kk), desc_kmajor(s2_addr, SR * 128, kk), kk != 0);
       wgmma_commit();
-      wgmma_wait<1>();  // S
-      wgmma_fence_regs(s);
-      const float* vec = smem_vec + st * (2 * SR);
+      if (DKV && (cw == 0 || t + 1 < T)) named_barrier_arrive(2 - cw, 256);
+      const uint32_t vec_addr = vec_lane + st * (2 * SR * 4);
       int vlo[2], vhi[2];  // visible streamed columns [vlo, vhi] (relative to c0) of this thread's two rows
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
@@ -570,28 +583,49 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
           vlo[r] = p.wl < 0 ? 0 : ri + sq.off - p.wl - c0;
           vhi[r] = min(sq.Sk - 1, p.wr < 0 ? sq.Sk - 1 : ri + sq.off + p.wr) - c0;
         }
+      }
+      // Only tiles on a mask edge test columns: in the others every column of this thread's rows is visible
+      const bool edge = vlo[0] > 0 || vlo[1] > 0 || vhi[0] < SR - 1 || vhi[1] < SR - 1;
+      wgmma_wait<1>();  // S
+      wgmma_fence_regs(s);
+      auto p_tile = [&](auto masked, auto cap) {
 #pragma unroll
         for (int jj = 0; jj < SR / 8; ++jj) {
-          float pv[2];
+          float2 l2v = make_float2(0.f, 0.f);
+          if constexpr (DKV) l2v = lds_f32x2(vec_addr + 8 * jj);
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = 8 * jj + cq + e;
-            const int i = 4 * jj + 2 * r + e;
-            const float l2 = DKV ? vec[c] : my_lse2[r];
-            float x = s[i], dcap = 1.f;
-            if (capped) {
-              const float tcap = tanhf(x * cap_in);
-              x = p.softcap * tcap * kLog2e;
-              dcap = 1.f - tcap * tcap;
-            } else {
-              x *= scale_log2;
+          for (int r = 0; r < 2; ++r) {
+            float pv[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * jj + cq + e;
+              const int i = 4 * jj + 2 * r + e;
+              const float l2 = DKV ? (e ? l2v.y : l2v.x) : my_lse2[r];
+              float x = s[i], dcap = 1.f;
+              if constexpr (cap) {
+                const float tcap = tanhf(x * cap_in);
+                x = p.softcap * tcap * kLog2e - l2;
+                dcap = 1.f - tcap * tcap;
+              } else {
+                // x * scale - lse with one rounding in every copy of the loop (given as a product and a difference,
+                // the compiler may form the product once for all copies and round it separately)
+                x = fmaf(x, scale_log2, -l2);
+              }
+              const bool vis = !masked || ((c >= vlo[r]) && (c <= vhi[r]));
+              pv[e] = vis ? exp2f(x) : 0.f;
+              s[i] = pv[e] * dcap;
             }
-            const bool vis = (c >= vlo[r]) && (c <= vhi[r]);
-            pv[e] = vis ? exp2f(x - l2) : 0.f;
-            s[i] = pv[e] * dcap;
+            pf[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(pv[0], pv[1]);  // = pack_a_frag(P, jj / 2)
           }
-          pf[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(pv[0], pv[1]);  // = pack_a_frag(P, jj / 2)
         }
+      };
+      // one copy of the loop per (mask edge, soft-cap) case: a branch on either inside it is taken per element
+      if (capped) {
+        if (edge) p_tile(std::true_type{}, std::true_type{});
+        else p_tile(std::false_type{}, std::true_type{});
+      } else {
+        if (edge) p_tile(std::true_type{}, std::false_type{});
+        else p_tile(std::false_type{}, std::false_type{});
       }
       if constexpr (DKV) {
         wgmma_fence_regs(acc1);
@@ -602,23 +636,29 @@ flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_r1, const __grid_
       }
       wgmma_wait<DKV ? 1 : 0>();  // dP
       wgmma_fence_regs(dp);
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
+      auto ds_tile = [&](auto masked) {
 #pragma unroll
         for (int jj = 0; jj < SR / 8; ++jj) {
-          float ds[2];
+          float2 dlv = make_float2(0.f, 0.f);
+          if constexpr (DKV) dlv = lds_f32x2(vec_addr + SR * 4 + 8 * jj);
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = 8 * jj + cq + e;
-            const int i = 4 * jj + 2 * r + e;
-            const float dl = DKV ? vec[SR + c] : my_delta[r];
-            // dP may be NaN at masked columns (DQ: V rows past the end of the sequence), where dS must be exactly 0
-            const bool vis = (c >= vlo[r]) && (c <= vhi[r]);
-            ds[e] = vis ? s[i] * (dp[i] - dl) : 0.f;
+          for (int r = 0; r < 2; ++r) {
+            float ds[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * jj + cq + e;
+              const int i = 4 * jj + 2 * r + e;
+              const float dl = DKV ? (e ? dlv.y : dlv.x) : my_delta[r];
+              // dP may be NaN at masked columns (DQ: V rows past the end of the sequence), where dS must be exactly 0
+              const bool vis = !masked || ((c >= vlo[r]) && (c <= vhi[r]));
+              ds[e] = vis ? s[i] * (dp[i] - dl) : 0.f;
+            }
+            df[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(ds[0], ds[1]);
           }
-          df[jj >> 1][2 * (jj & 1) + r] = pack_bf16x2(ds[0], ds[1]);
         }
-      }
+      };
+      if (edge) ds_tile(std::true_type{});
+      else ds_tile(std::false_type{});
       float(&acc_ds)[DQK / 2] = pick<DKV>(acc2, acc1);
       wgmma_fence_regs(acc_ds);
       wgmma_fence();
