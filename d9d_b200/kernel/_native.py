@@ -53,6 +53,14 @@ def native_launch_count() -> int:
     return _proxy.launches if _proxy is not None else 0
 
 
+def contiguous_aligned(t: torch.Tensor) -> torch.Tensor:
+    """``t.contiguous()``, copied into a fresh buffer when its first element is not 16-byte aligned.  The native kernels
+    load and store 16 bytes at a time and refuse such operands; ``.contiguous()`` alone returns a contiguous view at an
+    element offset (``flat[3:3 + n]``) unchanged."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 def on_gpu(*tensors: torch.Tensor) -> bool:
     """True if the op must run on the native CUDA path."""
     return any(t is not None and t.is_cuda for t in tensors)

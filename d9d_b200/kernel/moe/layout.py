@@ -8,7 +8,7 @@ from torch.autograd import Function
 
 from d9d_b200.core.autograd import GLOBAL_GRAD_CONTEXT, GradDirection
 
-from .._native import fused_wgrad_buffer, fused_wgrad_owner, grad_dtype_of, native_ops, on_gpu
+from .._native import contiguous_aligned, fused_wgrad_buffer, fused_wgrad_owner, grad_dtype_of, native_ops, on_gpu
 
 ALIGN = 128  # GEMM BLOCK_M: expert segments never share an M-tile, per-expert K ranges are BLOCK_K aligned
 
@@ -105,7 +105,7 @@ def _gather_reference(yp: torch.Tensor, dpp: torch.Tensor | None, layout: MoELay
 
 def _scatter(x, probs, layout: MoELayout):
     if on_gpu(x):
-        xp, pp = native_ops().moe_permute(x.contiguous(), None if probs is None else probs.float().contiguous(),
+        xp, pp = native_ops().moe_permute(contiguous_aligned(x), None if probs is None else probs.float().contiguous(),
                                           layout.row_map, layout.counts, layout.seg_offsets, layout.capacity)
         return xp, (pp if probs is not None else None)
     return _scatter_reference(x, probs, layout)
@@ -113,7 +113,7 @@ def _scatter(x, probs, layout: MoELayout):
 
 def _gather(yp, dpp, layout: MoELayout):
     if on_gpu(yp):
-        y, dprobs = native_ops().moe_gather(yp.contiguous(), None if dpp is None else dpp.contiguous(), layout.row_map,
+        y, dprobs = native_ops().moe_gather(contiguous_aligned(yp), None if dpp is None else dpp.contiguous(), layout.row_map,
                                             layout.num_tokens, layout.top_k)
         return y, (dprobs if dpp is not None else None)
     return _gather_reference(yp, dpp, layout)

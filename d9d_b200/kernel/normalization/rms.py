@@ -8,7 +8,7 @@ from typing import Any
 import torch
 from torch.autograd import Function
 
-from .._native import native_ops, on_gpu
+from .._native import contiguous_aligned, native_ops, on_gpu
 
 
 def rms_norm_reference(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, zero_centered: bool = False) -> torch.Tensor:
@@ -23,8 +23,8 @@ class RMSNormFunction(Function):
     @staticmethod
     def forward(ctx: Any, x: torch.Tensor, weight: torch.Tensor, eps: float, zero_centered: bool) -> torch.Tensor:
         ops = native_ops()
-        xc = x.contiguous()
-        out, inv_rms = ops.rms_norm_fwd(xc, weight.contiguous(), eps, zero_centered)
+        xc = contiguous_aligned(x)
+        out, inv_rms = ops.rms_norm_fwd(xc, contiguous_aligned(weight), eps, zero_centered)
         ctx.save_for_backward(xc, weight, inv_rms)
         ctx.zero_centered = zero_centered
         return out
@@ -32,7 +32,8 @@ class RMSNormFunction(Function):
     @staticmethod
     def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
         x, weight, inv_rms = ctx.saved_tensors
-        dx, dw = native_ops().rms_norm_bwd(grad_output.contiguous(), x, weight.contiguous(), inv_rms, ctx.zero_centered)
+        dx, dw = native_ops().rms_norm_bwd(contiguous_aligned(grad_output), x, contiguous_aligned(weight), inv_rms,
+                                           ctx.zero_centered)
         return dx, dw, None, None
 
 

@@ -7,7 +7,7 @@ from typing import Any
 import torch
 from torch.autograd import Function
 
-from .._native import native_ops, on_gpu
+from .._native import contiguous_aligned, native_ops, on_gpu
 
 
 def silu_mul_reference(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
@@ -17,14 +17,14 @@ def silu_mul_reference(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
 class SiLUMulFunction(Function):
     @staticmethod
     def forward(ctx: Any, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
-        x, y = x.contiguous(), y.contiguous()
+        x, y = contiguous_aligned(x), contiguous_aligned(y)
         ctx.save_for_backward(x, y)
         return native_ops().silu_mul_fwd(x, y)
 
     @staticmethod
     def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
         x, y = ctx.saved_tensors
-        return native_ops().silu_mul_bwd(grad_output.contiguous(), x, y)
+        return native_ops().silu_mul_bwd(contiguous_aligned(grad_output), x, y)
 
 
 def silu_mul(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
@@ -36,14 +36,14 @@ def silu_mul(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
 class SiLUMulProbsFunction(Function):
     @staticmethod
     def forward(ctx: Any, x: torch.Tensor, y: torch.Tensor, probs: torch.Tensor) -> torch.Tensor:
-        x, y, probs = x.contiguous(), y.contiguous(), probs.contiguous()
+        x, y, probs = contiguous_aligned(x), contiguous_aligned(y), probs.contiguous()
         ctx.save_for_backward(x, y, probs)
         return native_ops().silu_mul_probs_fwd(x, y, probs)
 
     @staticmethod
     def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
         x, y, probs = ctx.saved_tensors
-        return native_ops().silu_mul_probs_bwd(grad_output.contiguous(), x, y, probs)
+        return native_ops().silu_mul_probs_bwd(contiguous_aligned(grad_output), x, y, probs)
 
 
 def silu_mul_probs(x: torch.Tensor, y: torch.Tensor, probs: torch.Tensor) -> torch.Tensor:

@@ -24,6 +24,10 @@ inline int dtype_code(const Tensor& t) {
 }
 
 #define CHECK_CUDA_CONTIG(t) TORCH_CHECK((t).is_cuda() && (t).is_contiguous(), #t " must be a contiguous CUDA tensor")
+// Operands the kernels load or store 16 bytes at a time (uint4 / float4). A contiguous view at an element offset keeps
+// is_contiguous() but not the alignment, so it is refused here rather than reaching a misaligned vector access.
+#define CHECK_ALIGNED16(t) \
+  TORCH_CHECK(reinterpret_cast<uintptr_t>((t).data_ptr()) % 16 == 0, #t " must start on a 16-byte boundary")
 
 // ------------------------------------------------------------------ GEMM ------------------------
 int epi_for(const Tensor& d, bool accumulate) {
@@ -276,10 +280,11 @@ void gemm_mxfp8(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tenso
 
 // ------------------------------------------------------------------ RMSNorm ---------------------
 std::tuple<Tensor, Tensor> rms_norm_fwd(const Tensor& x, const Tensor& w, double eps, bool zero_centered) {
-  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(w);
+  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(w); CHECK_ALIGNED16(x); CHECK_ALIGNED16(w);
   TORCH_CHECK(x.scalar_type() == w.scalar_type(), "rms_norm: x and weight dtypes must match");
   c10::cuda::CUDAGuard guard(x.device());
   const int N = static_cast<int>(x.size(-1));
+  TORCH_CHECK(N > 0 && w.numel() == N, "rms_norm: weight must have x.size(-1) elements");
   const int64_t M = x.numel() / N;
   Tensor out = at::empty_like(x);
   Tensor inv = at::empty({M}, x.options().dtype(at::kFloat));
@@ -291,9 +296,14 @@ std::tuple<Tensor, Tensor> rms_norm_fwd(const Tensor& x, const Tensor& w, double
 std::tuple<Tensor, Tensor> rms_norm_bwd(const Tensor& dout, const Tensor& x, const Tensor& w, const Tensor& inv_rms,
                                         bool zero_centered) {
   CHECK_CUDA_CONTIG(dout); CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(w); CHECK_CUDA_CONTIG(inv_rms);
+  CHECK_ALIGNED16(dout); CHECK_ALIGNED16(x); CHECK_ALIGNED16(w);
+  TORCH_CHECK(dout.scalar_type() == x.scalar_type() && w.scalar_type() == x.scalar_type() && dout.numel() == x.numel(),
+              "rms_norm bwd: dout, x and weight must share a dtype and dout the shape of x");
   c10::cuda::CUDAGuard guard(x.device());
   const int N = static_cast<int>(x.size(-1));
+  TORCH_CHECK(N > 0 && w.numel() == N, "rms_norm bwd: weight must have x.size(-1) elements");
   const int64_t M = x.numel() / N;
+  TORCH_CHECK(inv_rms.scalar_type() == at::kFloat && inv_rms.numel() == M, "rms_norm bwd: inv_rms must be fp32 with one value per row");
   Tensor dx = at::empty_like(x);
   Tensor dw = at::empty_like(w);
   Tensor partial = at::empty({d9d::rms_norm_bwd_num_partials(), N}, x.options().dtype(at::kFloat));
@@ -304,7 +314,7 @@ std::tuple<Tensor, Tensor> rms_norm_bwd(const Tensor& dout, const Tensor& x, con
 
 // ------------------------------------------------------------------ SiLU * mul -------------------
 Tensor silu_mul_fwd(const Tensor& x, const Tensor& y) {
-  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(y);
+  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(y); CHECK_ALIGNED16(x); CHECK_ALIGNED16(y);
   TORCH_CHECK(x.scalar_type() == y.scalar_type() && x.numel() == y.numel());
   c10::cuda::CUDAGuard guard(x.device());
   Tensor out = at::empty_like(x);
@@ -314,6 +324,9 @@ Tensor silu_mul_fwd(const Tensor& x, const Tensor& y) {
 
 std::tuple<Tensor, Tensor> silu_mul_bwd(const Tensor& dout, const Tensor& x, const Tensor& y) {
   CHECK_CUDA_CONTIG(dout); CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(y);
+  CHECK_ALIGNED16(dout); CHECK_ALIGNED16(x); CHECK_ALIGNED16(y);
+  TORCH_CHECK(dout.scalar_type() == x.scalar_type() && y.scalar_type() == x.scalar_type() && dout.numel() == x.numel() &&
+              y.numel() == x.numel(), "silu_mul bwd: dout, x and y must share a dtype and a size");
   c10::cuda::CUDAGuard guard(x.device());
   Tensor dx = at::empty_like(x), dy = at::empty_like(y);
   d9d::silu_mul_bwd(dout.data_ptr(), x.data_ptr(), y.data_ptr(), dx.data_ptr(), dy.data_ptr(), x.numel(),
@@ -328,8 +341,10 @@ static const int* valid_rows_ptr(const c10::optional<Tensor>& v) {
 }
 
 Tensor silu_mul_probs_fwd(const Tensor& x, const Tensor& y, const Tensor& probs, const c10::optional<Tensor>& valid_rows) {
-  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(y); CHECK_CUDA_CONTIG(probs);
+  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(y); CHECK_CUDA_CONTIG(probs); CHECK_ALIGNED16(x); CHECK_ALIGNED16(y);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && y.scalar_type() == at::kBFloat16 && probs.scalar_type() == at::kFloat);
+  TORCH_CHECK(x.dim() == 2 && y.sizes() == x.sizes() && probs.numel() == x.size(0),
+              "silu_mul_probs: x and y must be [rows, cols] and probs [rows]");
   c10::cuda::CUDAGuard guard(x.device());
   Tensor out = at::empty_like(x);
   d9d::silu_mul_probs_fwd(x.data_ptr(), y.data_ptr(), probs.data_ptr<float>(), out.data_ptr(), x.size(0),
@@ -340,6 +355,11 @@ Tensor silu_mul_probs_fwd(const Tensor& x, const Tensor& y, const Tensor& probs,
 std::tuple<Tensor, Tensor, Tensor> silu_mul_probs_bwd(const Tensor& dout, const Tensor& x, const Tensor& y,
                                                       const Tensor& probs, const c10::optional<Tensor>& valid_rows) {
   CHECK_CUDA_CONTIG(dout); CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(y); CHECK_CUDA_CONTIG(probs);
+  CHECK_ALIGNED16(dout); CHECK_ALIGNED16(x); CHECK_ALIGNED16(y);
+  TORCH_CHECK(dout.scalar_type() == at::kBFloat16 && x.scalar_type() == at::kBFloat16 && y.scalar_type() == at::kBFloat16 &&
+              probs.scalar_type() == at::kFloat, "silu_mul_probs bwd: bf16 dout / x / y and fp32 probs required");
+  TORCH_CHECK(x.dim() == 2 && y.sizes() == x.sizes() && dout.sizes() == x.sizes() && probs.numel() == x.size(0),
+              "silu_mul_probs bwd: dout, x and y must be [rows, cols] and probs [rows]");
   c10::cuda::CUDAGuard guard(x.device());
   Tensor dx = at::empty_like(x), dy = at::empty_like(y), dp = at::empty_like(probs);
   d9d::silu_mul_probs_bwd(dout.data_ptr(), x.data_ptr(), y.data_ptr(), probs.data_ptr<float>(), dx.data_ptr(),
@@ -384,6 +404,8 @@ Tensor rope_apply(const Tensor& x, const Tensor& cos_cache, const Tensor& sin_ca
                   bool inverse) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.scalar_type() == at::kBFloat16);
   TORCH_CHECK(x.stride(2) == 1 && x.stride(1) == x.size(2), "rope: heads must be contiguous");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 4 == 0 && x.stride(0) % 2 == 0,
+              "rope: x and its token stride must be 4-byte aligned (the kernel moves bf16 pairs)");
   CHECK_CUDA_CONTIG(cos_cache); CHECK_CUDA_CONTIG(sin_cache); CHECK_CUDA_CONTIG(pos);
   TORCH_CHECK(cos_cache.scalar_type() == at::kFloat && sin_cache.scalar_type() == at::kFloat && pos.scalar_type() == at::kLong);
   c10::cuda::CUDAGuard guard(x.device());
@@ -419,8 +441,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> moe_build_layout(const Tensor& topk_i
 // x[T,H] (+ probs[T,k]) -> xp[capacity,H] (+ pp[capacity]); pad rows zeroed, rows past the last segment untouched
 std::tuple<Tensor, Tensor> moe_permute(const Tensor& x, const c10::optional<Tensor>& probs, const Tensor& row_map,
                                        const Tensor& counts, const Tensor& seg_offsets, int64_t capacity) {
-  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(row_map);
-  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2);
+  CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(row_map); CHECK_ALIGNED16(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.size(1) % 8 == 0, "moe_permute: x must be bf16 [T, H], H % 8 == 0");
   c10::cuda::CUDAGuard guard(x.device());
   const int64_t T = x.size(0), H = x.size(1);
   const int k = static_cast<int>(row_map.numel() / std::max<int64_t>(T, 1));
@@ -445,7 +467,10 @@ std::tuple<Tensor, Tensor> moe_permute(const Tensor& x, const c10::optional<Tens
 // zero the pad rows [seg[e] + counts[e], seg[e+1]) of an aligned expert-sorted buffer (and of its per-row fp32 side array)
 void moe_zero_pad(Tensor xp, const c10::optional<Tensor>& pp, const Tensor& counts, const Tensor& seg_offsets) {
   TORCH_CHECK(xp.is_cuda() && xp.dim() == 2 && xp.scalar_type() == at::kBFloat16 && xp.stride(1) == 1 && xp.stride(0) == xp.size(1));
+  TORCH_CHECK(xp.size(1) % 8 == 0, "moe_zero_pad: xp rows must be a multiple of 8 elements");
+  CHECK_ALIGNED16(xp);
   TORCH_CHECK(counts.scalar_type() == at::kInt && seg_offsets.scalar_type() == at::kInt && counts.is_contiguous() && seg_offsets.is_contiguous());
+  TORCH_CHECK(seg_offsets.numel() == counts.numel() + 1, "moe_zero_pad: seg_offsets must have one entry more than counts");
   c10::cuda::CUDAGuard guard(xp.device());
   float* p = nullptr;
   if (pp.has_value()) {
@@ -459,8 +484,8 @@ void moe_zero_pad(Tensor xp, const c10::optional<Tensor>& pp, const Tensor& coun
 // y[T,H] = sum_j yp[row_map[t,j]];   with dpp: also dprobs[T,k] = dpp[row_map[t,j]]
 std::tuple<Tensor, Tensor> moe_gather(const Tensor& yp, const c10::optional<Tensor>& dpp, const Tensor& row_map,
                                       int64_t T, int64_t k) {
-  CHECK_CUDA_CONTIG(yp); CHECK_CUDA_CONTIG(row_map);
-  TORCH_CHECK(yp.scalar_type() == at::kBFloat16 && row_map.numel() == T * k);
+  CHECK_CUDA_CONTIG(yp); CHECK_CUDA_CONTIG(row_map); CHECK_ALIGNED16(yp);
+  TORCH_CHECK(yp.scalar_type() == at::kBFloat16 && yp.dim() == 2 && row_map.numel() == T * k);
   c10::cuda::CUDAGuard guard(yp.device());
   const int H = static_cast<int>(yp.size(1));
   Tensor y = at::empty({T, H}, yp.options());
@@ -478,14 +503,14 @@ std::tuple<Tensor, Tensor> moe_gather(const Tensor& yp, const c10::optional<Tens
 
 // ------------------------------------------------------------------ grad utils -------------------
 void sumsq_accumulate_(const Tensor& x, Tensor out) {
-  CHECK_CUDA_CONTIG(x);
+  CHECK_CUDA_CONTIG(x); CHECK_ALIGNED16(x);
   TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kFloat && out.numel() == 1);
   c10::cuda::CUDAGuard guard(x.device());
   d9d::sumsq_accumulate(x.data_ptr(), x.numel(), dtype_code(x), out.data_ptr<float>(), cur_stream());
 }
 
 void scale_inplace_(Tensor x, const Tensor& scale) {
-  CHECK_CUDA_CONTIG(x);
+  CHECK_CUDA_CONTIG(x); CHECK_ALIGNED16(x);
   TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.numel() == 1);
   c10::cuda::CUDAGuard guard(x.device());
   d9d::scale_inplace(x.data_ptr(), x.numel(), dtype_code(x), scale.data_ptr<float>(), cur_stream());
@@ -596,18 +621,27 @@ static void check_qk(const Tensor& q, const Tensor& k) {
               k.scalar_type() == at::kBFloat16, "qk_norm_rope: q/k must be bf16 [T, H, D]");
   TORCH_CHECK(q.stride(2) == 1 && k.stride(2) == 1 && q.stride(1) == q.size(2) && k.stride(1) == k.size(2) &&
               q.size(0) == k.size(0) && q.size(2) == k.size(2), "qk_norm_rope: heads must be densely packed");
+  CHECK_ALIGNED16(q); CHECK_ALIGNED16(k);
+  TORCH_CHECK(q.stride(0) % 8 == 0 && k.stride(0) % 8 == 0, "qk_norm_rope: token strides must be multiples of 8 elements");
+}
+
+static void check_qk_params(const Tensor& q, const Tensor& wq, const Tensor& wk, const Tensor& cos_t, const Tensor& sin_t) {
+  CHECK_CUDA_CONTIG(wq); CHECK_CUDA_CONTIG(wk); CHECK_CUDA_CONTIG(cos_t); CHECK_CUDA_CONTIG(sin_t);
+  CHECK_ALIGNED16(wq); CHECK_ALIGNED16(wk); CHECK_ALIGNED16(cos_t); CHECK_ALIGNED16(sin_t);
+  TORCH_CHECK(wq.scalar_type() == at::kBFloat16 && wk.scalar_type() == at::kBFloat16 && cos_t.scalar_type() == at::kFloat &&
+              sin_t.scalar_type() == at::kFloat, "qk_norm_rope: bf16 weights and fp32 cos / sin required");
+  const int64_t T = q.size(0), D = q.size(2), rope_dim = cos_t.size(-1);
+  TORCH_CHECK(cos_t.numel() == T * rope_dim && sin_t.numel() == T * rope_dim, "qk_norm_rope: cos / sin must be [T, rope_dim]");
+  TORCH_CHECK(wq.numel() == D && wk.numel() == D, "qk_norm_rope: weights must have head_dim elements");
 }
 
 std::tuple<Tensor, Tensor, Tensor> qk_norm_rope_fwd(const Tensor& q, const Tensor& k, const Tensor& wq, const Tensor& wk,
                                                     const Tensor& cos_t, const Tensor& sin_t, double eps, bool zero_centered,
                                                     int64_t style) {
   check_qk(q, k);
-  CHECK_CUDA_CONTIG(wq); CHECK_CUDA_CONTIG(wk); CHECK_CUDA_CONTIG(cos_t); CHECK_CUDA_CONTIG(sin_t);
-  TORCH_CHECK(wq.scalar_type() == at::kBFloat16 && wk.scalar_type() == at::kBFloat16 && cos_t.scalar_type() == at::kFloat &&
-              sin_t.scalar_type() == at::kFloat);
+  check_qk_params(q, wq, wk, cos_t, sin_t);
   c10::cuda::CUDAGuard guard(q.device());
   const int64_t T = q.size(0), Hq = q.size(1), Hk = k.size(1), D = q.size(2), rope_dim = cos_t.size(-1);
-  TORCH_CHECK(cos_t.numel() == T * rope_dim && sin_t.numel() == T * rope_dim && wq.numel() == D && wk.numel() == D);
   Tensor qo = at::empty({T, Hq, D}, q.options()), ko = at::empty({T, Hk, D}, k.options());
   Tensor inv = at::empty({T, Hq + Hk}, q.options().dtype(at::kFloat));
   d9d::qk_norm_rope_fwd(q.data_ptr(), k.data_ptr(), wq.data_ptr(), wk.data_ptr(), cos_t.data_ptr<float>(), sin_t.data_ptr<float>(), T,
@@ -622,9 +656,14 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> qk_norm_rope_bwd(const Tensor& dq_out
                                                             const Tensor& sin_t, const Tensor& inv_rms, bool zero_centered,
                                                             int64_t style) {
   check_qk(q, k);
+  check_qk_params(q, wq, wk, cos_t, sin_t);
   CHECK_CUDA_CONTIG(dq_out); CHECK_CUDA_CONTIG(dk_out); CHECK_CUDA_CONTIG(inv_rms);
+  CHECK_ALIGNED16(dq_out); CHECK_ALIGNED16(dk_out);
+  TORCH_CHECK(dq_out.scalar_type() == at::kBFloat16 && dk_out.scalar_type() == at::kBFloat16 &&
+              dq_out.numel() == q.numel() && dk_out.numel() == k.numel(), "qk_norm_rope bwd: dq_out / dk_out must match q / k");
   c10::cuda::CUDAGuard guard(q.device());
   const int64_t T = q.size(0), Hq = q.size(1), Hk = k.size(1), D = q.size(2), rope_dim = cos_t.size(-1);
+  TORCH_CHECK(inv_rms.scalar_type() == at::kFloat && inv_rms.numel() == T * (Hq + Hk), "qk_norm_rope bwd: inv_rms must be fp32 [T, Hq + Hk]");
   Tensor dq = at::empty({T, Hq, D}, q.options()), dk = at::empty({T, Hk, D}, k.options());
   const int grid = d9d::qk_norm_rope_grid(T, static_cast<int>(Hq + Hk));
   auto fopt = q.options().dtype(at::kFloat);

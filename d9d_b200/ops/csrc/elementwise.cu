@@ -989,7 +989,8 @@ void rope_apply(const void* x, void* out, const float* cos_cache, const float* s
   if (blocks > cap) blocks = cap;
   const int grid = static_cast<int>(blocks);
   const int vec = D / 32;
-  if (D % 64 != 0 || (rope_dim / 2) % vec != 0 || rope_dim > D)
+  // rope_dim a multiple of 2 * vec: an odd rope_dim would rotate an element without its partner
+  if (D <= 0 || D % 64 != 0 || rope_dim % (2 * vec) != 0 || rope_dim > D)
     throw std::runtime_error("d9d rope: unsupported head_dim / rope_dim combination");
 #define D9D_ROPE(V) \
   rope_kernel<V><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)out, cos_cache, sin_cache, pos, T, H, rope_dim, ldx, ldo, style, inverse)

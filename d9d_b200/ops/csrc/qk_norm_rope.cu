@@ -289,8 +289,12 @@ void qk_norm_rope_bwd(const void* dq_out, const void* dk_out, const void* q, con
                       const float* cos_t, const float* sin_t, const float* inv_rms, long long T, int Hq, int Hk, int D,
                       int rope_dim, long long ldq, long long ldk, bool zero_centered, int style, void* dq, void* dk,
                       float* dw_partial, float* dwq, float* dwk, cudaStream_t s) {
-  if (T == 0) return;
   check_dims(D, rope_dim);
+  if (T == 0) {  // no token contributes: the weight gradients are zero (the reduce kernel that writes them does not run)
+    cudaMemsetAsync(dwq, 0, static_cast<size_t>(D) * sizeof(float), s);
+    cudaMemsetAsync(dwk, 0, static_cast<size_t>(D) * sizeof(float), s);
+    return;
+  }
   const int grid = qk_norm_rope_grid(T, Hq + Hk);
 #define D9D_QKB(V)                                                                                                   \
   qk_norm_rope_bwd_kernel<V><<<grid, 256, 0, s>>>((const __nv_bfloat16*)dq_out, (const __nv_bfloat16*)dk_out,        \
