@@ -14,5 +14,7 @@ def sr_round_reference(x: torch.Tensor, seed: int) -> torch.Tensor:
     bits = x.detach().float().cpu().contiguous().view(torch.int32)
     noise = torch.randint(0, 1 << 16, bits.shape, generator=g, dtype=torch.int32)
     finite = (bits & 0x7F800000) != 0x7F800000
-    rounded = torch.where(finite, bits + noise, bits) & ~0xFFFF
+    # a NaN whose payload lies only in the dropped low bits keeps a quiet bit, so it does not turn into an inf
+    quiet = torch.where((bits & 0xFFFF) != 0, 0x00400000, 0).to(torch.int32)
+    rounded = torch.where(finite, bits + noise, bits | quiet) & ~0xFFFF
     return rounded.view(torch.float32).to(torch.bfloat16).to(x.device)

@@ -264,10 +264,11 @@ __device__ __forceinline__ uint4 philox4x32(uint64_t seed, uint64_t offset) {
 }
 
 // Stochastic rounding fp32 -> bf16: add 16 random bits below the kept mantissa, truncate.
-// E[round(x)] == x.  NaN/Inf pass through untouched.
+// E[round(x)] == x.  Inf passes through; a NaN whose payload lies only in the dropped low 16 bits gets the bf16 quiet
+// bit, so that it stays a NaN instead of becoming an inf.
 __device__ __forceinline__ uint16_t sr_bf16_bits(float x, uint32_t rnd16) {
   uint32_t b = __float_as_uint(x);
-  if ((b & 0x7F800000u) == 0x7F800000u) return static_cast<uint16_t>(b >> 16);
+  if ((b & 0x7F800000u) == 0x7F800000u) return static_cast<uint16_t>((b >> 16) | ((b & 0xFFFFu) ? 0x40u : 0u));
   b += (rnd16 & 0xFFFFu);
   return static_cast<uint16_t>(b >> 16);
 }

@@ -102,12 +102,16 @@ class StochasticAdamW(Optimizer):
 
     @torch.no_grad()
     def step(self, closure: None = None) -> None:  # type: ignore[override]
+        """One fused launch per (step count, gradient dtype) bucket of each parameter group.  Parameters without a
+        gradient are skipped and keep their state.  Each launch draws one seed from the generator: groups in order, and
+        within a group the buckets in the order of their first parameter."""
         if closure is not None:
             raise ValueError("Closure is not supported")
         for gi, group in enumerate(self.param_groups):
             beta1, beta2 = group["betas"]
             # bucket by (step, grad dtype): one fused launch per bucket (normally exactly one per group)
             buckets: dict[tuple[int, torch.dtype], list[tuple[torch.Tensor, ...]]] = {}
+            first: dict[tuple[int, torch.dtype], int] = {}
             for p in group["params"]:
                 if p.grad is None:
                     continue
@@ -120,12 +124,15 @@ class StochasticAdamW(Optimizer):
                     state["exp_avg_sq"] = _new_state(p, group["state_dtype"])
                 state["step"] += 1
                 key = (int(state["step"]), _local(p.grad).dtype)
+                first.setdefault(key, id(p))
                 buckets.setdefault(key, []).append(
                     (_local(p), _local(p.grad), _local(state["exp_avg"]), _local(state["exp_avg_sq"]))
                 )
             for (step, grad_dtype), items in buckets.items():
                 ps, gs, ms, vs = (list(col) for col in zip(*items, strict=True))
-                plan_key = (gi, step == 1, grad_dtype, len(ps))
+                # a bucket's plan is found again by its first parameter, not its step count: a parameter that got its
+                # first gradient later lags by a step for good, and its bucket must not evict the group's plan
+                plan_key = (gi, grad_dtype, first[(step, grad_dtype)], len(ps))
                 self._plans[plan_key] = adamw_stochastic_bf16_multi_(
                     ps, gs, ms, vs, lr=group["lr"], beta1=beta1, beta2=beta2, eps=group["eps"],
                     weight_decay=group["weight_decay"], step=step, generator=self._generator,

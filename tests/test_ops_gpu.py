@@ -285,59 +285,6 @@ def test_silu_mul_probs(ops):
     assert _rel_err(dx, xr.grad) < 1e-2 and _rel_err(dy, yr.grad) < 1e-2 and _rel_err(dp, pr.grad) < 1e-3
 
 
-# ----------------------------------------------------------------------------- stochastic rounding
-def test_sr_copy_statistics(ops):
-    n = 1 << 20
-    src = torch.full((n,), 1.0 + 2.0**-10, device="cuda")  # between two bf16 values (spacing 2^-7)
-    dst = torch.empty(n, device="cuda", dtype=torch.bfloat16)
-    ops.sr_copy_(dst, src, 123)
-    assert abs(dst.float().mean().item() - src[0].item()) < 2e-4  # unbiased
-    vals = dst.float().unique()
-    assert len(vals) == 2
-    dst2 = torch.empty_like(dst)
-    ops.sr_copy_(dst2, src, 123)
-    assert torch.equal(dst, dst2)  # reproducible for a (seed, offset)
-    ops.sr_copy_(dst2, src, 124)
-    assert not torch.equal(dst, dst2)
-    x = torch.randn(1001, device="cuda")
-    y = torch.empty(1001, device="cuda", dtype=torch.bfloat16)
-    ops.sr_copy_(y, x, 5)
-    assert (y.float() - x).abs().max() < 2.0**-7 * x.abs().max() * 1.01
-    exact = torch.randn(4096, device="cuda").bfloat16().float()
-    y2 = torch.empty(4096, device="cuda", dtype=torch.bfloat16)
-    ops.sr_copy_(y2, exact, 9)
-    assert torch.equal(y2.float(), exact)  # representable values are never perturbed
-
-
-# ----------------------------------------------------------------------------- AdamW
-@pytest.mark.parametrize("grad_dtype", [torch.float32, torch.bfloat16])
-@pytest.mark.parametrize("state_dtype", [torch.float32, torch.bfloat16])
-def test_adamw_sr_multi(grad_dtype, state_dtype):
-    from d9d_b200.kernel.stochastic import adamw_stochastic_bf16_multi_
-
-    sizes = [5, 1000, 8192, 8193, 70001]
-    ps = [torch.randn(s, device="cuda").bfloat16() for s in sizes]
-    gs = [torch.randn(s, device="cuda").to(grad_dtype) for s in sizes]
-    ms = [(torch.randn(s, device="cuda") * 0.1).to(state_dtype) for s in sizes]
-    vs = [(torch.rand(s, device="cuda") * 0.1).to(state_dtype) for s in sizes]
-    p0 = [p.float().clone() for p in ps]
-    m0 = [m.float().clone() for m in ms]
-    v0 = [v.float().clone() for v in vs]
-    lr, b1, b2, eps, wd, step = 1e-2, 0.9, 0.95, 1e-8, 0.1, 3
-    adamw_stochastic_bf16_multi_(ps, gs, ms, vs, lr=lr, beta1=b1, beta2=b2, eps=eps, weight_decay=wd, step=step, seed=77)
-    for p, g, m, v, pp, mm, vv in zip(ps, gs, ms, vs, p0, m0, v0):
-        gf = g.float()
-        pe = pp * (1 - lr * wd)
-        me = b1 * mm + (1 - b1) * gf
-        ve = b2 * vv + (1 - b2) * gf * gf
-        pe = pe - lr * (me / (1 - b1**step)) / ((ve / (1 - b2**step)).sqrt() + eps)
-        ulp = pe.abs().clamp_min(1e-30) * 2.0**-7
-        assert ((p.float() - pe).abs() <= ulp * 1.01 + 1e-30).all()
-        tol = 2.0**-7 if state_dtype == torch.bfloat16 else 1e-6
-        assert ((m.float() - me).abs() <= me.abs() * tol + 1e-7).all()
-        assert ((v.float() - ve).abs() <= ve.abs() * tol + 1e-7).all()
-
-
 # ----------------------------------------------------------------------------- RoPE
 @pytest.mark.parametrize("D,rope_dim", [(128, 128), (64, 64), (128, 64), (256, 256)])
 @pytest.mark.parametrize("style", [0, 1])
