@@ -1,7 +1,9 @@
 """The fused router kernel (``route_topk``) against the PyTorch definition (``route_topk_general``), forward and
 forward+backward, on the DeepSeek-V3 routing (sigmoid scores, 8 groups of which 4 stay eligible, bias, renormalised,
 scale 2.5, E = 256, k = 8) and on the flagship softmax router (Qwen3-MoE: E = 128, k = 8), whose kernel path the
-DeepSeek options leave unchanged.
+DeepSeek options leave unchanged.  An auxiliary-loss arm times the fused kernel with the load-balancing and router z
+losses off and on, at the flagship shape and at a group-limited softmax shape (DeepSeek-V2 style: E = 160, 8 groups of
+which 3 stay eligible, k = 6).
 
 Timing: CUDA events around ``--iters`` back-to-back calls after ``--warmup`` calls; median of ``--repeats`` windows.
 Usage: python benchmarks/bench_router.py [--out results/bench_router.json]
@@ -26,6 +28,11 @@ SHAPES = [  # name, T, E, k, options
     ("deepseek_v3", 16384, 256, 8, {"score_function": "sigmoid", "num_groups": 8, "topk_groups": 4, "scaling_factor": 2.5}),
     ("flagship_softmax", 16384, 128, 8, {}),
 ]
+AUX_SHAPES = [  # name, T, E, k, options; renormalised
+    ("flagship_softmax", 16384, 128, 8, {}),
+    ("grouped_softmax", 16384, 160, 6, {"num_groups": 8, "topk_groups": 3}),
+]
+AUX_ON = {"load_balancing_coef": 1e-2, "z_loss_coef": 1e-3, "token_loss_weight": 1e-3}
 
 
 def _time_ms(fn, iters: int, warmup: int, repeats: int) -> float:
@@ -79,6 +86,28 @@ def main() -> None:
         row["speedup_fwd"] = round(row["general_fwd_us"] / row["native_fwd_us"], 2)
         row["speedup_fwd_bwd"] = round(row["general_fwd_bwd_us"] / row["native_fwd_bwd_us"], 2)
         results["shapes"].append(row)
+        print(json.dumps(row), flush=True)
+    results["aux_shapes"] = []
+    for name, T, E, k, opts in AUX_SHAPES:
+        torch.manual_seed(0)
+        x = torch.randn(T, E, device="cuda").bfloat16().requires_grad_()
+        dprobs = torch.randn(T, k, device="cuda")
+        sums = torch.zeros(3, device="cuda")
+        row = {"name": name, "T": T, "E": E, "k": k, **opts}
+        for arm, aux in (("off", {}), ("on", {**AUX_ON, "aux_loss_sums": sums})):
+
+            def fwd(aux=aux):
+                with torch.no_grad():
+                    route_topk(x, k, True, **opts, **aux)
+
+            def fwd_bwd(aux=aux):
+                _, probs = route_topk(x, k, True, **opts, **aux)
+                x.grad = None
+                probs.backward(dprobs)
+
+            row[f"aux_{arm}_fwd_us"] = round(1e3 * _time_ms(fwd, args.iters, args.warmup, args.repeats), 2)
+            row[f"aux_{arm}_fwd_bwd_us"] = round(1e3 * _time_ms(fwd_bwd, args.iters, args.warmup, args.repeats), 2)
+        results["aux_shapes"].append(row)
         print(json.dumps(row), flush=True)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

@@ -1,5 +1,17 @@
 """Fused MoE routing: fp32 softmax or sigmoid scores + top-k (+ selection bias, + group-limited selection, + renormalisation,
-+ scaling) and its backward."""
++ scaling) and its backward, optionally with the softmax router's auxiliary losses folded into that backward.
+
+Auxiliary losses of one call (``T`` tokens, ``E`` experts, top-``k``, ``s = softmax(logits)`` in fp32 - unbiased, not
+renormalised, not scaled - and ``c_e`` the number of the ``T k`` selections that went to expert ``e``):
+
+* load balancing (Switch Transformer): ``A = E sum_e f_e P_e`` with ``f_e = c_e / (k T)`` (no gradient) and
+  ``P_e = mean_t s[t, e]``; 1 when balanced, up to ``E / k`` when every token picks the same ``k`` experts;
+* router z-loss (ST-MoE): ``Z = mean_t lse_t^2`` with ``lse_t = logsumexp_e logits[t, e]``.
+
+With ``w`` the loss weight per token, the call's auxiliary objective ``w T (coef_lb A + coef_z Z)`` is back-propagated by
+adding its gradient to the logits' gradient in backward, and ``(w T A, w T Z, w T)`` is added to an optional fp32 ``[3]``
+accumulator there - once per call, even when activation recomputation runs the forward twice.
+"""
 
 from __future__ import annotations
 
@@ -10,6 +22,53 @@ import torch.nn.functional as F
 from torch.autograd import Function
 
 from .._native import native_ops, on_gpu
+
+
+def _aux_terms(counts: torch.Tensor, score_sum: torch.Tensor, lse2_sum: torch.Tensor, num_tokens: int, top_k: int,
+               lb_coef: float, z_coef: float, token_weight: float) -> tuple[torch.Tensor, float, torch.Tensor]:
+    """One call's statistics (``counts [E]``, ``score_sum [E] = sum_t s[t]``, ``lse2_sum [1] = sum_t lse_t^2``) ->
+    ``g [E]`` fp32 (load balancing: ``dlogits[t] += s_t (g - s_t . g)``), the z-loss factor ``2 w coef_z``
+    (``dlogits[t] += 2 w coef_z lse_t s_t``) and ``(w T A, w T Z, w T)`` fp32 ``[3]``."""
+    num_experts = counts.numel()
+    t = max(num_tokens, 1)  # no tokens: no counts, no gradient, weight 0
+    omega = token_weight * num_tokens
+    c = counts.float()
+    g = c * (token_weight * lb_coef * num_experts / (top_k * t))
+    logged = torch.cat([
+        torch.dot(c, score_sum.float()).reshape(1) * (omega * num_experts / (top_k * t * t)),
+        lse2_sum.float().reshape(1) * (omega / t),
+        lse2_sum.new_full((1,), omega, dtype=torch.float32),
+    ])
+    return g, 2.0 * token_weight * z_coef, logged
+
+
+class _AuxLossGrad(Function):
+    """CPU path (and numerics oracle) of the auxiliary losses: identity on the selected probabilities; backward adds
+    ``w T (coef_lb grad A + coef_z grad Z)`` to the logits' gradient, in fp32 from the plain PyTorch definitions."""
+
+    @staticmethod
+    def forward(ctx: Any, chosen_p: torch.Tensor, logits: torch.Tensor, chosen: torch.Tensor, top_k: int, lb_coef: float,
+                z_coef: float, token_weight: float, sums: torch.Tensor | None):
+        ctx.save_for_backward(logits.detach(), chosen)
+        ctx.args = (top_k, lb_coef, z_coef, token_weight, sums)
+        return chosen_p.view_as(chosen_p)
+
+    @staticmethod
+    def backward(ctx: Any, dprobs: torch.Tensor):  # type: ignore[override]
+        logits, chosen = ctx.saved_tensors
+        top_k, lb_coef, z_coef, token_weight, sums = ctx.args
+        x = logits.reshape(-1, logits.shape[-1]).float()
+        s = F.softmax(x, dim=-1)
+        lse = torch.logsumexp(x, dim=-1)
+        counts = torch.bincount(chosen.reshape(-1), minlength=x.shape[-1])
+        g, zc, logged = _aux_terms(counts, s.sum(0), (lse * lse).sum().reshape(1), x.shape[0], top_k, lb_coef, z_coef,
+                                   token_weight)
+        dlogits = s * (g - (s @ g)[:, None]) + zc * lse[:, None] * s
+        if sums is not None:
+            sums.add_(logged)
+        # autograd adds this term to the selection gradient in the logits' dtype: exact for the fp32 logits the oracle
+        # is used with; for bf16 logits each term is rounded once before the sum (the kernel rounds their fp32 sum)
+        return dprobs, dlogits.to(logits.dtype).reshape(logits.shape), None, None, None, None, None, None
 
 
 def route_topk_reference(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None):
@@ -44,6 +103,32 @@ class _RouteTopK(Function):
         dlogits = native_ops().router_topk_bwd(logits, idx, dprobs.float().contiguous(), ctx.renormalize, ctx.score_function,
                                                ctx.scaling_factor)
         return dlogits, None, None, None, None, None, None, None
+
+
+class _RouteTopKAux(Function):
+    """Softmax routing on the fused kernel with the auxiliary-loss statistics from the same pass (deterministic, so a
+    recomputed forward reproduces them bit for bit) and both auxiliary gradients folded into the fused backward."""
+
+    @staticmethod
+    def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None,
+                num_groups: int, topk_groups: int, scaling_factor: float, lb_coef: float, z_coef: float, token_weight: float,
+                sums: torch.Tensor | None):
+        idx, probs, counts, score_sum, lse2_sum = native_ops().router_topk_aux_fwd(
+            logits, expert_bias, top_k, renormalize, num_groups, topk_groups, scaling_factor)
+        ctx.save_for_backward(logits, idx, counts, score_sum, lse2_sum)
+        ctx.args = (renormalize, scaling_factor, top_k, lb_coef, z_coef, token_weight, sums)
+        ctx.mark_non_differentiable(idx)
+        return idx, probs
+
+    @staticmethod
+    def backward(ctx: Any, _didx: torch.Tensor, dprobs: torch.Tensor):  # type: ignore[override]
+        logits, idx, counts, score_sum, lse2_sum = ctx.saved_tensors
+        renormalize, scaling_factor, top_k, lb_coef, z_coef, token_weight, sums = ctx.args
+        g, zc, logged = _aux_terms(counts, score_sum, lse2_sum, logits.shape[0], top_k, lb_coef, z_coef, token_weight)
+        dlogits = native_ops().router_topk_aux_bwd(logits, idx, dprobs.float().contiguous(), renormalize, scaling_factor, g, zc)
+        if sums is not None:
+            sums.add_(logged)
+        return dlogits, None, None, None, None, None, None, None, None, None, None
 
 
 def route_topk_general(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None,
@@ -81,31 +166,60 @@ def route_topk_general(logits: torch.Tensor, top_k: int, renormalize: bool, expe
 
 
 def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None,
-               score_function: str = "softmax", num_groups: int = 1, topk_groups: int = 1, scaling_factor: float = 1.0):
+               score_function: str = "softmax", num_groups: int = 1, topk_groups: int = 1, scaling_factor: float = 1.0, *,
+               load_balancing_coef: float = 0.0, z_loss_coef: float = 0.0, token_loss_weight: float | None = None,
+               aux_loss_sums: torch.Tensor | None = None):
     """``logits [..., E]`` -> ``(indices [..., k] int64, probabilities [..., k] fp32)``.
 
     bf16 CUDA logits with ``E <= 1024``, ``k <= min(32, E)`` and at most 32 expert groups run on the fused CUDA kernel,
     whatever the routing options (softmax or sigmoid scores, bias, group-limited selection, renormalisation, scaling).
     Other inputs use the PyTorch definitions: ``route_topk_reference`` for plain softmax top-k, ``route_topk_general``
     for the DeepSeek variants.
+
+    Auxiliary losses (softmax scores only; see the module docstring): with ``load_balancing_coef > 0`` or
+    ``z_loss_coef > 0`` the backward also adds the gradient of ``token_loss_weight * T * (load_balancing_coef * A +
+    z_loss_coef * Z)`` to the logits, and adds ``(w T A, w T Z, w T)`` to ``aux_loss_sums`` (fp32 ``[3]``, optional).
+    With both coefficients 0 the call is exactly the one without them.
     """
     num_experts = logits.shape[-1]
     if num_groups > 1 and (num_experts % num_groups != 0 or not 0 < topk_groups <= num_groups):
         raise ValueError("experts must split evenly into groups and 0 < topk_groups <= num_groups")
     if score_function not in ("softmax", "sigmoid"):
         raise ValueError(f"unknown router score function {score_function!r}")
+    if load_balancing_coef < 0 or z_loss_coef < 0:
+        raise ValueError("auxiliary loss coefficients must be non-negative")
+    aux = load_balancing_coef > 0 or z_loss_coef > 0
+    if aux:
+        if score_function != "softmax":
+            raise ValueError("the load-balancing and z auxiliary losses are defined for softmax routers only")
+        if token_loss_weight is None:
+            raise ValueError("auxiliary losses need token_loss_weight, the loss weight of one token")
+        if aux_loss_sums is not None and (aux_loss_sums.dtype != torch.float32 or aux_loss_sums.shape != (3,)
+                                          or aux_loss_sums.device != logits.device):
+            raise ValueError("aux_loss_sums must be an fp32 [3] tensor on the logits' device")
     if (on_gpu(logits) and logits.dtype == torch.bfloat16 and num_experts <= 1024 and top_k <= min(32, num_experts)
             and num_groups <= 32):
         flat = logits.reshape(logits.shape[:-1].numel(), num_experts)  # also when there are no tokens
         if not flat.is_contiguous():
             flat = flat.contiguous()
         groups = (num_groups, topk_groups) if num_groups > 1 else (1, 1)
-        idx, probs = _RouteTopK.apply(flat, top_k, renormalize, None if expert_bias is None else expert_bias.float().contiguous(),
-                                      score_function, *groups, float(scaling_factor))
+        bias = None if expert_bias is None else expert_bias.float().contiguous()
+        if aux:
+            idx, probs = _RouteTopKAux.apply(flat, top_k, renormalize, bias, *groups, float(scaling_factor),
+                                             float(load_balancing_coef), float(z_loss_coef), float(token_loss_weight),
+                                             aux_loss_sums)
+        else:
+            idx, probs = _RouteTopK.apply(flat, top_k, renormalize, bias, score_function, *groups, float(scaling_factor))
         return idx.view(*logits.shape[:-1], top_k), probs.view(*logits.shape[:-1], top_k)
     if score_function != "softmax" or num_groups > 1 or scaling_factor != 1.0:
-        return route_topk_general(logits, top_k, renormalize, expert_bias, score_function, num_groups, topk_groups, scaling_factor)
-    return route_topk_reference(logits, top_k, renormalize, expert_bias)
+        chosen, chosen_p = route_topk_general(logits, top_k, renormalize, expert_bias, score_function, num_groups, topk_groups,
+                                              scaling_factor)
+    else:
+        chosen, chosen_p = route_topk_reference(logits, top_k, renormalize, expert_bias)
+    if aux:
+        chosen_p = _AuxLossGrad.apply(chosen_p, logits, chosen, top_k, float(load_balancing_coef), float(z_loss_coef),
+                                      float(token_loss_weight), aux_loss_sums)
+    return chosen, chosen_p
 
 
 __all__ = ["route_topk", "route_topk_general", "route_topk_reference"]

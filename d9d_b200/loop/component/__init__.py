@@ -4,6 +4,7 @@ from .batch_maths import BatchMaths
 from .checkpointer import StateCheckpointer
 from .data_loader_factory import DataLoaderFactory, IteratorBatchGroup, StatefulDataLoaderDataParallelAware
 from .expert_bias_balancer import ExpertBiasBalancer
+from .moe_aux_loss import MoEAuxLoss
 from .garbage_collector import ManualGarbageCollector
 from .gradient_clipper import GradientClipper
 from .gradient_manager import GradientManager
@@ -24,6 +25,7 @@ __all__ = [
     "DataLoaderFactory",
     "ExpertBiasBalancer",
     "ForwardResult",
+    "MoEAuxLoss",
     "GradientClipper",
     "GradientManager",
     "InferenceProcessor",

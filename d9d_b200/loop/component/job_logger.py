@@ -98,6 +98,10 @@ class JobLogger(Stateful):
     def _due(self) -> bool:
         return self._stepper.should_do_action(self._config.period_steps, enable_on_last_step_if_periodic=True)
 
+    def is_due(self) -> bool:
+        """Whether this step logs the metrics (the same answer on every rank)."""
+        return self._due()
+
     def trigger_sync(self) -> None:
         if self._due():
             self._collector.schedule_collection(self._ctx)

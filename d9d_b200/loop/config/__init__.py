@@ -13,6 +13,7 @@ from .config import (
     JobLoggerConfig,
     Fp8LinearConfig,
     ModelStageFactoryConfig,
+    MoEAuxLossConfig,
     PipeliningConfig,
     ProfilingConfig,
     TimeoutConfig,
@@ -26,6 +27,7 @@ __all__ = [
     "DataLoadingConfig",
     "DeterminismConfig",
     "ExpertBiasBalancingConfig",
+    "MoEAuxLossConfig",
     "GarbageCollectionConfig",
     "GradientClippingConfig",
     "GradientManagerConfig",

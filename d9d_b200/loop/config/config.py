@@ -1,7 +1,7 @@
 from pathlib import Path
 from typing import Literal
 
-from pydantic import BaseModel
+from pydantic import BaseModel, NonNegativeFloat
 
 from d9d_b200.pipelining.factory import AnyPipelineScheduleConfig
 from d9d_b200.tracker import AnyTrackerConfig, RunConfig
@@ -93,6 +93,19 @@ class ExpertBiasBalancingConfig(BaseModel):
     update_rate: float
 
 
+class MoEAuxLossConfig(BaseModel):
+    """Train softmax MoE routers with the Switch Transformer load-balancing loss and the ST-MoE router z-loss, per MoE layer
+    and forward: ``load_balancing_coef * A + z_loss_coef * Z`` with ``A = E sum_e f_e P_e`` (``f_e``: share of the ``T k``
+    selections that went to expert ``e``, ``P_e``: mean softmax score of expert ``e``) and ``Z = mean_t logsumexp(x_t)^2``,
+    weighted like the LM loss (``T * LOSS_WEIGHT_PER_TOKEN``) and summed over the MoE layers.  ``A`` is ``k`` times
+    smaller than Hugging Face's ``load_balancing_loss_func``, which also averages over layers: HF's
+    ``router_aux_loss_coef`` ``c`` corresponds to ``load_balancing_coef = c * k / num_moe_layers``.  Sigmoid routers are
+    refused (they balance with ``expert_bias_balancing``)."""
+
+    load_balancing_coef: NonNegativeFloat = 0.0
+    z_loss_coef: NonNegativeFloat = 0.0
+
+
 class TimeoutConfig(BaseModel):
     init_timeout: int = 10000
     step_timeout: int = 100
@@ -113,6 +126,7 @@ class TrainerConfig(BaseModel):
     gradient_manager: GradientManagerConfig
     timeout: TimeoutConfig = TimeoutConfig()
     expert_bias_balancing: ExpertBiasBalancingConfig | None = None  # None: expert biases stay as loaded
+    moe_aux_loss: MoEAuxLossConfig | None = None  # None: routers train without auxiliary losses
 
 
 class InferenceConfig(BaseModel):

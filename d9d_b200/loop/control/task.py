@@ -69,6 +69,12 @@ class ComputeLossContext:
     stepper: "Stepper"
 
 
+# Loss weight of one token: ``CausalLMTask`` weighs a microbatch of ``n`` target tokens ``n * LOSS_WEIGHT_PER_TOKEN``, and
+# the MoE routers' auxiliary losses weigh a forward of ``T`` tokens ``T * LOSS_WEIGHT_PER_TOKEN``, so both are
+# token-weighted means in the same units.
+LOSS_WEIGHT_PER_TOKEN = 1 / 1000
+
+
 @dataclasses.dataclass(kw_only=True)
 class ComputeLossResult:
     loss: torch.Tensor

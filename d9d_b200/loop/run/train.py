@@ -80,6 +80,8 @@ class TrainingConfigurator:
             garbage_collector=house.gc, checkpointer=house.checkpointer, profiler=house.profiler, timeout_manager=base.timeout,
             expert_bias_balancer=parts.ExpertBiasBalancer(dist_context=ctx, tracked_modules=modules, config=cfg.expert_bias_balancing)
             if cfg.expert_bias_balancing is not None else None,
+            moe_aux_loss=parts.MoEAuxLoss(dist_context=ctx, tracked_modules=modules, config=cfg.moe_aux_loss)
+            if cfg.moe_aux_loss is not None else None,
         )
 
     def configure(self) -> "Trainer":
@@ -91,7 +93,8 @@ class Trainer:
 
     One iteration == one optimizer step: forward/backward over the accumulation group (gradient buckets all-reduce
     on the side stream as they fill), metric sync kicked off asynchronously, gradient wait + ``1/sum(w)`` scaling,
-    clipping, optimizer, expert-bias balancing (when configured), LR scheduler, logging, ``zero_grad``, housekeeping, post-step checkpoint.
+    clipping, optimizer, expert-bias balancing (when configured), LR scheduler, logging (+ the MoE auxiliary losses when
+    configured), ``zero_grad``, housekeeping, post-step checkpoint.
     """
 
     def __init__(self, state: TrainJobState):
@@ -128,6 +131,8 @@ class Trainer:
                 s.event_bus.trigger(events.EVENT_TRAIN_STEP_PRE, step_ctx)
                 if s.expert_bias_balancer is not None:
                     s.expert_bias_balancer.reset_counters()
+                if s.moe_aux_loss is not None:
+                    s.moe_aux_loss.reset()
                 with s.event_bus.bounded(events.EVENT_TRAIN_FORWARD_BACKWARD_PRE, events.EVENT_TRAIN_FORWARD_BACKWARD_POST, step_ctx):
                     for batch in batch_group:
                         result = s.task_operator.forward_backward(batch)
@@ -142,6 +147,8 @@ class Trainer:
                     s.expert_bias_balancer.update()
                 s.lr_scheduler.step()
                 s.logger.log(run, loss_value=s.gradient_manager.compute_global_loss())
+                if s.moe_aux_loss is not None and s.logger.is_due():
+                    s.moe_aux_loss.log(run)
                 s.gradient_manager.zero_grad()
                 gc.collect_periodic()
                 if profiler:

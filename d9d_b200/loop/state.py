@@ -18,6 +18,7 @@ from d9d_b200.core.protocol import LRSchedulerProtocol, OptimizerProtocol
 from d9d_b200.loop.component import (
     BatchMaths,
     ExpertBiasBalancer,
+    MoEAuxLoss,
     GradientClipper,
     GradientManager,
     InferenceTaskOperator,
@@ -83,6 +84,7 @@ class TrainJobState(JobState):
     gradient_clipper: GradientClipper
     exporter: ModelStageExporter
     expert_bias_balancer: ExpertBiasBalancer | None = None
+    moe_aux_loss: MoEAuxLoss | None = None  # not checkpointed: its sums restart every step
 
 
 @dataclasses.dataclass(kw_only=True)

@@ -32,6 +32,11 @@ class TopKRouter(nn.Module, ModuleLateInit):
     """Linear gate -> fp32 softmax over all experts -> top-k (optionally biased selection) -> optional renorm
     (softmax / selection / renormalisation are one fused kernel on CUDA, ``ops/csrc/router.cu``).
 
+    Softmax routers can also train with the load-balancing and router z auxiliary losses (``set_aux_loss``, off by
+    default; definitions in ``d9d_b200.kernel.router``): their gradients are added in the router's backward, and
+    ``aux_loss_sums`` (fp32, not saved) accumulates ``(sum w T A, sum w T Z, sum w T)`` over the backward passes since
+    ``reset_aux_loss_sums``.
+
     Parity: reference ``d9d/module/block/moe/router.py:24-107``.
     """
 
@@ -44,19 +49,51 @@ class TopKRouter(nn.Module, ModuleLateInit):
             nn.Buffer(torch.empty(num_experts, dtype=torch.float32), persistent=True)
             if (enable_expert_bias or options.enable_expert_bias) else None
         )
+        self.aux_loss_sums = nn.Buffer(torch.empty(3, dtype=torch.float32), persistent=False)
         self._num_experts = num_experts
         self._top_k = top_k
         self._renormalize = renormalize_probabilities
         self._options = options
+        self._load_balancing_coef = 0.0
+        self._z_loss_coef = 0.0
+        self._token_loss_weight: float | None = None
+
+    @property
+    def score_function(self) -> str:
+        return self._options.score_function
+
+    def set_aux_loss(self, load_balancing_coef: float, z_loss_coef: float, token_loss_weight: float) -> None:
+        """Train with ``token_loss_weight * T * (load_balancing_coef * A + z_loss_coef * Z)`` per forward of ``T``
+        tokens (softmax routers only; both coefficients 0 switch the losses off)."""
+        if load_balancing_coef < 0 or z_loss_coef < 0:
+            raise ValueError("auxiliary loss coefficients must be non-negative")
+        if (load_balancing_coef > 0 or z_loss_coef > 0) and self.score_function != "softmax":
+            raise ValueError(f"the load-balancing and z auxiliary losses need a softmax router, not {self.score_function!r} "
+                             "(sigmoid routers balance with the expert bias)")
+        self._load_balancing_coef = float(load_balancing_coef)
+        self._z_loss_coef = float(z_loss_coef)
+        self._token_loss_weight = float(token_loss_weight)
+
+    @torch.no_grad()
+    def reset_aux_loss_sums(self) -> None:
+        if self.aux_loss_sums.dtype == torch.float32:
+            self.aux_loss_sums.zero_()
+        else:  # the module was cast whole: the sums stay fp32
+            self.aux_loss_sums = torch.zeros(3, dtype=torch.float32, device=self.aux_loss_sums.device)
 
     def forward(self, hidden_states: torch.Tensor) -> RoutingResult:
         o = self._options
+        aux = {}
+        if self._load_balancing_coef > 0 or self._z_loss_coef > 0:
+            aux = {"load_balancing_coef": self._load_balancing_coef, "z_loss_coef": self._z_loss_coef,
+                   "token_loss_weight": self._token_loss_weight, "aux_loss_sums": self.aux_loss_sums}
         chosen, chosen_p = route_topk(self.gate(hidden_states), self._top_k, self._renormalize, self.expert_bias,
                                       score_function=o.score_function, num_groups=o.num_expert_groups,
-                                      topk_groups=o.topk_expert_groups, scaling_factor=o.routed_scaling_factor)
+                                      topk_groups=o.topk_expert_groups, scaling_factor=o.routed_scaling_factor, **aux)
         return RoutingResult(selected_expert_indices=chosen, selected_probabilities=chosen_p)
 
     def reset_parameters(self) -> None:
         if self.expert_bias is not None:
             nn.init.zeros_(self.expert_bias)
         self.gate.reset_parameters()
+        self.reset_aux_loss_sums()

@@ -206,6 +206,18 @@ void router_topk_fwd(const void* logits, const float* bias, long long T, int E, 
                      int num_groups, int topk_groups, float scale, long long* idx, float* probs, cudaStream_t stream);
 void router_topk_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
                      bool renorm, bool sigmoid, float scale, void* dlogits, cudaStream_t stream);
+// Softmax routing with the auxiliary-loss statistics, deterministic (no atomics): the same idx / probs, plus
+// counts [E] int32 (selections per expert), score_sum [E] = sum_t softmax(x_t)[e] and lse2_sum [1] = sum_t lse_t^2, via
+// part_counts [P, E], part_scores [P, E], part_lse2 [P] with P = router_aux_parts(T) (0 when T = 0: zeros are written).
+int router_aux_parts(long long T);
+void router_topk_aux_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, int num_groups,
+                         int topk_groups, float scale, long long* idx, float* probs, int* part_counts,
+                         float* part_scores, float* part_lse2, int* counts, float* score_sum, float* lse2_sum,
+                         cudaStream_t stream);
+// router_topk_bwd for softmax, plus the auxiliary gradients: dlogits[t, e] += s_e (g_e - sum_j s_j g_j) + z_coef lse_t s_e
+// with g [E] fp32 (load-balancing term) and z_coef = 2 w_tok coef_z (z-loss term)
+void router_topk_aux_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
+                         bool renorm, float scale, const float* g, float z_coef, void* dlogits, cudaStream_t stream);
 
 // ------------------------------------------------------------------ expert-parallel exchange over NVLink ----
 // peer_base: device array [world] of symmetric-arena base pointers; off_* are byte offsets of regions inside the arena.

@@ -2,8 +2,12 @@
 // selection bias, + optional DeepSeek-V3 group-limited selection, + optional renormalisation and scaling of the selected
 // scores) in one pass, one warp per token; and its backward.
 // Replaces softmax / topk (radix select + sort) / gather / div / sum launches of the eager path.
-// The options are template parameters: the plain softmax instantiations (<VPL, false, false, false> forward,
-// <VPL, false, false> backward) compile to the same instructions as before the options existed.
+// The options are template parameters: the plain softmax instantiations (<VPL, false, false, false, false> forward,
+// <VPL, false, false, false> backward) compile to the same instructions as before the options existed.
+// AUX (softmax only) adds the router's auxiliary losses: the forward also produces the per-expert selection counts,
+// sum_t s[t, e] and sum_t lse_t^2 (per-warp registers -> per-block partials in a fixed order -> router_aux_finalize_kernel,
+// no atomics, so two passes over the same logits agree bit for bit); the backward adds the load-balancing and z-loss
+// gradients to dlogits before its bf16 rounding.
 #include <stdexcept>
 
 #include "common.cuh"
@@ -16,8 +20,9 @@ constexpr float RENORM_EPS = 1e-20f;
 constexpr int ROUTER_WARPS = 8;  // 256 threads per block
 
 template <int VPL>  // experts per lane: E <= 32 * VPL
-__device__ __forceinline__ void load_row_softmax(const __nv_bfloat16* __restrict__ row, int E, int lane, float (&p)[VPL]) {
-  float mx = -INFINITY;
+__device__ __forceinline__ void load_row_softmax(const __nv_bfloat16* __restrict__ row, int E, int lane, float (&p)[VPL],
+                                                 float& mx, float& sum) {
+  mx = -INFINITY;
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
     const int e = lane + i * 32;  // strided ownership keeps global loads coalesced
@@ -25,7 +30,7 @@ __device__ __forceinline__ void load_row_softmax(const __nv_bfloat16* __restrict
     mx = fmaxf(mx, p[i]);
   }
   mx = warp_max(mx);
-  float sum = 0.f;
+  sum = 0.f;
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
     p[i] = (lane + i * 32 < E) ? __expf(p[i] - mx) : 0.f;
@@ -37,8 +42,10 @@ __device__ __forceinline__ void load_row_softmax(const __nv_bfloat16* __restrict
   for (int i = 0; i < VPL; ++i) p[i] *= inv;
 }
 
+// softmax also leaves the row max and the sum of exp(x - max) (lse = max + log(sum)); sigmoid leaves them untouched
 template <int VPL, bool SIGMOID>
-__device__ __forceinline__ void load_row_scores(const __nv_bfloat16* __restrict__ row, int E, int lane, float (&p)[VPL]) {
+__device__ __forceinline__ void load_row_scores(const __nv_bfloat16* __restrict__ row, int E, int lane, float (&p)[VPL],
+                                                float& mx, float& sum) {
   if constexpr (SIGMOID) {
 #pragma unroll
     for (int i = 0; i < VPL; ++i) {
@@ -48,7 +55,7 @@ __device__ __forceinline__ void load_row_scores(const __nv_bfloat16* __restrict_
 #pragma unroll
     for (int i = 0; i < VPL; ++i) p[i] = 1.f / (1.f + __expf(-p[i]));  // padding lanes are never selected
   } else {
-    load_row_softmax<VPL>(row, E, lane, p);
+    load_row_softmax<VPL>(row, E, lane, p, mx, sum);
   }
 }
 
@@ -102,17 +109,32 @@ __device__ __forceinline__ void mask_dropped_groups(float (&key)[VPL], float* __
 
 // The new option instantiations declare a minimum of one block per SM: without it ptxas caps some of them at 64 registers
 // and spills.  A minimum of 0 is the plain __launch_bounds__(256) of the softmax path.
-template <int VPL, bool SIGMOID, bool GROUPED, bool SCALED>
-__global__ void __launch_bounds__(256, GROUPED ? 1 : 0)
+// AUX: block b writes part_counts[b, E], part_scores[b, E] and part_lse2[b] (sums over the block's tokens).
+template <int VPL, bool SIGMOID, bool GROUPED, bool SCALED, bool AUX>
+__global__ void __launch_bounds__(256, (GROUPED || AUX) ? 1 : 0)
     router_fwd_kernel(const __nv_bfloat16* __restrict__ logits, const float* __restrict__ bias, long long T, int E, int k,
                       bool renorm, long long* __restrict__ idx_out, float* __restrict__ probs_out, int G,
-                      int topk_groups, float scale) {
+                      int topk_groups, float scale, int* __restrict__ part_counts, float* __restrict__ part_scores,
+                      float* __restrict__ part_lse2) {
+  static_assert(!(AUX && SIGMOID), "auxiliary losses are defined for softmax routers only");
   const int lane = threadIdx.x & 31;
   const long long warp = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  float acc_s[VPL], acc_lse2 = 0.f;  // AUX: lane-owned sum_t s[t, e] and (warp-uniform) sum_t lse_t^2
+  int acc_c[VPL];                    // AUX: lane-owned selection counts
+  if constexpr (AUX) {
+#pragma unroll
+    for (int i = 0; i < VPL; ++i) { acc_s[i] = 0.f; acc_c[i] = 0; }
+  }
   for (long long t = warp; t < T; t += warps) {
-    float p[VPL], key[VPL];
-    load_row_scores<VPL, SIGMOID>(logits + t * E, E, lane, p);
+    float p[VPL], key[VPL], mx, sum;
+    load_row_scores<VPL, SIGMOID>(logits + t * E, E, lane, p, mx, sum);
+    if constexpr (AUX) {
+#pragma unroll
+      for (int i = 0; i < VPL; ++i) acc_s[i] += p[i];  // padding lanes hold 0
+      const float lse = mx + __logf(sum);
+      acc_lse2 += lse * lse;
+    }
 #pragma unroll
     for (int i = 0; i < VPL; ++i) {
       const int e = lane + i * 32;
@@ -125,6 +147,7 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0)
     float sel_p = 0.f;   // lane j keeps the j-th selection
     int sel_e = 0;
     float total = 0.f;
+    unsigned picked = 0u;  // AUX: bit i set when this lane's expert lane + 32 i was selected
     for (int j = 0; j < k; ++j) {
       // arg-max over the warp; ties go to the lower expert index
       float best = -INFINITY;
@@ -142,7 +165,10 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0)
         const float op = __shfl_xor_sync(0xffffffffu, best_p, off);
         if (ob > best || (ob == best && oe < best_e)) { best = ob; best_e = oe; best_p = op; }
       }
-      if ((best_e & 31) == lane) key[best_e >> 5] = -INFINITY;  // owner retires the winner
+      if ((best_e & 31) == lane) {  // owner retires the winner
+        key[best_e >> 5] = -INFINITY;
+        if constexpr (AUX) picked |= 1u << (best_e >> 5);
+      }
       if (lane == j) { sel_p = best_p; sel_e = best_e; }
       total += best_p;
     }
@@ -152,22 +178,110 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0)
       if constexpr (SCALED) w *= scale;
       probs_out[t * k + lane] = w;
     }
+    if constexpr (AUX) {
+#pragma unroll
+      for (int i = 0; i < VPL; ++i) acc_c[i] += (picked >> i) & 1u;
+    }
+  }
+  if constexpr (AUX) {
+    // block reduction in warp order: s_*[e] = ((w0 + w1) + w2) + ...
+    __shared__ float s_scores[32 * VPL];
+    __shared__ int s_counts[32 * VPL];
+    __shared__ float s_lse2[ROUTER_WARPS];
+    const int w = threadIdx.x >> 5;
+    for (int r = 0; r < ROUTER_WARPS; ++r) {
+      if (w == r) {
+#pragma unroll
+        for (int i = 0; i < VPL; ++i) {
+          const int e = lane + i * 32;
+          if (e < E) {
+            s_scores[e] = r ? s_scores[e] + acc_s[i] : acc_s[i];
+            s_counts[e] = r ? s_counts[e] + acc_c[i] : acc_c[i];
+          }
+        }
+      }
+      __syncthreads();
+    }
+    if (lane == 0) s_lse2[w] = acc_lse2;
+    __syncthreads();
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+      part_scores[static_cast<long long>(blockIdx.x) * E + e] = s_scores[e];
+      part_counts[static_cast<long long>(blockIdx.x) * E + e] = s_counts[e];
+    }
+    if (threadIdx.x == 0) {
+      float v = 0.f;
+      for (int r = 0; r < ROUTER_WARPS; ++r) v += s_lse2[r];
+      part_lse2[blockIdx.x] = v;
+    }
+  }
+}
+
+// Sums the forward's [parts, E] partials in a fixed order.  Blocks of 32 x 32 threads: block b < ceil(E / 32) owns
+// experts 32 b + x, thread row y sums parts y, y + 32, ... and row 0 then adds the 32 row sums in order; the last block
+// sums part_lse2 the same way.  With no parts (T = 0) it writes zeros.
+__global__ void __launch_bounds__(1024)
+    router_aux_finalize_kernel(const int* __restrict__ part_counts, const float* __restrict__ part_scores,
+                               const float* __restrict__ part_lse2, int parts, int E, int* __restrict__ counts,
+                               float* __restrict__ score_sum, float* __restrict__ lse2_sum) {
+  __shared__ float s_sum[32][33];
+  __shared__ int s_cnt[32][33];
+  const int x = threadIdx.x, y = threadIdx.y;
+  if (static_cast<int>(blockIdx.x) * 32 < E) {  // block-uniform branch
+    const int e = blockIdx.x * 32 + x;
+    int c = 0;
+    float s = 0.f;
+    if (e < E) {
+      for (int b = y; b < parts; b += 32) {
+        c += part_counts[static_cast<long long>(b) * E + e];
+        s += part_scores[static_cast<long long>(b) * E + e];
+      }
+    }
+    s_cnt[y][x] = c;
+    s_sum[y][x] = s;
+    __syncthreads();
+    if (y == 0 && e < E) {
+      int cc = 0;
+      float ss = 0.f;
+      for (int r = 0; r < 32; ++r) { cc += s_cnt[r][x]; ss += s_sum[r][x]; }
+      counts[e] = cc;
+      score_sum[e] = ss;
+    }
+  } else {
+    const int tid = y * 32 + x;
+    float v = 0.f;
+    for (int b = tid; b < parts; b += 1024) v += part_lse2[b];
+    s_sum[y][x] = v;
+    __syncthreads();
+    if (tid == 0) {
+      float t = 0.f;
+      for (int r = 0; r < 32; ++r)
+        for (int q = 0; q < 32; ++q) t += s_sum[r][q];
+      *lse2_sum = t;
+    }
   }
 }
 
 // r_j = scale * s_j (/ (S + eps) when renorm).  With dr' = scale * dr: ds_j = (dr'_j - sum_i dr'_i r_i) / (S + eps) when
 // renorm, else dr'_j; dp = scatter(ds).  softmax: dlogits[e] = p_e * (dp_e - sum_j ds_j s_j); sigmoid: s_e (1 - s_e) dp_e.
-template <int VPL, bool SIGMOID, bool SCALED>
-__global__ void __launch_bounds__(256, (SIGMOID || SCALED) ? 1 : 0)
+// AUX (softmax): dlogits[e] += p_e * (g_e - sum_j p_j g_j) + z_coef * lse * p_e, folded in as dp_e += g_e and
+// inner += sum_j p_j g_j - z_coef * lse (g: load-balancing gradient per expert, z_coef = 2 w_tok coef_z).
+template <int VPL, bool SIGMOID, bool SCALED, bool AUX>
+__global__ void __launch_bounds__(256, (SIGMOID || SCALED || AUX) ? 1 : 0)
     router_bwd_kernel(const __nv_bfloat16* __restrict__ logits, const long long* __restrict__ idx,
                       const float* __restrict__ dprobs, long long T, int E, int k, bool renorm,
-                      __nv_bfloat16* __restrict__ dlogits, float scale) {
+                      __nv_bfloat16* __restrict__ dlogits, float scale, const float* __restrict__ g, float z_coef) {
+  static_assert(!(AUX && SIGMOID), "auxiliary losses are defined for softmax routers only");
   const int lane = threadIdx.x & 31;
   const long long warp = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  float gv[VPL];  // AUX: this lane's g_e, loaded once
+  if constexpr (AUX) {
+#pragma unroll
+    for (int i = 0; i < VPL; ++i) gv[i] = (lane + i * 32 < E) ? g[lane + i * 32] : 0.f;
+  }
   for (long long t = warp; t < T; t += warps) {
-    float p[VPL];
-    load_row_scores<VPL, SIGMOID>(logits + t * E, E, lane, p);
+    float p[VPL], mx, sum;
+    load_row_scores<VPL, SIGMOID>(logits + t * E, E, lane, p, mx, sum);
     // lane j < k handles selection j
     const int my_e = (lane < k) ? static_cast<int>(idx[t * k + lane]) : -1;
     float my_dr = (lane < k) ? dprobs[t * k + lane] : 0.f;
@@ -191,10 +305,20 @@ __global__ void __launch_bounds__(256, (SIGMOID || SCALED) ? 1 : 0)
       my_ds = (lane < k) ? (my_dr - dot) / S : 0.f;
     }
     float inner = 0.f;
-    if constexpr (!SIGMOID) inner = warp_sum(my_ds * my_s);
+    if constexpr (AUX) {
+      float pg = 0.f;
+#pragma unroll
+      for (int i = 0; i < VPL; ++i) pg += p[i] * gv[i];
+      inner = warp_sum(my_ds * my_s + pg) - z_coef * (mx + __logf(sum));
+    } else if constexpr (!SIGMOID) {
+      inner = warp_sum(my_ds * my_s);
+    }
     float dp[VPL];
 #pragma unroll
-    for (int i = 0; i < VPL; ++i) dp[i] = 0.f;
+    for (int i = 0; i < VPL; ++i) {
+      if constexpr (AUX) dp[i] = gv[i];
+      else dp[i] = 0.f;
+    }
     for (int j = 0; j < k; ++j) {
       const int e = __shfl_sync(0xffffffffu, my_e, j);
       const float d = __shfl_sync(0xffffffffu, my_ds, j);
@@ -228,35 +352,42 @@ inline int grid_for(long long T) {
   return static_cast<int>(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
 }
 
+// aux: softmax only, with part_* sized [grid_for(T), E] / [grid_for(T)]
 template <int VPL>
 void launch_fwd(const __nv_bfloat16* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
-                int G, int topk_groups, float scale, long long* idx, float* probs, cudaStream_t stream) {
+                int G, int topk_groups, float scale, long long* idx, float* probs, bool aux, int* part_counts,
+                float* part_scores, float* part_lse2, cudaStream_t stream) {
   const bool grouped = G > 1, scaled = scale != 1.f;
   const size_t smem = grouped ? sizeof(float) * ROUTER_WARPS * E : 0;  // <= 32 KiB for E <= 1024
-#define D9D_ROUTER_FWD(SIG, GRP, SCL)                                                                               \
-  if (sigmoid == SIG && grouped == GRP && scaled == SCL) {                                                          \
-    router_fwd_kernel<VPL, SIG, GRP, SCL><<<grid_for(T), 256, smem, stream>>>(logits, bias, T, E, k, renorm, idx,   \
-                                                                              probs, G, topk_groups, scale);        \
-    return;                                                                                                         \
+#define D9D_ROUTER_FWD(SIG, GRP, SCL, AUX)                                                                             \
+  if (sigmoid == SIG && grouped == GRP && scaled == SCL && aux == AUX) {                                               \
+    router_fwd_kernel<VPL, SIG, GRP, SCL, AUX><<<grid_for(T), 256, smem, stream>>>(                                    \
+        logits, bias, T, E, k, renorm, idx, probs, G, topk_groups, scale, part_counts, part_scores, part_lse2);      \
+    return;                                                                                                            \
   }
-  D9D_ROUTER_FWD(false, false, false) D9D_ROUTER_FWD(false, false, true)
-  D9D_ROUTER_FWD(false, true, false) D9D_ROUTER_FWD(false, true, true)
-  D9D_ROUTER_FWD(true, false, false) D9D_ROUTER_FWD(true, false, true)
-  D9D_ROUTER_FWD(true, true, false) D9D_ROUTER_FWD(true, true, true)
+  D9D_ROUTER_FWD(false, false, false, false) D9D_ROUTER_FWD(false, false, true, false)
+  D9D_ROUTER_FWD(false, true, false, false) D9D_ROUTER_FWD(false, true, true, false)
+  D9D_ROUTER_FWD(true, false, false, false) D9D_ROUTER_FWD(true, false, true, false)
+  D9D_ROUTER_FWD(true, true, false, false) D9D_ROUTER_FWD(true, true, true, false)
+  D9D_ROUTER_FWD(false, false, false, true) D9D_ROUTER_FWD(false, false, true, true)
+  D9D_ROUTER_FWD(false, true, false, true) D9D_ROUTER_FWD(false, true, true, true)
 #undef D9D_ROUTER_FWD
 }
 
 template <int VPL>
 void launch_bwd(const __nv_bfloat16* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                bool renorm, bool sigmoid, float scale, __nv_bfloat16* dlogits, cudaStream_t stream) {
-  const bool scaled = scale != 1.f;
-#define D9D_ROUTER_BWD(SIG, SCL)                                                                                     \
-  if (sigmoid == SIG && scaled == SCL) {                                                                             \
-    router_bwd_kernel<VPL, SIG, SCL><<<grid_for(T), 256, 0, stream>>>(logits, idx, dprobs, T, E, k, renorm, dlogits, \
-                                                                      scale);                                        \
+                bool renorm, bool sigmoid, float scale, __nv_bfloat16* dlogits, const float* g, float z_coef,
+                cudaStream_t stream) {
+  const bool scaled = scale != 1.f, aux = g != nullptr;
+#define D9D_ROUTER_BWD(SIG, SCL, AUX)                                                                                \
+  if (sigmoid == SIG && scaled == SCL && aux == AUX) {                                                               \
+    router_bwd_kernel<VPL, SIG, SCL, AUX><<<grid_for(T), 256, 0, stream>>>(logits, idx, dprobs, T, E, k, renorm,    \
+                                                                           dlogits, scale, g, z_coef);               \
     return;                                                                                                          \
   }
-  D9D_ROUTER_BWD(false, false) D9D_ROUTER_BWD(false, true) D9D_ROUTER_BWD(true, false) D9D_ROUTER_BWD(true, true)
+  D9D_ROUTER_BWD(false, false, false) D9D_ROUTER_BWD(false, true, false)
+  D9D_ROUTER_BWD(true, false, false) D9D_ROUTER_BWD(true, true, false)
+  D9D_ROUTER_BWD(false, false, true) D9D_ROUTER_BWD(false, true, true)
 #undef D9D_ROUTER_BWD
 }
 
@@ -272,22 +403,54 @@ void launch_bwd(const __nv_bfloat16* logits, const long long* idx, const float* 
     else LAUNCH<32>(__VA_ARGS__);             \
   } while (0)
 
+static void check_router_shape(int E, int k) {
+  if (E > 1024 || k > 32 || k > E) throw std::runtime_error("d9d router: E <= 1024 and k <= min(32, E) required");
+}
+
+static void check_router_groups(int E, int num_groups, int topk_groups) {
+  if (num_groups < 1 || num_groups > 32 || E % num_groups != 0 || topk_groups < 1 || topk_groups > num_groups)
+    throw std::runtime_error("d9d router: 1 <= num_groups <= 32 dividing E and 1 <= topk_groups <= num_groups required");
+}
+
 void router_topk_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
                      int num_groups, int topk_groups, float scale, long long* idx, float* probs, cudaStream_t stream) {
   if (T == 0) return;
-  if (E > 1024 || k > 32 || k > E) throw std::runtime_error("d9d router: E <= 1024 and k <= min(32, E) required");
-  if (num_groups < 1 || num_groups > 32 || E % num_groups != 0 || topk_groups < 1 || topk_groups > num_groups)
-    throw std::runtime_error("d9d router: 1 <= num_groups <= 32 dividing E and 1 <= topk_groups <= num_groups required");
+  check_router_shape(E, k);
+  check_router_groups(E, num_groups, topk_groups);
   D9D_ROUTER_DISPATCH(launch_fwd, static_cast<const __nv_bfloat16*>(logits), bias, T, E, k, renorm, sigmoid,
-                      num_groups, topk_groups, scale, idx, probs, stream);
+                      num_groups, topk_groups, scale, idx, probs, false, nullptr, nullptr, nullptr, stream);
 }
 
 void router_topk_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
                      bool renorm, bool sigmoid, float scale, void* dlogits, cudaStream_t stream) {
   if (T == 0) return;
-  if (E > 1024 || k > 32 || k > E) throw std::runtime_error("d9d router: E <= 1024 and k <= min(32, E) required");
+  check_router_shape(E, k);
   D9D_ROUTER_DISPATCH(launch_bwd, static_cast<const __nv_bfloat16*>(logits), idx, dprobs, T, E, k, renorm, sigmoid,
-                      scale, static_cast<__nv_bfloat16*>(dlogits), stream);
+                      scale, static_cast<__nv_bfloat16*>(dlogits), nullptr, 0.f, stream);
+}
+
+int router_aux_parts(long long T) { return T > 0 ? grid_for(T) : 0; }
+
+void router_topk_aux_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, int num_groups,
+                         int topk_groups, float scale, long long* idx, float* probs, int* part_counts,
+                         float* part_scores, float* part_lse2, int* counts, float* score_sum, float* lse2_sum,
+                         cudaStream_t stream) {
+  check_router_shape(E, k);
+  check_router_groups(E, num_groups, topk_groups);
+  if (T > 0)
+    D9D_ROUTER_DISPATCH(launch_fwd, static_cast<const __nv_bfloat16*>(logits), bias, T, E, k, renorm, false,
+                        num_groups, topk_groups, scale, idx, probs, true, part_counts, part_scores, part_lse2, stream);
+  router_aux_finalize_kernel<<<(E + 31) / 32 + 1, dim3(32, 32), 0, stream>>>(part_counts, part_scores, part_lse2,
+                                                                             router_aux_parts(T), E, counts, score_sum,
+                                                                             lse2_sum);
+}
+
+void router_topk_aux_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
+                         bool renorm, float scale, const float* g, float z_coef, void* dlogits, cudaStream_t stream) {
+  if (T == 0) return;
+  check_router_shape(E, k);
+  D9D_ROUTER_DISPATCH(launch_bwd, static_cast<const __nv_bfloat16*>(logits), idx, dprobs, T, E, k, renorm, false,
+                      scale, static_cast<__nv_bfloat16*>(dlogits), g, z_coef, stream);
 }
 
 }  // namespace d9d

@@ -15,6 +15,7 @@ from d9d_b200.core.dist_context import DistributedContext
 from d9d_b200.core.types import ScalarTree
 from d9d_b200.dataset import SyntheticTokenDataset, shard_batch_along_sequence, shard_dataset_data_parallel
 from d9d_b200.loop.control import (
+    LOSS_WEIGHT_PER_TOKEN,
     BuildForwardInputsContext,
     BuildForwardInputsResult,
     ComputeLossContext,
@@ -134,8 +135,10 @@ class CausalLMTask(TrainTask):
     def compute_loss(self, ctx: ComputeLossContext) -> ComputeLossResult:
         num_tokens = (ctx.state["labels"] != LM_IGNORE_INDEX).sum()
         ctx.state["num_tokens"] = num_tokens
-        # a context-parallel rank may hold no target token of a microbatch: its loss is 0 with weight 0
-        return ComputeLossResult(loss=ctx.pipeline_results["logps"].sum() / num_tokens.clamp_min(1), loss_weight=num_tokens / 1000)
+        # a context-parallel rank may hold no target token of a microbatch: its loss is 0 with weight 0.  The count is
+        # divided by 1 / LOSS_WEIGHT_PER_TOKEN (exactly 1000.0): each weight is the correctly rounded fp32 n / 1000
+        return ComputeLossResult(loss=ctx.pipeline_results["logps"].sum() / num_tokens.clamp_min(1),
+                                 loss_weight=num_tokens / (1 / LOSS_WEIGHT_PER_TOKEN))
 
 
 class CausalLMPerplexityTask(InferenceTask):
