@@ -3,7 +3,8 @@ forward+backward, on the DeepSeek-V3 routing (sigmoid scores, 8 groups of which 
 scale 2.5, E = 256, k = 8) and on the flagship softmax router (Qwen3-MoE: E = 128, k = 8), whose kernel path the
 DeepSeek options leave unchanged.  An auxiliary-loss arm times the fused kernel with the load-balancing and router z
 losses off and on, at the flagship shape and at a group-limited softmax shape (DeepSeek-V2 style: E = 160, 8 groups of
-which 3 stay eligible, k = 6).
+which 3 stay eligible, k = 6).  A sequence-balance arm times the fused kernel with the sequence-wise balance loss off and
+on at the DeepSeek-V3 routing, T = 16 384 tokens in sequences of S = 4 096 (DeepSeek-V3's pre-training length).
 
 Timing: CUDA events around ``--iters`` back-to-back calls after ``--warmup`` calls; median of ``--repeats`` windows.
 Usage: python benchmarks/bench_router.py [--out results/bench_router.json]
@@ -33,6 +34,10 @@ AUX_SHAPES = [  # name, T, E, k, options; renormalised
     ("grouped_softmax", 16384, 160, 6, {"num_groups": 8, "topk_groups": 3}),
 ]
 AUX_ON = {"load_balancing_coef": 1e-2, "z_loss_coef": 1e-3, "token_loss_weight": 1e-3}
+SEQ_SHAPES = [  # name, T, E, k, sequence length, options; biased, renormalised
+    ("deepseek_v3", 16384, 256, 8, 4096, {"score_function": "sigmoid", "num_groups": 8, "topk_groups": 4, "scaling_factor": 2.5}),
+]
+SEQ_ON = {"sequence_balance_coef": 1e-4, "token_loss_weight": 1e-3}  # DeepSeek-V3's alpha
 
 
 def _time_ms(fn, iters: int, warmup: int, repeats: int) -> float:
@@ -108,6 +113,29 @@ def main() -> None:
             row[f"aux_{arm}_fwd_us"] = round(1e3 * _time_ms(fwd, args.iters, args.warmup, args.repeats), 2)
             row[f"aux_{arm}_fwd_bwd_us"] = round(1e3 * _time_ms(fwd_bwd, args.iters, args.warmup, args.repeats), 2)
         results["aux_shapes"].append(row)
+        print(json.dumps(row), flush=True)
+    results["seq_shapes"] = []
+    for name, T, E, k, S, opts in SEQ_SHAPES:
+        torch.manual_seed(0)
+        x = torch.randn(T, E, device="cuda").bfloat16().requires_grad_()
+        bias = torch.randn(E, device="cuda") * 0.01
+        dprobs = torch.randn(T, k, device="cuda")
+        sums = torch.zeros(2, device="cuda")
+        row = {"name": name, "T": T, "E": E, "k": k, "S": S, **opts}
+        for arm, seq in (("off", {}), ("on", {**SEQ_ON, "sequence_length": S, "sequence_balance_sums": sums})):
+
+            def fwd(seq=seq):
+                with torch.no_grad():
+                    route_topk(x, k, True, bias, **opts, **seq)
+
+            def fwd_bwd(seq=seq):
+                _, probs = route_topk(x, k, True, bias, **opts, **seq)
+                x.grad = None
+                probs.backward(dprobs)
+
+            row[f"seq_{arm}_fwd_us"] = round(1e3 * _time_ms(fwd, args.iters, args.warmup, args.repeats), 2)
+            row[f"seq_{arm}_fwd_bwd_us"] = round(1e3 * _time_ms(fwd_bwd, args.iters, args.warmup, args.repeats), 2)
+        results["seq_shapes"].append(row)
         print(json.dumps(row), flush=True)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

@@ -11,6 +11,16 @@ renormalised, not scaled - and ``c_e`` the number of the ``T k`` selections that
 With ``w`` the loss weight per token, the call's auxiliary objective ``w T (coef_lb A + coef_z Z)`` is back-propagated by
 adding its gradient to the logits' gradient in backward, and ``(w T A, w T Z, w T)`` is added to an optional fp32 ``[3]``
 accumulator there - once per call, even when activation recomputation runs the forward twice.
+
+Sequence-wise balance loss (DeepSeek-V3 eqs. 17-20, DeepSeek-V2's ``seq_aux``; softmax or sigmoid scores): the ``T`` tokens
+are ``B = T / S`` sequences of ``S`` consecutive tokens, ``s[t]`` is the unbiased, unrenormalised, unscaled balance score
+(softmax: ``softmax(x_t)``; sigmoid: ``sigmoid(x_t) / sum_j sigmoid(x_t)_j``) and ``c[b, e]`` the number of the ``S k``
+actual selections (after bias and group limits) of sequence ``b`` that went to expert ``e``:
+
+* ``A_b = E / (k S^2) sum_e c[b, e] sum_{t in b} s[t, e]``; 1 when balanced, up to ``E / k``.
+
+The call's objective ``w S coef_seq sum_b A_b`` (``= w T coef_seq mean_b A_b``) is back-propagated the same way, and
+``(w S sum_b A_b, w T)`` is added to an optional fp32 ``[2]`` accumulator in backward.
 """
 
 from __future__ import annotations
@@ -69,6 +79,59 @@ class _AuxLossGrad(Function):
         # autograd adds this term to the selection gradient in the logits' dtype: exact for the fp32 logits the oracle
         # is used with; for bf16 logits each term is rounded once before the sum (the kernel rounds their fp32 sum)
         return dprobs, dlogits.to(logits.dtype).reshape(logits.shape), None, None, None, None, None, None
+
+
+def _seq_balance_terms(counts: torch.Tensor, score_sum: torch.Tensor, seq_len: int, top_k: int, coef: float,
+                       token_weight: float) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per-sequence statistics (``counts [B, E]``, ``score_sum [B, E] = sum_{t in b} s[t]``) -> ``g [B, E]`` fp32
+    (``dlogits[t] += ds_t/dx_t^T (g_b - s_t . g_b)``, ``g_b = w coef E c_b / (k S)``) and ``(w S sum_b A_b, w T)``
+    fp32 ``[2]``; device-side, no host synchronisation."""
+    num_seqs, num_experts = counts.shape
+    c = counts.float()
+    per_count = token_weight * num_experts / (top_k * seq_len)
+    logged = torch.cat([(c * score_sum.float()).sum().reshape(1) * per_count,
+                        counts.new_full((1,), token_weight * num_seqs * seq_len, dtype=torch.float32)])
+    return c * (per_count * coef), logged
+
+
+def _balance_scores(x: torch.Tensor, score_function: str) -> tuple[torch.Tensor, torch.Tensor]:
+    """fp32 ``x [T, E]`` -> the balance scores ``s`` and their Jacobian's diagonal factor: ``ds/dx^T v = d (v - s . v)``
+    with ``d = s`` (softmax) or ``sigmoid (1 - sigmoid) / sum_j sigmoid_j`` (normalised sigmoid)."""
+    if score_function == "softmax":
+        s = F.softmax(x, dim=-1)
+        return s, s
+    sig = torch.sigmoid(x)
+    total = sig.sum(-1, keepdim=True)
+    return sig / total, sig * (1 - sig) / total
+
+
+class _SeqBalanceGrad(Function):
+    """CPU path (and numerics oracle) of the sequence-wise balance loss: identity on the selected probabilities; backward
+    adds ``w S coef_seq grad sum_b A_b`` to the logits' gradient, in fp32 from the plain PyTorch definition."""
+
+    @staticmethod
+    def forward(ctx: Any, chosen_p: torch.Tensor, logits: torch.Tensor, chosen: torch.Tensor, top_k: int, score_function: str,
+                seq_len: int, coef: float, token_weight: float, sums: torch.Tensor | None):
+        ctx.save_for_backward(logits.detach(), chosen)
+        ctx.args = (top_k, score_function, seq_len, coef, token_weight, sums)
+        return chosen_p.view_as(chosen_p)
+
+    @staticmethod
+    def backward(ctx: Any, dprobs: torch.Tensor):  # type: ignore[override]
+        logits, chosen = ctx.saved_tensors
+        top_k, score_function, seq_len, coef, token_weight, sums = ctx.args
+        x = logits.reshape(-1, logits.shape[-1]).float()
+        num_seqs, num_experts = x.shape[0] // seq_len, x.shape[1]
+        s, d = _balance_scores(x, score_function)
+        sel = chosen.reshape(num_seqs, seq_len * top_k)
+        counts = torch.zeros(num_seqs, num_experts, dtype=torch.int64, device=x.device).scatter_add_(1, sel, torch.ones_like(sel))
+        g, logged = _seq_balance_terms(counts, s.reshape(num_seqs, seq_len, num_experts).sum(1), seq_len, top_k, coef,
+                                       token_weight)
+        g = g.repeat_interleave(seq_len, dim=0)
+        dlogits = d * (g - (s * g).sum(-1, keepdim=True))
+        if sums is not None:
+            sums.add_(logged)
+        return dprobs, dlogits.to(logits.dtype).reshape(logits.shape), None, None, None, None, None, None, None
 
 
 def route_topk_reference(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None):
@@ -131,6 +194,44 @@ class _RouteTopKAux(Function):
         return dlogits, None, None, None, None, None, None, None, None, None, None
 
 
+class _RouteTopKSeq(Function):
+    """Routing on the fused kernel with per-sequence statistics from the same pass (deterministic, so a recomputed forward
+    reproduces them bit for bit) and the sequence-wise balance gradient - plus, for softmax, the batch load-balancing and
+    z-loss gradients, whose statistics are the per-sequence ones summed - folded into the fused backward."""
+
+    @staticmethod
+    def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None,
+                score_function: str, num_groups: int, topk_groups: int, scaling_factor: float, seq_len: int, seq_coef: float,
+                lb_coef: float, z_coef: float, token_weight: float, seq_sums: torch.Tensor | None,
+                aux_sums: torch.Tensor | None):
+        idx, probs, counts, score_sum, lse2_sum = native_ops().router_topk_seq_fwd(
+            logits, expert_bias, top_k, renormalize, score_function, num_groups, topk_groups, scaling_factor, seq_len)
+        ctx.save_for_backward(logits, idx, counts, score_sum, lse2_sum)
+        ctx.args = (renormalize, score_function, scaling_factor, top_k, seq_len, seq_coef, lb_coef, z_coef, token_weight,
+                    seq_sums, aux_sums)
+        ctx.mark_non_differentiable(idx)
+        return idx, probs
+
+    @staticmethod
+    def backward(ctx: Any, _didx: torch.Tensor, dprobs: torch.Tensor):  # type: ignore[override]
+        logits, idx, counts, score_sum, lse2_sum = ctx.saved_tensors
+        (renormalize, score_function, scaling_factor, top_k, seq_len, seq_coef, lb_coef, z_coef, token_weight, seq_sums,
+         aux_sums) = ctx.args
+        g, logged = _seq_balance_terms(counts, score_sum, seq_len, top_k, seq_coef, token_weight)
+        zc = 0.0
+        if lb_coef > 0 or z_coef > 0:
+            g_batch, zc, aux_logged = _aux_terms(counts.sum(0), score_sum.sum(0), lse2_sum.sum().reshape(1), logits.shape[0],
+                                                 top_k, lb_coef, z_coef, token_weight)
+            g = g + g_batch
+            if aux_sums is not None:
+                aux_sums.add_(aux_logged)
+        dlogits = native_ops().router_topk_seq_bwd(logits, idx, dprobs.float().contiguous(), renormalize, score_function,
+                                                   scaling_factor, g.contiguous(), zc, seq_len)
+        if seq_sums is not None:
+            seq_sums.add_(logged)
+        return dlogits, *([None] * 14)
+
+
 def route_topk_general(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None,
                        score_function: str = "softmax", num_groups: int = 1, topk_groups: int = 1, scaling_factor: float = 1.0):
     """DeepSeek-style routing in plain PyTorch (differentiable through the selected scores).
@@ -168,7 +269,8 @@ def route_topk_general(logits: torch.Tensor, top_k: int, renormalize: bool, expe
 def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None,
                score_function: str = "softmax", num_groups: int = 1, topk_groups: int = 1, scaling_factor: float = 1.0, *,
                load_balancing_coef: float = 0.0, z_loss_coef: float = 0.0, token_loss_weight: float | None = None,
-               aux_loss_sums: torch.Tensor | None = None):
+               aux_loss_sums: torch.Tensor | None = None, sequence_balance_coef: float = 0.0,
+               sequence_length: int | None = None, sequence_balance_sums: torch.Tensor | None = None):
     """``logits [..., E]`` -> ``(indices [..., k] int64, probabilities [..., k] fp32)``.
 
     bf16 CUDA logits with ``E <= 1024``, ``k <= min(32, E)`` and at most 32 expert groups run on the fused CUDA kernel,
@@ -180,6 +282,12 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
     ``z_loss_coef > 0`` the backward also adds the gradient of ``token_loss_weight * T * (load_balancing_coef * A +
     z_loss_coef * Z)`` to the logits, and adds ``(w T A, w T Z, w T)`` to ``aux_loss_sums`` (fp32 ``[3]``, optional).
     With both coefficients 0 the call is exactly the one without them.
+
+    Sequence-wise balance loss (softmax or sigmoid scores; see the module docstring): with ``sequence_balance_coef > 0``
+    the tokens are ``T / sequence_length`` sequences of ``sequence_length`` consecutive tokens (it must divide ``T``), the
+    backward also adds the gradient of ``token_loss_weight * sequence_length * sequence_balance_coef * sum_b A_b`` and adds
+    ``(w S sum_b A_b, w T)`` to ``sequence_balance_sums`` (fp32 ``[2]``, optional).  With the coefficient 0 the call is
+    exactly the one without it.
     """
     num_experts = logits.shape[-1]
     if num_groups > 1 and (num_experts % num_groups != 0 or not 0 < topk_groups <= num_groups):
@@ -197,6 +305,20 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
         if aux_loss_sums is not None and (aux_loss_sums.dtype != torch.float32 or aux_loss_sums.shape != (3,)
                                           or aux_loss_sums.device != logits.device):
             raise ValueError("aux_loss_sums must be an fp32 [3] tensor on the logits' device")
+    if sequence_balance_coef < 0:
+        raise ValueError("the sequence balance coefficient must be non-negative")
+    seq = sequence_balance_coef > 0
+    if seq:
+        if token_loss_weight is None:
+            raise ValueError("auxiliary losses need token_loss_weight, the loss weight of one token")
+        num_tokens = logits.shape[:-1].numel()
+        if sequence_length is None or sequence_length < 1 or num_tokens % sequence_length != 0:
+            raise ValueError(f"the sequence-wise balance loss needs sequence_length, a positive divisor of the token count "
+                             f"({num_tokens}), got {sequence_length}")
+        if sequence_balance_sums is not None and (sequence_balance_sums.dtype != torch.float32
+                                                  or sequence_balance_sums.shape != (2,)
+                                                  or sequence_balance_sums.device != logits.device):
+            raise ValueError("sequence_balance_sums must be an fp32 [2] tensor on the logits' device")
     if (on_gpu(logits) and logits.dtype == torch.bfloat16 and num_experts <= 1024 and top_k <= min(32, num_experts)
             and num_groups <= 32):
         flat = logits.reshape(logits.shape[:-1].numel(), num_experts)  # also when there are no tokens
@@ -204,7 +326,12 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
             flat = flat.contiguous()
         groups = (num_groups, topk_groups) if num_groups > 1 else (1, 1)
         bias = None if expert_bias is None else expert_bias.float().contiguous()
-        if aux:
+        if seq:
+            idx, probs = _RouteTopKSeq.apply(flat, top_k, renormalize, bias, score_function, *groups, float(scaling_factor),
+                                             int(sequence_length), float(sequence_balance_coef), float(load_balancing_coef),
+                                             float(z_loss_coef), float(token_loss_weight), sequence_balance_sums,
+                                             aux_loss_sums)
+        elif aux:
             idx, probs = _RouteTopKAux.apply(flat, top_k, renormalize, bias, *groups, float(scaling_factor),
                                              float(load_balancing_coef), float(z_loss_coef), float(token_loss_weight),
                                              aux_loss_sums)
@@ -219,6 +346,9 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
     if aux:
         chosen_p = _AuxLossGrad.apply(chosen_p, logits, chosen, top_k, float(load_balancing_coef), float(z_loss_coef),
                                       float(token_loss_weight), aux_loss_sums)
+    if seq:
+        chosen_p = _SeqBalanceGrad.apply(chosen_p, logits, chosen, top_k, score_function, int(sequence_length),
+                                         float(sequence_balance_coef), float(token_loss_weight), sequence_balance_sums)
     return chosen, chosen_p
 
 

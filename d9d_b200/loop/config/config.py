@@ -100,10 +100,16 @@ class MoEAuxLossConfig(BaseModel):
     weighted like the LM loss (``T * LOSS_WEIGHT_PER_TOKEN``) and summed over the MoE layers.  ``A`` is ``k`` times
     smaller than Hugging Face's ``load_balancing_loss_func``, which also averages over layers: HF's
     ``router_aux_loss_coef`` ``c`` corresponds to ``load_balancing_coef = c * k / num_moe_layers``.  Sigmoid routers are
-    refused (they balance with ``expert_bias_balancing``)."""
+    refused for these two terms (they balance with ``expert_bias_balancing``).
+
+    ``sequence_balance_coef`` adds the sequence-wise balance loss of softmax and sigmoid routers (DeepSeek-V3 eqs. 17-20,
+    ``alpha``; DeepSeek-V2's ``seq_aux``): ``sequence_balance_coef * mean_b A_b`` per MoE layer and forward of ``B``
+    sequences, ``A_b = E / (k S^2) sum_e c[b, e] sum_{t in b} s[t, e]`` over the sequence's ``S`` tokens, weighted like the
+    other terms.  It needs whole sequences on every rank: context and tensor (sequence) parallel meshes are refused."""
 
     load_balancing_coef: NonNegativeFloat = 0.0
     z_loss_coef: NonNegativeFloat = 0.0
+    sequence_balance_coef: NonNegativeFloat = 0.0
 
 
 class TimeoutConfig(BaseModel):

@@ -54,7 +54,13 @@ class MoELayer(nn.Module, ModuleLateInit):
         x = hidden_states.reshape(-1, shape[-1])
         shared = self.shared_expert(x) if self.shared_expert is not None else None
 
-        routing = self.router(x)
+        seq = {}
+        if self.router.sequence_balance_coef > 0:
+            if hidden_states.dim() != 3:
+                raise ValueError("the sequence-wise balance loss needs the MoE input as [batch, sequence, hidden], got "
+                                 f"{tuple(shape)}")
+            seq = {"sequence_length": shape[-2]}
+        routing = self.router(x, **seq)
         self._update_tokens_per_expert(routing.selected_expert_indices)
 
         xp, pp, grouping = self._communicator.dispatch(x, routing.selected_expert_indices, routing.selected_probabilities)

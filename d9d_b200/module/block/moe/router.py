@@ -35,7 +35,9 @@ class TopKRouter(nn.Module, ModuleLateInit):
     Softmax routers can also train with the load-balancing and router z auxiliary losses (``set_aux_loss``, off by
     default; definitions in ``d9d_b200.kernel.router``): their gradients are added in the router's backward, and
     ``aux_loss_sums`` (fp32, not saved) accumulates ``(sum w T A, sum w T Z, sum w T)`` over the backward passes since
-    ``reset_aux_loss_sums``.
+    ``reset_aux_loss_sums``.  Softmax and sigmoid routers can train with the sequence-wise balance loss
+    (``set_sequence_balance_loss``, off by default): ``forward`` then needs the sequence length, and
+    ``sequence_balance_sums`` (fp32, not saved) accumulates ``(sum w S sum_b A_b, sum w T)``.
 
     Parity: reference ``d9d/module/block/moe/router.py:24-107``.
     """
@@ -50,6 +52,7 @@ class TopKRouter(nn.Module, ModuleLateInit):
             if (enable_expert_bias or options.enable_expert_bias) else None
         )
         self.aux_loss_sums = nn.Buffer(torch.empty(3, dtype=torch.float32), persistent=False)
+        self.sequence_balance_sums = nn.Buffer(torch.empty(2, dtype=torch.float32), persistent=False)
         self._num_experts = num_experts
         self._top_k = top_k
         self._renormalize = renormalize_probabilities
@@ -57,6 +60,7 @@ class TopKRouter(nn.Module, ModuleLateInit):
         self._load_balancing_coef = 0.0
         self._z_loss_coef = 0.0
         self._token_loss_weight: float | None = None
+        self._sequence_balance_coef = 0.0
 
     @property
     def score_function(self) -> str:
@@ -74,19 +78,38 @@ class TopKRouter(nn.Module, ModuleLateInit):
         self._z_loss_coef = float(z_loss_coef)
         self._token_loss_weight = float(token_loss_weight)
 
+    @property
+    def sequence_balance_coef(self) -> float:
+        return self._sequence_balance_coef
+
+    def set_sequence_balance_loss(self, coef: float, token_loss_weight: float) -> None:
+        """Train with ``token_loss_weight * S * coef * sum_b A_b`` per forward of sequences of ``S`` tokens (softmax or
+        sigmoid routers; coefficient 0 switches the loss off)."""
+        if coef < 0:
+            raise ValueError("the sequence balance coefficient must be non-negative")
+        self._sequence_balance_coef = float(coef)
+        self._token_loss_weight = float(token_loss_weight)
+
     @torch.no_grad()
     def reset_aux_loss_sums(self) -> None:
-        if self.aux_loss_sums.dtype == torch.float32:
-            self.aux_loss_sums.zero_()
-        else:  # the module was cast whole: the sums stay fp32
-            self.aux_loss_sums = torch.zeros(3, dtype=torch.float32, device=self.aux_loss_sums.device)
+        """Zero ``aux_loss_sums`` and ``sequence_balance_sums``."""
+        for name, size in (("aux_loss_sums", 3), ("sequence_balance_sums", 2)):
+            sums = getattr(self, name)
+            if sums.dtype == torch.float32:
+                sums.zero_()
+            else:  # the module was cast whole: the sums stay fp32
+                setattr(self, name, torch.zeros(size, dtype=torch.float32, device=sums.device))
 
-    def forward(self, hidden_states: torch.Tensor) -> RoutingResult:
+    def forward(self, hidden_states: torch.Tensor, sequence_length: int | None = None) -> RoutingResult:
+        """``hidden_states [T, D]``; ``sequence_length``: tokens per sequence (the sequence-wise balance loss needs it)."""
         o = self._options
         aux = {}
         if self._load_balancing_coef > 0 or self._z_loss_coef > 0:
             aux = {"load_balancing_coef": self._load_balancing_coef, "z_loss_coef": self._z_loss_coef,
                    "token_loss_weight": self._token_loss_weight, "aux_loss_sums": self.aux_loss_sums}
+        if self._sequence_balance_coef > 0:
+            aux |= {"sequence_balance_coef": self._sequence_balance_coef, "sequence_length": sequence_length,
+                    "token_loss_weight": self._token_loss_weight, "sequence_balance_sums": self.sequence_balance_sums}
         chosen, chosen_p = route_topk(self.gate(hidden_states), self._top_k, self._renormalize, self.expert_bias,
                                       score_function=o.score_function, num_groups=o.num_expert_groups,
                                       topk_groups=o.topk_expert_groups, scaling_factor=o.routed_scaling_factor, **aux)

@@ -218,6 +218,21 @@ void router_topk_aux_fwd(const void* logits, const float* bias, long long T, int
 // with g [E] fp32 (load-balancing term) and z_coef = 2 w_tok coef_z (z-loss term)
 void router_topk_aux_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
                          bool renorm, float scale, const float* g, float z_coef, void* dlogits, cudaStream_t stream);
+// Routing with per-sequence statistics for the sequence-wise balance loss (softmax or sigmoid), deterministic: the same
+// idx / probs, plus for each of the T / seq_len sequences of seq_len consecutive tokens counts [T / seq_len, E] int32,
+// score_sum [T / seq_len, E] = sum_{t in seq} s[t] (softmax: s = softmax(x_t); sigmoid: s = sigma(x_t) / sum_j sigma(x_t)_j)
+// and lse2_sum [T / seq_len] = sum_{t in seq} lse_t^2 (softmax; zeros for sigmoid), via part_counts [P, E],
+// part_scores [P, E], part_lse2 [P] with P = T / seq_len * router_seq_parts(T, seq_len).  seq_len must divide T.
+int router_seq_parts(long long T, long long seq_len);
+void router_topk_seq_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
+                         int num_groups, int topk_groups, float scale, long long seq_len, long long* idx, float* probs,
+                         int* part_counts, float* part_scores, float* part_lse2, int* counts, float* score_sum,
+                         float* lse2_sum, cudaStream_t stream);
+// router_topk_bwd plus the balance gradient of g [T / seq_len, E] fp32, row t / seq_len for token t: softmax
+// dlogits[t, e] += s_e (g_e - s.g) + z_coef lse_t s_e; sigmoid dlogits[t, e] += sigma_e (1 - sigma_e) (g_e - s.g) / sum_j sigma_j
+void router_topk_seq_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
+                         bool renorm, bool sigmoid, float scale, const float* g, float z_coef, long long seq_len,
+                         void* dlogits, cudaStream_t stream);
 
 // ------------------------------------------------------------------ expert-parallel exchange over NVLink ----
 // peer_base: device array [world] of symmetric-arena base pointers; off_* are byte offsets of regions inside the arena.
