@@ -29,7 +29,8 @@ from d9d_b200.ops import build as ops_build  # noqa: E402
 
 UNITS = ["gemm_dense.cu", "gemm_dense_pair.cu", "gemm_grouped.cu", "gemm_ce.cu", "gemm_comm_fwd.cu", "gemm_comm_wgrad.cu"]
 MODES = {0: "DENSE", 1: "GROUPED_M", 2: "GROUPED_K"}
-EPIS = {0: "BF16", 1: "F32", 2: "F32_ACC", 3: "BF16_ACC", 4: "CE_LSE", 5: "CE_DLOGITS"}
+EPIS = {0: "BF16", 1: "F32", 2: "F32_ACC", 3: "BF16_ACC", 4: "CE_LSE", 5: "CE_DLOGITS", 6: "CE_LSE_SUM",
+        7: "CE_DLOGITS_REG"}
 COMMS = {0: "-", 1: "AG_A", 2: "RS_D", 3: "AG_KA", 4: "AG_KB", 5: "WAIT_A"}
 _GEMM = re.compile(r"gemm_kernelILi(\d+)ELi(\d+)ELb([01])ELb([01])ELi(\d+)ELi(\d+)ELi(\d+)EE")
 _ATTN_FWD = re.compile(r"flash_attn_fwd_kernelILi(\d+)ELi(\d+)EE")
@@ -42,7 +43,7 @@ def _name(mangled: str) -> str | None:
         return None
     mode, bn, a_mn, b_mn, epi, comm, ctas = (int(x) for x in m.groups())
     layout = ("MN" if a_mn else "K") + "/" + ("MN" if b_mn else "K")
-    return f"{MODES[mode]:<9} BN {bn:<3} A/B {layout:<5} {EPIS[epi]:<10} comm {COMMS[comm]:<6} ctas {ctas}"
+    return f"{MODES[mode]:<9} BN {bn:<3} A/B {layout:<5} {EPIS[epi]:<14} comm {COMMS[comm]:<6} ctas {ctas}"
 
 
 def _attn_name(mangled: str) -> str | None:
@@ -115,7 +116,7 @@ def main() -> int:
             logs = list(pool.map(lambda u: compile_unit(u, Path(tmp)), units))
     bad = 0
     n = 0
-    print(f"{'unit':<20} {'instance':<58} {'regs':>4} {'stack':>6} {'spill st':>9} {'spill ld':>9}  advisories")
+    print(f"{'unit':<20} {'instance':<62} {'regs':>4} {'stack':>6} {'spill st':>9} {'spill ld':>9}  advisories")
     for unit, log in zip(units, logs):
         for r in sorted(parse(log), key=lambda r: namer(r["fn"]) or r["fn"]):
             name = namer(r["fn"])
@@ -125,7 +126,7 @@ def main() -> int:
             adv = ",".join(sorted(r["adv"])) or "-"
             flag = _flagged(r, name, args.units)
             bad += bool(flag)
-            print(f"{unit:<20} {name or r['fn']:<58} {r['regs']:>4} {r['stack']:>6} {r['st']:>9} {r['ld']:>9}  {adv}"
+            print(f"{unit:<20} {name or r['fn']:<62} {r['regs']:>4} {r['stack']:>6} {r['st']:>9} {r['ld']:>9}  {adv}"
                   + ("   <-- spills / serialised" if flag else ""))
     print(f"{n} instances, {bad} with spills or serialised wgmma")
     return 1 if bad else 0

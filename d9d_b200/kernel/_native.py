@@ -9,6 +9,7 @@ _KERNELS_PER_OP = {
     "moe_permute": 2,
     "ce_forward": 3,  # zero-fill of the target-logit buffer + GEMM + finalize
     "ce_forward_ex": 3,
+    "ce_forward_reg": 3,
     "flash_attn_bwd": 3,  # delta pre-pass + dK/dV kernel + dQ kernel
 }
 

@@ -14,6 +14,9 @@ Replaces the reference's dependency on the cut-cross-entropy Triton kernels (``d
   5 GB bf16 ``dlogits`` a 16k x 151k problem would need) without paying a read-modify-write pass over ``dC`` per chunk.
 * the classifier may be given as several row blocks (``SplitLanguageModellingHead`` keeps one weight per vocabulary
   split): every block is consumed in place - no ``torch.cat`` of the weights, no split of the gradient.
+* label smoothing ``eps`` and the z-loss ``zeta`` regularise the per-token loss (see ``linear_cross_entropy``).  They run
+  on their own epilogue instances (the forward also sums each row's logits when ``eps > 0``; the backward writes the
+  regularised gradient); with both at 0 the plain kernels run.
 """
 
 from __future__ import annotations
@@ -40,15 +43,23 @@ _V_TILE = 128  # rows of dC produced by one GEMM m-tile
 _CAT_SPLITS = os.environ.get("D9D_CCE_CAT_SPLITS", "0") == "1"
 
 
-def linear_cross_entropy_reference(e, c, targets, bias=None, ignore_index=IGNORE_INDEX, softcap=None):
+def linear_cross_entropy_reference(e, c, targets, bias=None, ignore_index=IGNORE_INDEX, softcap=None, label_smoothing=0.0,
+                                   z_loss_coef=0.0):
+    """Materialised-logits oracle: ``(loss[T], lse[T])`` with ``loss = cross_entropy(z, y, label_smoothing) + z_loss_coef
+    * lse^2`` (0 at ignored targets); with both coefficients 0 the loss is the NLL."""
     logits = e.float() @ c.float().t()
     if bias is not None:
         logits = logits + bias.float()
     if softcap is not None:
         logits = torch.tanh(logits / softcap) * softcap
     lse = torch.logsumexp(logits, dim=-1)
-    nll = torch.nn.functional.cross_entropy(logits, targets, ignore_index=ignore_index, reduction="none")
-    return nll, lse
+    if label_smoothing == 0 and z_loss_coef == 0:
+        nll = torch.nn.functional.cross_entropy(logits, targets, ignore_index=ignore_index, reduction="none")
+        return nll, lse
+    loss = torch.nn.functional.cross_entropy(logits, targets, ignore_index=ignore_index, reduction="none",
+                                             label_smoothing=label_smoothing)
+    loss = torch.where(targets == ignore_index, torch.zeros_like(loss), loss + z_loss_coef * lse * lse)
+    return loss, lse
 
 
 class _EmulatedOps:
@@ -77,13 +88,21 @@ class _EmulatedOps:
         nll = torch.where(target == ignore_index, torch.zeros_like(lse), lse - tgt_logit)
         return nll, lse, tgt_logit
 
+    def ce_forward_reg(self, h, w, target, ignore_index, bias=None, softcap=0.0, col_offset=0):
+        nll, lse, tgt_logit = self.ce_forward_ex(h, w, target, ignore_index, bias, softcap, col_offset)
+        return nll, lse, tgt_logit, self._logits(h, w, bias, softcap)[0].sum(-1)
+
     def ce_dlogits(self, h, w, target, lse, grad, out, ignore_index, bias=None, softcap=0.0, col_offset=0):
+        self.ce_dlogits_reg(h, w, target, lse, grad, out, ignore_index, 0.0, 0.0, 1, bias, softcap, col_offset)
+
+    def ce_dlogits_reg(self, h, w, target, lse, grad, out, ignore_index, z_loss_coef, label_smoothing, num_classes,
+                       bias=None, softcap=0.0, col_offset=0):
         z, dz = self._logits(h, w, bias, softcap)
-        p = torch.exp(z - lse[:, None])
+        p = torch.exp(z - lse[:, None]) * (1 + 2 * z_loss_coef * lse[:, None]) - label_smoothing / num_classes
         local = target - col_offset
         inside = (target != ignore_index) & (local >= 0) & (local < w.shape[0])
         rows = torch.nonzero(inside)[:, 0]
-        p[rows, local[rows]] -= 1
+        p[rows, local[rows]] -= 1 - label_smoothing
         g = torch.where(target == ignore_index, torch.zeros_like(grad), grad)
         out.copy_((p * g[:, None] * dz).to(out.dtype))
 
@@ -138,7 +157,9 @@ def _sm_count(device: torch.device) -> int:
 
 
 class _LinearCEFunction(Function):
-    """``(nll[T], lse[T]) = CE(e @ cat(weights)^T + bias)``.
+    """``(loss[T], lse[T], nll[T] | None)``: the per-token loss of ``e @ cat(weights)^T + bias`` (see
+    ``linear_cross_entropy``), its log-sum-exp and, when the loss is regularised, the plain NLL (else ``None``: the loss
+    is the NLL).
 
     Inputs after ``n_splits``: the ``n_splits`` classifier blocks, then per block the leaf parameter that owns a
     pre-allocated gradient buffer (``fused_wgrad_owner``; the block itself is then passed detached) or ``None``.
@@ -146,7 +167,7 @@ class _LinearCEFunction(Function):
 
     @staticmethod
     def forward(ctx: Any, e: torch.Tensor, targets: torch.Tensor, bias: torch.Tensor | None, ignore_index: int, softcap: float,
-                emulate: bool, n_splits: int, *blocks: torch.Tensor | None):
+                emulate: bool, label_smoothing: float, z_loss_coef: float, n_splits: int, *blocks: torch.Tensor | None):
         weights, owners = blocks[:n_splits], blocks[n_splits:]
         ops = _EmulatedOps() if emulate else native_ops()
         bias32 = None if bias is None else bias.detach().float().contiguous()
@@ -154,34 +175,49 @@ class _LinearCEFunction(Function):
         parts = []
         for w in weights:
             b = None if bias32 is None else bias32[v0 : v0 + w.shape[0]]
-            parts.append(ops.ce_forward_ex(e, w, targets, ignore_index, b, softcap, v0))
+            if label_smoothing > 0:  # (nll, lse, tgt_logit, zsum): the smoothing term needs the row's logit sum
+                parts.append(ops.ce_forward_reg(e, w, targets, ignore_index, b, softcap, v0))
+            else:
+                parts.append(ops.ce_forward_ex(e, w, targets, ignore_index, b, softcap, v0))
             v0 += w.shape[0]
         if n_splits == 1:
-            nll, lse, _ = parts[0]
+            nll, lse = parts[0][:2]
         else:
             lse = torch.logsumexp(torch.stack([p[1] for p in parts]), dim=0)
             tgt_logit = torch.stack([p[2] for p in parts]).sum(0)
             nll = torch.where(targets == ignore_index, torch.zeros_like(lse), lse - tgt_logit)
+        regularised = label_smoothing > 0 or z_loss_coef > 0
+        loss = nll
+        if regularised:
+            reg = z_loss_coef * lse * lse
+            if label_smoothing > 0:
+                zsum = parts[0][3] if n_splits == 1 else torch.stack([p[3] for p in parts]).sum(0)
+                reg = reg + label_smoothing * (lse - zsum / v0)
+            loss = torch.where(targets == ignore_index, torch.zeros_like(lse), (1 - label_smoothing) * nll + reg)
         ctx.save_for_backward(e, targets, lse, bias32, *weights)
         ctx.owners = owners
         ctx.ignore_index, ctx.softcap, ctx.emulate, ctx.n_splits = ignore_index, softcap, emulate, n_splits
+        ctx.label_smoothing, ctx.z_loss_coef, ctx.regularised = label_smoothing, z_loss_coef, regularised
         ctx.bias_dtype = None if bias is None else bias.dtype
         ctx.mark_non_differentiable(lse)
-        return nll, lse
+        if not regularised:
+            return nll, lse, None
+        ctx.mark_non_differentiable(nll)
+        return loss, lse, nll
 
     @staticmethod
-    def backward(ctx: Any, grad_nll: torch.Tensor, _grad_lse: torch.Tensor):  # type: ignore[override]
+    def backward(ctx: Any, grad_loss: torch.Tensor, _grad_lse: torch.Tensor, _grad_nll: torch.Tensor | None):  # type: ignore[override]
         e, targets, lse, bias32, *weights = ctx.saved_tensors
         n = ctx.n_splits
         ops = _EmulatedOps() if ctx.emulate else native_ops()
         T, K = e.shape
-        w_base = 7  # position of the first classifier block among the forward inputs
+        w_base = 9  # position of the first classifier block among the forward inputs
         dir_w = GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.weight)
         need_e = ctx.needs_input_grad[0] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.inputs)
         need_b = bias32 is not None and ctx.needs_input_grad[2] and dir_w
         fused = [ctx.owners[i] is not None and ctx.needs_input_grad[w_base + n + i] and dir_w for i in range(n)]
         plain = [ctx.owners[i] is None and ctx.needs_input_grad[w_base + i] and dir_w for i in range(n)]
-        g = grad_nll.float().contiguous()
+        g = grad_loss.float().contiguous()
 
         chunks, width, multi = plan_vocab_chunks([w.shape[0] for w in weights], T, K, _CHUNK_BYTES, _sm_count(e.device))
         buf = torch.empty(T, width, device=e.device, dtype=torch.bfloat16)
@@ -204,7 +240,11 @@ class _LinearCEFunction(Function):
             dl = buf[:, : r1 - r0]
             col0 = starts[i] + r0
             b = None if bias32 is None else bias32[col0 : col0 + (r1 - r0)]
-            ops.ce_dlogits(e, w, targets, lse, g, dl, ctx.ignore_index, b, ctx.softcap, col0)
+            if ctx.regularised:
+                ops.ce_dlogits_reg(e, w, targets, lse, g, dl, ctx.ignore_index, ctx.z_loss_coef, ctx.label_smoothing,
+                                   starts[-1], b, ctx.softcap, col0)
+            else:
+                ops.ce_dlogits(e, w, targets, lse, g, dl, ctx.ignore_index, b, ctx.softcap, col0)
             if need_e:
                 ops.gemm(dl, w, de_acc, False, True, not first)  # dE (+)= dL[T, v] @ C[v, K]
             if fused[i]:
@@ -218,7 +258,27 @@ class _LinearCEFunction(Function):
         if need_e:
             de = de_acc if de_acc.dtype == e.dtype else de_acc.to(e.dtype)
         db = None if dbias is None else dbias.to(ctx.bias_dtype)
-        return (de, None, db, None, None, None, None, *dcs, *([None] * n))
+        return (de, None, db, None, None, None, None, None, None, *dcs, *([None] * n))
+
+
+class _LossSums(Function):
+    """Identity on the per-token loss whose backward adds ``(sum nll, sum lse^2, count)`` over the non-ignored tokens to
+    ``sums``: a forward recomputed for its backward (activation checkpointing) counts once."""
+
+    @staticmethod
+    def forward(ctx: Any, loss: torch.Tensor, nll: torch.Tensor, lse: torch.Tensor, valid: torch.Tensor, sums: torch.Tensor):
+        ctx.save_for_backward(nll, lse, valid)
+        ctx.sums = sums
+        return loss.view_as(loss)
+
+    @staticmethod
+    def backward(ctx: Any, grad: torch.Tensor):  # type: ignore[override]
+        nll, lse, valid = ctx.saved_tensors
+        with torch.no_grad():
+            zero = torch.zeros((), dtype=torch.float32, device=nll.device)
+            ctx.sums.add_(torch.stack([torch.where(valid, nll.float(), zero).sum(),
+                                       torch.where(valid, lse.float().square(), zero).sum(), valid.sum().float()]))
+        return grad, None, None, None, None
 
 
 def _native_eligible(e2: torch.Tensor, weights: Sequence[torch.Tensor]) -> bool:
@@ -236,15 +296,34 @@ def linear_cross_entropy(
     shift: bool | int = 0,
     return_lse: bool = False,
     _emulate: bool = False,
+    label_smoothing: float = 0.0,
+    z_loss_coef: float = 0.0,
+    *,
+    loss_sums: torch.Tensor | None = None,
     **_unused: Any,
 ) -> torch.Tensor | tuple[torch.Tensor, torch.Tensor]:
-    """``cross_entropy(e @ c^T (+ bias), targets)`` with ``reduction in {none, mean, sum}``.
+    """``cross_entropy(e @ c^T (+ bias), targets, label_smoothing) + z_loss_coef * lse^2`` with
+    ``reduction in {none, mean, sum}``.
 
     ``e``: ``[..., K]`` embeddings; ``c``: ``[V, K]`` classifier or a sequence of row blocks of it (consumed in place);
     ``targets``: ``[...]`` int64.  ``shift=n`` drops the last ``n`` embeddings / first ``n`` targets along the sequence
     dim (causal LM shift).  ``softcap`` applies ``softcap * tanh(logits / softcap)``.  CCE's gradient-filtering options
     of the reference are accepted and ignored (gradients are exact).
+
+    Per token, with ``z`` the logits after bias and soft-cap over all ``V`` classes, ``lse = logsumexp(z)``, ``eps =
+    label_smoothing`` and ``zeta = z_loss_coef``: ``loss = (1 - eps) (lse - z_y) + eps (lse - mean_j z_j) + zeta lse^2``,
+    0 at ignored targets (``F.cross_entropy(z, y, label_smoothing=eps) + zeta lse^2``).  ``mean`` divides by the number
+    of non-ignored targets.  With both coefficients 0 this is the plain NLL, computed by the same kernels as without them.
+    ``loss_sums`` (fp32 ``[3]``, optional) accumulates ``(sum nll, sum lse^2, count)`` over the non-ignored tokens,
+    with the unsmoothed NLL, in backward (a recomputed forward counts once).
     """
+    if not (0.0 <= label_smoothing <= 1.0):
+        raise ValueError(f"label_smoothing must lie in [0, 1], got {label_smoothing}")
+    if not (0.0 <= z_loss_coef < math.inf):
+        raise ValueError(f"z_loss_coef must be finite and >= 0, got {z_loss_coef}")
+    label_smoothing, z_loss_coef = float(label_smoothing), float(z_loss_coef)
+    if loss_sums is not None and (loss_sums.dtype != torch.float32 or loss_sums.shape != (3,) or loss_sums.device != e.device):
+        raise ValueError("loss_sums must be an fp32 [3] tensor on the embeddings' device")
     if isinstance(shift, bool):
         shift = int(shift)
     if shift:
@@ -269,11 +348,19 @@ def linear_cross_entropy(
             wl = w if w.dtype == e2.dtype else w.to(e2.dtype)
             ws.append((wl.detach() if owner is not None else wl).contiguous())
             owners.append(owner)
-        nll, lse = _LinearCEFunction.apply(e2.contiguous(), t1.contiguous(), bias, ignore_index, float(softcap or 0.0),
-                                           _emulate, len(ws), *ws, *owners)
+        nll, lse, plain_nll = _LinearCEFunction.apply(e2.contiguous(), t1.contiguous(), bias, ignore_index,
+                                                      float(softcap or 0.0), _emulate, label_smoothing, z_loss_coef, len(ws),
+                                                      *ws, *owners)
     else:
         full = blocks[0] if len(blocks) == 1 else torch.cat(blocks, dim=0)
-        nll, lse = linear_cross_entropy_reference(e2, full, t1, bias, ignore_index, softcap)
+        nll, lse = linear_cross_entropy_reference(e2, full, t1, bias, ignore_index, softcap, label_smoothing, z_loss_coef)
+        plain_nll = None
+        if loss_sums is not None and (label_smoothing > 0 or z_loss_coef > 0):
+            with torch.no_grad():
+                plain_nll = linear_cross_entropy_reference(e2, full, t1, bias, ignore_index, softcap)[0]
+    if loss_sums is not None:
+        plain_nll = nll if plain_nll is None else plain_nll
+        nll = _LossSums.apply(nll, plain_nll.detach(), lse.detach(), t1 != ignore_index, loss_sums)
     if reduction == "none":
         loss = nll.view(lead_shape)
     elif reduction == "sum":
@@ -291,11 +378,13 @@ class LinearCrossEntropy(nn.Module):
     """Module wrapper with stored options (reference ``d9d/kernel/cce/main.py:228-282``)."""
 
     def __init__(self, ignore_index: int = IGNORE_INDEX, softcap: float | None = None, reduction: str = "mean",
-                 shift: bool | int = 0, **kwargs: Any):
+                 shift: bool | int = 0, label_smoothing: float = 0.0, z_loss_coef: float = 0.0, **kwargs: Any):
         super().__init__()
         self.ignore_index, self.softcap, self.reduction, self.shift = ignore_index, softcap, reduction, shift
+        self.label_smoothing, self.z_loss_coef = label_smoothing, z_loss_coef
         self.kwargs = kwargs
 
     def forward(self, e: torch.Tensor, c: torch.Tensor, targets: torch.Tensor, bias: torch.Tensor | None = None):
         return linear_cross_entropy(e, c, targets, bias=bias, ignore_index=self.ignore_index, softcap=self.softcap,
-                                    reduction=self.reduction, shift=self.shift)
+                                    reduction=self.reduction, shift=self.shift, label_smoothing=self.label_smoothing,
+                                    z_loss_coef=self.z_loss_coef)

@@ -5,6 +5,7 @@ from .checkpointer import StateCheckpointer
 from .data_loader_factory import DataLoaderFactory, IteratorBatchGroup, StatefulDataLoaderDataParallelAware
 from .expert_bias_balancer import ExpertBiasBalancer
 from .moe_aux_loss import MoEAuxLoss
+from .lm_loss import LMLoss
 from .garbage_collector import ManualGarbageCollector
 from .gradient_clipper import GradientClipper
 from .gradient_manager import GradientManager
@@ -26,6 +27,7 @@ __all__ = [
     "ExpertBiasBalancer",
     "ForwardResult",
     "MoEAuxLoss",
+    "LMLoss",
     "GradientClipper",
     "GradientManager",
     "InferenceProcessor",

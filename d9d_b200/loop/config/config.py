@@ -1,7 +1,7 @@
 from pathlib import Path
 from typing import Literal
 
-from pydantic import BaseModel, NonNegativeFloat
+from pydantic import BaseModel, Field, NonNegativeFloat
 
 from d9d_b200.pipelining.factory import AnyPipelineScheduleConfig
 from d9d_b200.tracker import AnyTrackerConfig, RunConfig
@@ -112,6 +112,14 @@ class MoEAuxLossConfig(BaseModel):
     sequence_balance_coef: NonNegativeFloat = 0.0
 
 
+class LMLossConfig(BaseModel):
+    """Regularise the LM loss per target token: ``cross_entropy(z, y, label_smoothing) + z_loss_coef * lse(z)^2`` in the
+    fused linear cross-entropy (PaLM's z-loss: ``z_loss_coef`` around 1e-4)."""
+
+    label_smoothing: float = Field(default=0.0, ge=0.0, le=1.0)
+    z_loss_coef: NonNegativeFloat = 0.0
+
+
 class TimeoutConfig(BaseModel):
     init_timeout: int = 10000
     step_timeout: int = 100
@@ -133,6 +141,7 @@ class TrainerConfig(BaseModel):
     timeout: TimeoutConfig = TimeoutConfig()
     expert_bias_balancing: ExpertBiasBalancingConfig | None = None  # None: expert biases stay as loaded
     moe_aux_loss: MoEAuxLossConfig | None = None  # None: routers train without auxiliary losses
+    lm_loss: LMLossConfig | None = None  # None: the LM head trains on the plain NLL and logs nothing more
 
 
 class InferenceConfig(BaseModel):

@@ -82,6 +82,8 @@ class TrainingConfigurator:
             if cfg.expert_bias_balancing is not None else None,
             moe_aux_loss=parts.MoEAuxLoss(dist_context=ctx, tracked_modules=modules, config=cfg.moe_aux_loss)
             if cfg.moe_aux_loss is not None else None,
+            lm_loss=parts.LMLoss(dist_context=ctx, tracked_modules=modules, config=cfg.lm_loss)
+            if cfg.lm_loss is not None else None,
         )
 
     def configure(self) -> "Trainer":
@@ -93,8 +95,8 @@ class Trainer:
 
     One iteration == one optimizer step: forward/backward over the accumulation group (gradient buckets all-reduce
     on the side stream as they fill), metric sync kicked off asynchronously, gradient wait + ``1/sum(w)`` scaling,
-    clipping, optimizer, expert-bias balancing (when configured), LR scheduler, logging (+ the MoE auxiliary losses when
-    configured), ``zero_grad``, housekeeping, post-step checkpoint.
+    clipping, optimizer, expert-bias balancing (when configured), LR scheduler, logging (+ the MoE auxiliary losses and
+    the LM loss terms when configured), ``zero_grad``, housekeeping, post-step checkpoint.
     """
 
     def __init__(self, state: TrainJobState):
@@ -133,6 +135,8 @@ class Trainer:
                     s.expert_bias_balancer.reset_counters()
                 if s.moe_aux_loss is not None:
                     s.moe_aux_loss.reset()
+                if s.lm_loss is not None:
+                    s.lm_loss.reset()
                 with s.event_bus.bounded(events.EVENT_TRAIN_FORWARD_BACKWARD_PRE, events.EVENT_TRAIN_FORWARD_BACKWARD_POST, step_ctx):
                     for batch in batch_group:
                         result = s.task_operator.forward_backward(batch)
@@ -149,6 +153,8 @@ class Trainer:
                 s.logger.log(run, loss_value=s.gradient_manager.compute_global_loss())
                 if s.moe_aux_loss is not None and s.logger.is_due():
                     s.moe_aux_loss.log(run)
+                if s.lm_loss is not None and s.logger.is_due():
+                    s.lm_loss.log(run)
                 s.gradient_manager.zero_grad()
                 gc.collect_periodic()
                 if profiler:

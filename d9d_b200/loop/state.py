@@ -19,6 +19,7 @@ from d9d_b200.loop.component import (
     BatchMaths,
     ExpertBiasBalancer,
     MoEAuxLoss,
+    LMLoss,
     GradientClipper,
     GradientManager,
     InferenceTaskOperator,
@@ -85,6 +86,7 @@ class TrainJobState(JobState):
     exporter: ModelStageExporter
     expert_bias_balancer: ExpertBiasBalancer | None = None
     moe_aux_loss: MoEAuxLoss | None = None  # not checkpointed: its sums restart every step
+    lm_loss: LMLoss | None = None  # not checkpointed: its sums restart every step
 
 
 @dataclasses.dataclass(kw_only=True)

@@ -182,7 +182,8 @@ class _HeadedDecoder(nn.Module, ModuleLateInit, ModuleSupportsPipelining):
 
 
 class DecoderForCausalLM(_HeadedDecoder):
-    """Adds ``lm_head``; the last stage outputs ``logps [B,S]`` = fp32 per-token NLL (0 at ignored labels)."""
+    """Adds ``lm_head``; the last stage outputs ``logps [B,S]`` = fp32 per-token training objective (0 at ignored labels):
+    the NLL, unless ``lm_head.set_loss_regularisation`` added label smoothing or a z-loss."""
 
     def __init__(self, backbone: DecoderBackbone, params: _BackboneParams, stage: PipelineStageInfo):
         super().__init__(stage, params.layer.hidden_size)

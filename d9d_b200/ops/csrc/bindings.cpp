@@ -5,6 +5,7 @@
 #include <torch/library.h>
 #include <torch/torch.h>
 
+#include <cmath>
 #include <tuple>
 #include <vector>
 
@@ -157,6 +158,62 @@ std::tuple<Tensor, Tensor, Tensor> ce_forward_ex(const Tensor& h, const Tensor& 
   return {nll, lse, tgt_logit};
 }
 
+// Operand checks of the regularised linear-CE ops, before anything touches the device
+void check_ce_reg_operands(const char* op, const Tensor& h, const Tensor& w, const Tensor& target,
+                           const c10::optional<Tensor>& bias, double softcap, int64_t col_offset) {
+  CHECK_CUDA_CONTIG(h); CHECK_CUDA_CONTIG(w); CHECK_CUDA_CONTIG(target);
+  TORCH_CHECK(h.dim() == 2 && w.dim() == 2 && target.dim() == 1, op, ": h [T, K], w [V, K] and target [T] expected");
+  TORCH_CHECK(h.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16, op, ": h and w must be bf16");
+  TORCH_CHECK(target.scalar_type() == at::kLong, op, ": target must be int64");
+  TORCH_CHECK(w.device() == h.device() && target.device() == h.device(), op, ": operands must be on one device");
+  TORCH_CHECK(w.size(1) == h.size(1) && target.numel() == h.size(0), op, ": shape mismatch");
+  TORCH_CHECK(h.size(1) % 8 == 0 && h.size(1) > 0, op, ": the hidden size must be a positive multiple of 8");
+  TORCH_CHECK(h.size(0) < (int64_t(1) << 31) && w.size(0) < (int64_t(1) << 31), op, ": too many rows");
+  CHECK_ALIGNED16(h); CHECK_ALIGNED16(w);
+  TORCH_CHECK(std::isfinite(softcap) && softcap >= 0.0, op, ": softcap must be finite and >= 0");
+  TORCH_CHECK(col_offset >= 0, op, ": col_offset must be >= 0");
+  if (bias.has_value()) {
+    CHECK_CUDA_CONTIG(*bias);
+    TORCH_CHECK(bias->device() == h.device() && bias->scalar_type() == at::kFloat && bias->numel() == w.size(0),
+                op, ": bias must be fp32 [V]");
+  }
+}
+
+// regularised linear-CE forward over a row slice w = C[col_offset : col_offset + V] of the classifier: ce_forward_ex's
+// (nll[T], lse[T], tgt_logit[T]) plus zsum[T], the sum of the row's logits over the slice (after bias and soft-cap)
+std::tuple<Tensor, Tensor, Tensor, Tensor> ce_forward_reg(const Tensor& h, const Tensor& w, const Tensor& target,
+                                                          int64_t ignore_index, const c10::optional<Tensor>& bias,
+                                                          double softcap, int64_t col_offset) {
+  check_ce_reg_operands("ce_forward_reg", h, w, target, bias, softcap, col_offset);
+  c10::cuda::CUDAGuard guard(h.device());
+  const int T = static_cast<int>(h.size(0)), K = static_cast<int>(h.size(1)), V = static_cast<int>(w.size(0));
+  const int bn = d9d::gemm_ce_block_n();
+  const int n_tiles = (V + bn - 1) / bn;
+  auto fopt = h.options().dtype(at::kFloat);
+  Tensor part_max = at::empty({n_tiles, T}, fopt), part_sum = at::empty({n_tiles, T}, fopt);
+  Tensor part_zsum = at::empty({n_tiles, T}, fopt);
+  Tensor tgt_logit = at::zeros({T}, fopt), lse = at::empty({T}, fopt), nll = at::empty({T}, fopt);
+  Tensor zsum = at::empty({T}, fopt);
+  d9d::GemmArgs g;
+  g.mode = 0; g.epi = 6;
+  g.M = T; g.N = V; g.K = K;
+  g.A = h.data_ptr(); g.B = w.data_ptr(); g.lda = K; g.ldb = K; g.ldd = V;
+  g.ce_target = reinterpret_cast<const long long*>(target.data_ptr<int64_t>());
+  g.ce_part_max = part_max.data_ptr<float>(); g.ce_part_sum = part_sum.data_ptr<float>();
+  g.ce_part_zsum = part_zsum.data_ptr<float>();
+  g.ce_tgt_logit = tgt_logit.data_ptr<float>();
+  g.ce_ignore_index = ignore_index;
+  g.ce_softcap = static_cast<float>(softcap);
+  g.ce_col_offset = col_offset;
+  if (bias.has_value()) g.ce_bias = bias->data_ptr<float>();
+  d9d::gemm_ce(g, cur_stream());
+  d9d::ce_finalize_zsum(part_max.data_ptr<float>(), part_sum.data_ptr<float>(), part_zsum.data_ptr<float>(),
+                        tgt_logit.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
+                        ignore_index, n_tiles, T, lse.data_ptr<float>(), nll.data_ptr<float>(), zsum.data_ptr<float>(),
+                        cur_stream());
+  return {nll, lse, tgt_logit, zsum};
+}
+
 // fused linear-CE forward: returns (nll[T] fp32, lse[T] fp32)
 std::tuple<Tensor, Tensor> ce_forward(const Tensor& h, const Tensor& w, const Tensor& target, int64_t ignore_index) {
   auto r = ce_forward_ex(h, w, target, ignore_index, c10::nullopt, 0.0, 0);
@@ -188,6 +245,43 @@ void ce_dlogits(const Tensor& h, const Tensor& w, const Tensor& target, const Te
     TORCH_CHECK(bias->scalar_type() == at::kFloat && bias->numel() == V, "ce: bias must be fp32 [V]");
     g.ce_bias = bias->data_ptr<float>();
   }
+  d9d::gemm_ce(g, cur_stream());
+}
+
+// regularised linear-CE backward, one chunk: out[T, V] (bf16) = grad[t] * d loss[t] / d logits[t, col_offset : col_offset + V]
+// with loss = (1 - eps) (lse - z_y) + eps (lse - sum_j z_j / num_classes) + zeta lse^2, i.e.
+// grad[t] * ((1 + 2 zeta lse) softmax - (1 - eps) onehot - eps / num_classes) * dz/dacc  (lse over the WHOLE vocabulary)
+void ce_dlogits_reg(const Tensor& h, const Tensor& w, const Tensor& target, const Tensor& lse, const Tensor& grad, Tensor out,
+                    int64_t ignore_index, double z_loss_coef, double label_smoothing, int64_t num_classes,
+                    const c10::optional<Tensor>& bias, double softcap, int64_t col_offset) {
+  check_ce_reg_operands("ce_dlogits_reg", h, w, target, bias, softcap, col_offset);
+  CHECK_CUDA_CONTIG(lse); CHECK_CUDA_CONTIG(grad);
+  TORCH_CHECK(lse.scalar_type() == at::kFloat && grad.scalar_type() == at::kFloat, "ce_dlogits_reg: lse and grad must be fp32");
+  TORCH_CHECK(lse.device() == h.device() && grad.device() == h.device() && out.device() == h.device(),
+              "ce_dlogits_reg: operands must be on one device");
+  TORCH_CHECK(lse.numel() == h.size(0) && grad.numel() == h.size(0), "ce_dlogits_reg: lse and grad must be [T]");
+  TORCH_CHECK(out.is_cuda() && out.dim() == 2 && out.stride(1) == 1 && out.scalar_type() == at::kBFloat16,
+              "ce_dlogits_reg: out must be a row-major bf16 matrix (row pitch may be padded)");
+  TORCH_CHECK(out.size(0) == h.size(0) && out.size(1) == w.size(0), "ce_dlogits_reg: out must be [T, V]");
+  TORCH_CHECK(std::isfinite(z_loss_coef) && z_loss_coef >= 0.0, "ce_dlogits_reg: z_loss_coef must be finite and >= 0");
+  TORCH_CHECK(label_smoothing >= 0.0 && label_smoothing <= 1.0, "ce_dlogits_reg: label_smoothing must lie in [0, 1]");
+  TORCH_CHECK(num_classes >= col_offset + w.size(0) && num_classes > 0 && num_classes < (int64_t(1) << 31),
+              "ce_dlogits_reg: num_classes must cover the slice (num_classes >= col_offset + V) and fit in int32");
+  c10::cuda::CUDAGuard guard(h.device());
+  const int T = static_cast<int>(h.size(0)), K = static_cast<int>(h.size(1)), V = static_cast<int>(w.size(0));
+  d9d::GemmArgs g;
+  g.mode = 0; g.epi = 7;
+  g.M = T; g.N = V; g.K = K;
+  g.A = h.data_ptr(); g.B = w.data_ptr(); g.D = out.data_ptr(); g.lda = K; g.ldb = K; g.ldd = out.stride(0);
+  g.ce_target = reinterpret_cast<const long long*>(target.data_ptr<int64_t>());
+  g.ce_lse = lse.data_ptr<float>(); g.ce_grad = grad.data_ptr<float>();
+  g.ce_ignore_index = ignore_index;
+  g.ce_softcap = static_cast<float>(softcap);
+  g.ce_col_offset = col_offset;
+  g.ce_z_loss = static_cast<float>(z_loss_coef);
+  g.ce_smoothing = static_cast<float>(label_smoothing);
+  g.ce_num_classes = static_cast<int>(num_classes);
+  if (bias.has_value()) g.ce_bias = bias->data_ptr<float>();
   d9d::gemm_ce(g, cur_stream());
 }
 
@@ -999,6 +1093,8 @@ TORCH_LIBRARY(d9d_b200, m) {
   m.def("ce_forward(Tensor h, Tensor w, Tensor target, int ignore_index) -> (Tensor, Tensor)");
   m.def("ce_forward_ex(Tensor h, Tensor w, Tensor target, int ignore_index, Tensor? bias=None, float softcap=0.0, int col_offset=0) -> (Tensor, Tensor, Tensor)");
   m.def("ce_dlogits(Tensor h, Tensor w, Tensor target, Tensor lse, Tensor grad, Tensor(a!) out, int ignore_index, Tensor? bias=None, float softcap=0.0, int col_offset=0) -> ()");
+  m.def("ce_forward_reg(Tensor h, Tensor w, Tensor target, int ignore_index, Tensor? bias=None, float softcap=0.0, int col_offset=0) -> (Tensor, Tensor, Tensor, Tensor)");
+  m.def("ce_dlogits_reg(Tensor h, Tensor w, Tensor target, Tensor lse, Tensor grad, Tensor(a!) out, int ignore_index, float z_loss_coef, float label_smoothing, int num_classes, Tensor? bias=None, float softcap=0.0, int col_offset=0) -> ()");
   m.def("quantize_rowwise(Tensor x) -> (Tensor, Tensor)");
   m.def("quantize_colwise_t(Tensor x) -> (Tensor, Tensor)");
   m.def("quantize_mx(Tensor x) -> (Tensor, Tensor)");
@@ -1061,6 +1157,8 @@ TORCH_LIBRARY_IMPL(d9d_b200, CUDA, m) {
   m.impl("ce_forward", &ce_forward);
   m.impl("ce_forward_ex", &ce_forward_ex);
   m.impl("ce_dlogits", &ce_dlogits);
+  m.impl("ce_forward_reg", &ce_forward_reg);
+  m.impl("ce_dlogits_reg", &ce_dlogits_reg);
   m.impl("quantize_rowwise", &quantize_rowwise);
   m.impl("quantize_colwise_t", &quantize_colwise_t);
   m.impl("quantize_mx", &quantize_mx);

@@ -48,6 +48,10 @@ struct GemmArgs {
   float ce_softcap = 0.f;              // logits -> softcap * tanh(logits / softcap); 0 = off
   const float* ce_bias = nullptr;      // [N] fp32 logit bias
   long long ce_col_offset = 0;         // B is a row slice of the classifier starting at this class id
+  float* ce_part_zsum = nullptr;       // [n_tiles, M] per-tile logit sums (regularised forward)
+  float ce_z_loss = 0.f;               // regularised backward: z-loss coefficient zeta
+  float ce_smoothing = 0.f;            // regularised backward: label smoothing eps
+  int ce_num_classes = 0;              // regularised backward: classes over all slices of the classifier
 };
 
 void gemm_dense(const GemmArgs& a, cudaStream_t stream);
@@ -64,6 +68,10 @@ int gemm_ce_block_n();
 // (part_max, part_sum)[n_tiles, M] + tgt_logit[M] -> lse[M], nll[M] (0 where target == ignore_index)
 void ce_finalize(const float* part_max, const float* part_sum, const float* tgt_logit, const long long* target,
                  long long ignore_index, int n_tiles, int M, float* lse, float* nll, cudaStream_t stream);
+// ce_finalize + part_zsum[n_tiles, M] -> zsum[M], summed over the tiles in order
+void ce_finalize_zsum(const float* part_max, const float* part_sum, const float* part_zsum, const float* tgt_logit,
+                      const long long* target, long long ignore_index, int n_tiles, int M, float* lse, float* nll,
+                      float* zsum, cudaStream_t stream);
 
 // ------------------------------------------------------------------ fp8 GEMM (wgmma e4m3, MX block scales) -----
 struct Fp8GemmArgs {

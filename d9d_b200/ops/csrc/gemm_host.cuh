@@ -152,8 +152,8 @@ void launch_one(const GemmArgs& a, cudaStream_t stream) {
   CUtensorMap td = ta;  // placeholder when the direct-store epilogue is used
   if (COMM == COMM_RS_D) {
     p.tma_epilogue = 1;  // output tiles are reduce-added through the peer maps
-  } else if (EPI != EPI_CE_LSE) {
-    constexpr bool out_bf16 = (EPI == EPI_BF16 || EPI == EPI_BF16_ACC || EPI == EPI_CE_DLOGITS);
+  } else if (EPI != EPI_CE_LSE && EPI != EPI_CE_LSE_SUM) {
+    constexpr bool out_bf16 = (EPI == EPI_BF16 || EPI == EPI_BF16_ACC || EPI == EPI_CE_DLOGITS || EPI == EPI_CE_DLOGITS_REG);
     const uint64_t groups = (MODE == GROUPED_K) ? a.num_groups : 1;
     p.tma_epilogue = make_tmap_out(&td, a.D, out_bf16, a.N, a.M, groups, a.ldd, a.d_group_stride) ? 1 : 0;
   }
@@ -185,6 +185,8 @@ void launch_one(const GemmArgs& a, cudaStream_t stream) {
   p.ce_part_max = a.ce_part_max; p.ce_part_sum = a.ce_part_sum; p.ce_tgt_logit = a.ce_tgt_logit;
   p.ce_ignore_index = a.ce_ignore_index; p.ce_softcap = a.ce_softcap; p.ce_bias = a.ce_bias;
   p.ce_col_offset = a.ce_col_offset;
+  p.ce_part_zsum = a.ce_part_zsum; p.ce_z_loss = a.ce_z_loss; p.ce_smoothing = a.ce_smoothing;
+  p.ce_num_classes = a.ce_num_classes;
 
   const long long m_tiles = (a.M + C::TILE_M - 1) / C::TILE_M, n_tiles = (a.N + BLOCK_N - 1) / BLOCK_N;
   long long tiles = m_tiles * n_tiles * (MODE == GROUPED_K ? a.num_groups : 1) * p.k_splits;

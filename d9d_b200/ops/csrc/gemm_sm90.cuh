@@ -50,7 +50,10 @@ enum Epi : int {
   EPI_BF16_ACC = 3,   // D(bf16) += acc   TMA path: rn(D + rn_bf16(acc)), the add done in bf16 in L2;
                       //                  direct-store path: rn(D + acc) with the add in fp32
   EPI_CE_LSE = 4,     // fused linear-CE forward: per (row, n_tile) running max / sum-exp / target logit
-  EPI_CE_DLOGITS = 5  // fused linear-CE backward: D(bf16) = g[row] * (exp(acc - lse[row]) - [col == target[row]])
+  EPI_CE_DLOGITS = 5, // fused linear-CE backward: D(bf16) = g[row] * (exp(acc - lse[row]) - [col == target[row]])
+  // regularised linear-CE (label smoothing eps, z-loss zeta over V classes in all):
+  EPI_CE_LSE_SUM = 6,    // EPI_CE_LSE + per (row, n_tile) sum of the tile's logits
+  EPI_CE_DLOGITS_REG = 7 // D(bf16) = g[row] * ((1 + 2 zeta lse[row]) p - (1 - eps) [col == target[row]] - eps / V)
 };
 
 // Tensor-parallel communication fused into the GEMM (operands / outputs living in NVLink peer memory):
@@ -101,6 +104,12 @@ struct Params {
   float ce_softcap;            // logits -> softcap * tanh(logits / softcap) (0 = off)
   const float* ce_bias;        // [N] fp32 added to the logits (or nullptr)
   long long ce_col_offset;     // B is a row slice of the classifier: global class id of its first row
+  // regularised CE (appended: the fields above keep their offsets, and Params still ends before the next 64-byte
+  // boundary, where the peer tensor maps of the fused-communication GEMMs begin)
+  float* ce_part_zsum;         // [n_tiles, M]  (LSE_SUM) sum of the tile's logits
+  float ce_z_loss;             // (DLOGITS_REG) zeta
+  float ce_smoothing;          // (DLOGITS_REG) eps
+  int ce_num_classes;          // (DLOGITS_REG) V: classes over all slices of the classifier
 };
 
 // logit transform shared by the fused-CE epilogues: z = softcap(acc + bias); returns z and dz/dacc
@@ -395,7 +404,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       const int col0 = t.n_blk * BLOCK_N;
       const bool have_acc = t.k_blocks > 0;
 
-      if constexpr (EPI == EPI_CE_LSE) {
+      if constexpr (EPI == EPI_CE_LSE || EPI == EPI_CE_LSE_SUM) {
         // softmax statistics of this tile's columns; a row's columns are spread over the 4 threads of a quad.  Accumulator
         // column o = 8 j + e of this thread is class col0 + cq + o: the column loops compare o with per-row bounds only
         const bool ce_xf = (p.ce_bias != nullptr) || (p.ce_softcap > 0.f);  // warp-uniform
@@ -449,10 +458,29 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             p.ce_part_max[static_cast<long long>(t.n_blk) * p.M + row] = mx;
             p.ce_part_sum[static_cast<long long>(t.n_blk) * p.M + row] = sum;
           }
+          if constexpr (EPI == EPI_CE_LSE_SUM) {
+            // the row's logit sum over the tile's valid columns, in a pass of its own once max and sum-exp are stored
+            // (accumulated inside the logits loop it kept one more register live there, and the single-CTA kernel spilt)
+            float zsum = 0.f;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) zsum += (8 * j + e < ncol) ? acc[4 * j + 2 * h + e] : 0.f;
+            }
+            zsum += __shfl_xor_sync(0xffffffffu, zsum, 1);
+            zsum += __shfl_xor_sync(0xffffffffu, zsum, 2);
+            if (row_ok && (lane & 3) == 0) p.ce_part_zsum[static_cast<long long>(t.n_blk) * p.M + row] = zsum;
+          }
         }
       } else {
-        if constexpr (EPI == EPI_CE_DLOGITS) {
-          // D(bf16) = g[row] * (softmax - onehot) * dz/dacc, computed in place on the accumulator (column o as in EPI_CE_LSE)
+        if constexpr (EPI == EPI_CE_DLOGITS || EPI == EPI_CE_DLOGITS_REG) {
+          // D(bf16) = g[row] * (softmax - onehot) * dz/dacc, computed in place on the accumulator (column o as in EPI_CE_LSE).
+          // DLOGITS_REG: g[row] * ((1 + 2 zeta lse) softmax - (1 - eps) onehot - eps / V) * dz/dacc
+          float p_scale = 1.f, hit = 1.f, uniform = 0.f;
+          if constexpr (EPI == EPI_CE_DLOGITS_REG) {
+            hit = 1.f - p.ce_smoothing;
+            uniform = p.ce_smoothing / static_cast<float>(p.ce_num_classes);
+          }
           const bool ce_xf = (p.ce_bias != nullptr) || (p.ce_softcap > 0.f);  // warp-uniform
           const float ce_inv_cap = p.ce_softcap > 0.f ? 1.f / p.ce_softcap : 0.f;
           const int ncol = p.N - col0 - cq;
@@ -469,6 +497,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             }
             const long long tgt_o = tgt - col0 - cq;
             const int trel = (tgt >= 0 && tgt_o >= 0 && tgt_o < BLOCK_N) ? static_cast<int>(tgt_o) : -1;
+            if constexpr (EPI == EPI_CE_DLOGITS_REG) p_scale = fmaf(2.f * p.ce_z_loss, lse, 1.f);
             auto dlogits = [&](auto xf) {
 #pragma unroll
               for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -482,7 +511,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                     z = ce_transform(z, b, p.ce_softcap, ce_inv_cap, dz);
                   }
                   float pr = __expf(z - lse);
-                  if (o == trel) pr -= 1.f;
+                  if constexpr (EPI == EPI_CE_DLOGITS_REG) {
+                    pr = fmaf(pr, p_scale, -uniform);
+                    if (o == trel) pr -= hit;
+                  } else {
+                    if (o == trel) pr -= 1.f;
+                  }
                   acc[4 * j + 2 * h + e] = pr * g * dz;
                 }
               }
@@ -491,7 +525,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             else dlogits(std::false_type{});
           }
         }
-        constexpr bool OUT_BF16 = (EPI == EPI_BF16 || EPI == EPI_BF16_ACC || EPI == EPI_CE_DLOGITS);
+        constexpr bool OUT_BF16 = (EPI == EPI_BF16 || EPI == EPI_BF16_ACC || EPI == EPI_CE_DLOGITS || EPI == EPI_CE_DLOGITS_REG);
         constexpr bool REDUCE = (EPI == EPI_F32_ACC || EPI == EPI_BF16_ACC);
         if (p.tma_epilogue) {
           // ---- TMA epilogue: 128-byte output chunks (32 fp32 / 64 bf16 columns) of the warp's 16 rows, staged swizzled ----
