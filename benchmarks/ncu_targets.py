@@ -65,7 +65,7 @@ def main() -> None:
     wqn = torch.ones(D, **bf)
     ang = torch.rand(B * S, D, device=dev)
     ops.qk_norm_rope_fwd(q.view(B * S, Hq, D), kk.view(B * S, Hk, D), wqn, wqn, ang.cos(), ang.sin(), 1e-6, False, 0)
-    ops.router_topk_fwd(torch.randn(T, E, **bf), None, k, True, "softmax", 1, 1, 1.0)
+    ops.router_topk_fwd(torch.randn(T, E, **bf), None, k, True, "softmax", 1, 1, 1.0, 0)
     torch.cuda.synchronize()
 
 

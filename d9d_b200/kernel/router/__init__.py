@@ -1,5 +1,5 @@
 """Fused MoE routing: fp32 softmax or sigmoid scores + top-k (+ selection bias, + group-limited selection, + renormalisation,
-+ scaling) and its backward, optionally with the softmax router's auxiliary losses folded into that backward.
++ scaling) and its backward, optionally with the router's auxiliary losses folded into that backward.
 
 Auxiliary losses of one call (``T`` tokens, ``E`` experts, top-``k``, ``s = softmax(logits)`` in fp32 - unbiased, not
 renormalised, not scaled - and ``c_e`` the number of the ``T k`` selections that went to expert ``e``):
@@ -21,6 +21,9 @@ actual selections (after bias and group limits) of sequence ``b`` that went to e
 
 The call's objective ``w S coef_seq sum_b A_b`` (``= w T coef_seq mean_b A_b``) is back-propagated the same way, and
 ``(w S sum_b A_b, w T)`` is added to an optional fp32 ``[2]`` accumulator in backward.
+
+All of them are computed from per-sequence statistics (``c[b, e]``, ``sum_{t in b} s[t, e]``, ``sum_{t in b} lse_t^2``):
+the batch losses from the rows summed, which is one sequence of all ``T`` tokens when the sequence-wise loss is off.
 """
 
 from __future__ import annotations
@@ -34,64 +37,38 @@ from torch.autograd import Function
 from .._native import native_ops, on_gpu
 
 
-def _aux_terms(counts: torch.Tensor, score_sum: torch.Tensor, lse2_sum: torch.Tensor, num_tokens: int, top_k: int,
-               lb_coef: float, z_coef: float, token_weight: float) -> tuple[torch.Tensor, float, torch.Tensor]:
-    """One call's statistics (``counts [E]``, ``score_sum [E] = sum_t s[t]``, ``lse2_sum [1] = sum_t lse_t^2``) ->
-    ``g [E]`` fp32 (load balancing: ``dlogits[t] += s_t (g - s_t . g)``), the z-loss factor ``2 w coef_z``
-    (``dlogits[t] += 2 w coef_z lse_t s_t``) and ``(w T A, w T Z, w T)`` fp32 ``[3]``."""
-    num_experts = counts.numel()
-    t = max(num_tokens, 1)  # no tokens: no counts, no gradient, weight 0
-    omega = token_weight * num_tokens
-    c = counts.float()
-    g = c * (token_weight * lb_coef * num_experts / (top_k * t))
-    logged = torch.cat([
-        torch.dot(c, score_sum.float()).reshape(1) * (omega * num_experts / (top_k * t * t)),
-        lse2_sum.float().reshape(1) * (omega / t),
-        lse2_sum.new_full((1,), omega, dtype=torch.float32),
-    ])
-    return g, 2.0 * token_weight * z_coef, logged
-
-
-class _AuxLossGrad(Function):
-    """CPU path (and numerics oracle) of the auxiliary losses: identity on the selected probabilities; backward adds
-    ``w T (coef_lb grad A + coef_z grad Z)`` to the logits' gradient, in fp32 from the plain PyTorch definitions."""
-
-    @staticmethod
-    def forward(ctx: Any, chosen_p: torch.Tensor, logits: torch.Tensor, chosen: torch.Tensor, top_k: int, lb_coef: float,
-                z_coef: float, token_weight: float, sums: torch.Tensor | None):
-        ctx.save_for_backward(logits.detach(), chosen)
-        ctx.args = (top_k, lb_coef, z_coef, token_weight, sums)
-        return chosen_p.view_as(chosen_p)
-
-    @staticmethod
-    def backward(ctx: Any, dprobs: torch.Tensor):  # type: ignore[override]
-        logits, chosen = ctx.saved_tensors
-        top_k, lb_coef, z_coef, token_weight, sums = ctx.args
-        x = logits.reshape(-1, logits.shape[-1]).float()
-        s = F.softmax(x, dim=-1)
-        lse = torch.logsumexp(x, dim=-1)
-        counts = torch.bincount(chosen.reshape(-1), minlength=x.shape[-1])
-        g, zc, logged = _aux_terms(counts, s.sum(0), (lse * lse).sum().reshape(1), x.shape[0], top_k, lb_coef, z_coef,
-                                   token_weight)
-        dlogits = s * (g - (s @ g)[:, None]) + zc * lse[:, None] * s
-        if sums is not None:
-            sums.add_(logged)
-        # autograd adds this term to the selection gradient in the logits' dtype: exact for the fp32 logits the oracle
-        # is used with; for bf16 logits each term is rounded once before the sum (the kernel rounds their fp32 sum)
-        return dprobs, dlogits.to(logits.dtype).reshape(logits.shape), None, None, None, None, None, None
-
-
-def _seq_balance_terms(counts: torch.Tensor, score_sum: torch.Tensor, seq_len: int, top_k: int, coef: float,
-                       token_weight: float) -> tuple[torch.Tensor, torch.Tensor]:
-    """Per-sequence statistics (``counts [B, E]``, ``score_sum [B, E] = sum_{t in b} s[t]``) -> ``g [B, E]`` fp32
-    (``dlogits[t] += ds_t/dx_t^T (g_b - s_t . g_b)``, ``g_b = w coef E c_b / (k S)``) and ``(w S sum_b A_b, w T)``
-    fp32 ``[2]``; device-side, no host synchronisation."""
+def _balance_grad(counts: torch.Tensor, score_sum: torch.Tensor, lse2_sum: torch.Tensor, num_tokens: int, top_k: int,
+                  losses: tuple) -> tuple[torch.Tensor, float]:
+    """Per-sequence statistics of ``num_tokens`` tokens (``counts [B, E]``, ``score_sum [B, E] = sum_{t in b} s[t]``,
+    ``lse2_sum [B] = sum_{t in b} lse_t^2``) -> the balance gradient ``g [B, E]`` fp32 (``dlogits[t] += ds_t/dx_t^T
+    (g_b - s_t . g_b)``) and the z-loss factor ``2 w coef_z`` (``dlogits[t] += 2 w coef_z lse_t s_t``).  Adds
+    ``(w S sum_b A_b, w T)`` to the sequence accumulator and ``(w T A, w T Z, w T)`` to the batch one; device-side, no
+    host synchronisation."""
+    seq_len, seq_coef, lb_coef, z_coef, token_weight, seq_sums, aux_sums = losses
     num_seqs, num_experts = counts.shape
     c = counts.float()
-    per_count = token_weight * num_experts / (top_k * seq_len)
-    logged = torch.cat([(c * score_sum.float()).sum().reshape(1) * per_count,
-                        counts.new_full((1,), token_weight * num_seqs * seq_len, dtype=torch.float32)])
-    return c * (per_count * coef), logged
+    g, zc = None, 0.0
+    if seq_coef > 0:  # sequence-wise balance, per row: g_b = w coef E c_b / (k S)
+        per_count = token_weight * num_experts / (top_k * seq_len)
+        g = c * (per_count * seq_coef)
+        if seq_sums is not None:
+            seq_sums.add_(torch.cat([(c * score_sum.float()).sum().reshape(1) * per_count,
+                                     c.new_full((1,), token_weight * num_tokens)]))
+    if lb_coef > 0 or z_coef > 0:  # batch load balancing and z-loss: from the rows summed, broadcast to every row
+        if num_seqs != 1:
+            c, score_sum, lse2_sum = c.sum(0, keepdim=True), score_sum.sum(0, keepdim=True), lse2_sum.sum().reshape(1)
+        t = max(num_tokens, 1)  # no tokens: no counts, no gradient, weight 0
+        omega = token_weight * num_tokens
+        g_batch = c * (token_weight * lb_coef * num_experts / (top_k * t))
+        g = g_batch if g is None else g + g_batch
+        zc = 2.0 * token_weight * z_coef
+        if aux_sums is not None:
+            aux_sums.add_(torch.cat([
+                torch.dot(c.view(-1), score_sum.float().view(-1)).reshape(1) * (omega * num_experts / (top_k * t * t)),
+                lse2_sum.float().reshape(1) * (omega / t),
+                c.new_full((1,), omega),
+            ]))
+    return g, zc
 
 
 def _balance_scores(x: torch.Tensor, score_function: str) -> tuple[torch.Tensor, torch.Tensor]:
@@ -105,33 +82,38 @@ def _balance_scores(x: torch.Tensor, score_function: str) -> tuple[torch.Tensor,
     return sig / total, sig * (1 - sig) / total
 
 
-class _SeqBalanceGrad(Function):
-    """CPU path (and numerics oracle) of the sequence-wise balance loss: identity on the selected probabilities; backward
-    adds ``w S coef_seq grad sum_b A_b`` to the logits' gradient, in fp32 from the plain PyTorch definition."""
+class _BalanceLossGrad(Function):
+    """CPU path (and numerics oracle) of the auxiliary losses: identity on the selected probabilities; backward computes
+    the ``num_seqs`` sequences' statistics and adds the losses' gradient to the logits' gradient, in fp32 from the plain
+    PyTorch definitions."""
 
     @staticmethod
     def forward(ctx: Any, chosen_p: torch.Tensor, logits: torch.Tensor, chosen: torch.Tensor, top_k: int, score_function: str,
-                seq_len: int, coef: float, token_weight: float, sums: torch.Tensor | None):
+                num_seqs: int, losses: tuple):
         ctx.save_for_backward(logits.detach(), chosen)
-        ctx.args = (top_k, score_function, seq_len, coef, token_weight, sums)
+        ctx.args = (top_k, score_function, num_seqs, losses)
         return chosen_p.view_as(chosen_p)
 
     @staticmethod
     def backward(ctx: Any, dprobs: torch.Tensor):  # type: ignore[override]
         logits, chosen = ctx.saved_tensors
-        top_k, score_function, seq_len, coef, token_weight, sums = ctx.args
+        top_k, score_function, num_seqs, losses = ctx.args
         x = logits.reshape(-1, logits.shape[-1]).float()
-        num_seqs, num_experts = x.shape[0] // seq_len, x.shape[1]
+        num_tokens, num_experts = x.shape
+        seq_len = num_tokens // num_seqs
         s, d = _balance_scores(x, score_function)
+        lse = torch.logsumexp(x, dim=-1) if score_function == "softmax" else x.new_zeros(num_tokens)
         sel = chosen.reshape(num_seqs, seq_len * top_k)
         counts = torch.zeros(num_seqs, num_experts, dtype=torch.int64, device=x.device).scatter_add_(1, sel, torch.ones_like(sel))
-        g, logged = _seq_balance_terms(counts, s.reshape(num_seqs, seq_len, num_experts).sum(1), seq_len, top_k, coef,
-                                       token_weight)
+        g, zc = _balance_grad(counts, s.reshape(num_seqs, seq_len, num_experts).sum(1),
+                              (lse * lse).reshape(num_seqs, seq_len).sum(1), num_tokens, top_k, losses)
         g = g.repeat_interleave(seq_len, dim=0)
         dlogits = d * (g - (s * g).sum(-1, keepdim=True))
-        if sums is not None:
-            sums.add_(logged)
-        return dprobs, dlogits.to(logits.dtype).reshape(logits.shape), None, None, None, None, None, None, None
+        if zc:
+            dlogits = dlogits + zc * lse[:, None] * s
+        # autograd adds this term to the selection gradient in the logits' dtype: exact for the fp32 logits the oracle
+        # is used with; for bf16 logits it is rounded once before the sum (the kernel rounds their fp32 sum)
+        return dprobs, dlogits.to(logits.dtype).reshape(logits.shape), None, None, None, None, None
 
 
 def route_topk_reference(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None):
@@ -148,88 +130,29 @@ def route_topk_reference(logits: torch.Tensor, top_k: int, renormalize: bool, ex
 
 
 class _RouteTopK(Function):
-    @staticmethod
-    def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None,
-                score_function: str, num_groups: int, topk_groups: int, scaling_factor: float):
-        idx, probs = native_ops().router_topk_fwd(logits, expert_bias, top_k, renormalize, score_function, num_groups,
-                                                  topk_groups, scaling_factor)
-        ctx.save_for_backward(logits, idx)
-        ctx.renormalize = renormalize
-        ctx.score_function = score_function
-        ctx.scaling_factor = scaling_factor
-        ctx.mark_non_differentiable(idx)
-        return idx, probs
-
-    @staticmethod
-    def backward(ctx: Any, _didx: torch.Tensor, dprobs: torch.Tensor):  # type: ignore[override]
-        logits, idx = ctx.saved_tensors
-        dlogits = native_ops().router_topk_bwd(logits, idx, dprobs.float().contiguous(), ctx.renormalize, ctx.score_function,
-                                               ctx.scaling_factor)
-        return dlogits, None, None, None, None, None, None, None
-
-
-class _RouteTopKAux(Function):
-    """Softmax routing on the fused kernel with the auxiliary-loss statistics from the same pass (deterministic, so a
-    recomputed forward reproduces them bit for bit) and both auxiliary gradients folded into the fused backward."""
+    """Routing on the fused kernel.  With auxiliary losses (``num_seqs > 0``) the same pass also produces the per-sequence
+    statistics (deterministic, so a recomputed forward reproduces them bit for bit) and the losses' gradients are folded
+    into the fused backward."""
 
     @staticmethod
     def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None,
-                num_groups: int, topk_groups: int, scaling_factor: float, lb_coef: float, z_coef: float, token_weight: float,
-                sums: torch.Tensor | None):
-        idx, probs, counts, score_sum, lse2_sum = native_ops().router_topk_aux_fwd(
-            logits, expert_bias, top_k, renormalize, num_groups, topk_groups, scaling_factor)
+                score_function: str, num_groups: int, topk_groups: int, scaling_factor: float, num_seqs: int,
+                losses: tuple | None):
+        idx, probs, counts, score_sum, lse2_sum = native_ops().router_topk_fwd(
+            logits, expert_bias, top_k, renormalize, score_function, num_groups, topk_groups, scaling_factor, num_seqs)
         ctx.save_for_backward(logits, idx, counts, score_sum, lse2_sum)
-        ctx.args = (renormalize, scaling_factor, top_k, lb_coef, z_coef, token_weight, sums)
+        ctx.args = (renormalize, score_function, scaling_factor, top_k, losses)
         ctx.mark_non_differentiable(idx)
         return idx, probs
 
     @staticmethod
     def backward(ctx: Any, _didx: torch.Tensor, dprobs: torch.Tensor):  # type: ignore[override]
         logits, idx, counts, score_sum, lse2_sum = ctx.saved_tensors
-        renormalize, scaling_factor, top_k, lb_coef, z_coef, token_weight, sums = ctx.args
-        g, zc, logged = _aux_terms(counts, score_sum, lse2_sum, logits.shape[0], top_k, lb_coef, z_coef, token_weight)
-        dlogits = native_ops().router_topk_aux_bwd(logits, idx, dprobs.float().contiguous(), renormalize, scaling_factor, g, zc)
-        if sums is not None:
-            sums.add_(logged)
-        return dlogits, None, None, None, None, None, None, None, None, None, None
-
-
-class _RouteTopKSeq(Function):
-    """Routing on the fused kernel with per-sequence statistics from the same pass (deterministic, so a recomputed forward
-    reproduces them bit for bit) and the sequence-wise balance gradient - plus, for softmax, the batch load-balancing and
-    z-loss gradients, whose statistics are the per-sequence ones summed - folded into the fused backward."""
-
-    @staticmethod
-    def forward(ctx: Any, logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None,
-                score_function: str, num_groups: int, topk_groups: int, scaling_factor: float, seq_len: int, seq_coef: float,
-                lb_coef: float, z_coef: float, token_weight: float, seq_sums: torch.Tensor | None,
-                aux_sums: torch.Tensor | None):
-        idx, probs, counts, score_sum, lse2_sum = native_ops().router_topk_seq_fwd(
-            logits, expert_bias, top_k, renormalize, score_function, num_groups, topk_groups, scaling_factor, seq_len)
-        ctx.save_for_backward(logits, idx, counts, score_sum, lse2_sum)
-        ctx.args = (renormalize, score_function, scaling_factor, top_k, seq_len, seq_coef, lb_coef, z_coef, token_weight,
-                    seq_sums, aux_sums)
-        ctx.mark_non_differentiable(idx)
-        return idx, probs
-
-    @staticmethod
-    def backward(ctx: Any, _didx: torch.Tensor, dprobs: torch.Tensor):  # type: ignore[override]
-        logits, idx, counts, score_sum, lse2_sum = ctx.saved_tensors
-        (renormalize, score_function, scaling_factor, top_k, seq_len, seq_coef, lb_coef, z_coef, token_weight, seq_sums,
-         aux_sums) = ctx.args
-        g, logged = _seq_balance_terms(counts, score_sum, seq_len, top_k, seq_coef, token_weight)
-        zc = 0.0
-        if lb_coef > 0 or z_coef > 0:
-            g_batch, zc, aux_logged = _aux_terms(counts.sum(0), score_sum.sum(0), lse2_sum.sum().reshape(1), logits.shape[0],
-                                                 top_k, lb_coef, z_coef, token_weight)
-            g = g + g_batch
-            if aux_sums is not None:
-                aux_sums.add_(aux_logged)
-        dlogits = native_ops().router_topk_seq_bwd(logits, idx, dprobs.float().contiguous(), renormalize, score_function,
-                                                   scaling_factor, g.contiguous(), zc, seq_len)
-        if seq_sums is not None:
-            seq_sums.add_(logged)
-        return dlogits, *([None] * 14)
+        renormalize, score_function, scaling_factor, top_k, losses = ctx.args
+        g, zc = (None, 0.0) if losses is None else _balance_grad(counts, score_sum, lse2_sum, logits.shape[0], top_k, losses)
+        dlogits = native_ops().router_topk_bwd(logits, idx, dprobs.float().contiguous(), renormalize, score_function,
+                                               scaling_factor, g, zc)
+        return dlogits, *([None] * 9)
 
 
 def route_topk_general(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias: torch.Tensor | None = None,
@@ -319,6 +242,13 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
                                                   or sequence_balance_sums.shape != (2,)
                                                   or sequence_balance_sums.device != logits.device):
             raise ValueError("sequence_balance_sums must be an fp32 [2] tensor on the logits' device")
+    # statistics per sequence: T / S sequences for the sequence-wise loss (one empty one without tokens), one for the batch
+    # losses alone, none without a loss
+    num_seqs = max(logits.shape[:-1].numel() // sequence_length, 1) if seq else int(aux)
+    losses = None
+    if aux or seq:
+        losses = (sequence_length, float(sequence_balance_coef), float(load_balancing_coef), float(z_loss_coef),
+                  float(token_loss_weight), sequence_balance_sums, aux_loss_sums)
     if (on_gpu(logits) and logits.dtype == torch.bfloat16 and num_experts <= 1024 and top_k <= min(32, num_experts)
             and num_groups <= 32):
         flat = logits.reshape(logits.shape[:-1].numel(), num_experts)  # also when there are no tokens
@@ -326,29 +256,16 @@ def route_topk(logits: torch.Tensor, top_k: int, renormalize: bool, expert_bias:
             flat = flat.contiguous()
         groups = (num_groups, topk_groups) if num_groups > 1 else (1, 1)
         bias = None if expert_bias is None else expert_bias.float().contiguous()
-        if seq:
-            idx, probs = _RouteTopKSeq.apply(flat, top_k, renormalize, bias, score_function, *groups, float(scaling_factor),
-                                             int(sequence_length), float(sequence_balance_coef), float(load_balancing_coef),
-                                             float(z_loss_coef), float(token_loss_weight), sequence_balance_sums,
-                                             aux_loss_sums)
-        elif aux:
-            idx, probs = _RouteTopKAux.apply(flat, top_k, renormalize, bias, *groups, float(scaling_factor),
-                                             float(load_balancing_coef), float(z_loss_coef), float(token_loss_weight),
-                                             aux_loss_sums)
-        else:
-            idx, probs = _RouteTopK.apply(flat, top_k, renormalize, bias, score_function, *groups, float(scaling_factor))
+        idx, probs = _RouteTopK.apply(flat, top_k, renormalize, bias, score_function, *groups, float(scaling_factor),
+                                      num_seqs, losses)
         return idx.view(*logits.shape[:-1], top_k), probs.view(*logits.shape[:-1], top_k)
     if score_function != "softmax" or num_groups > 1 or scaling_factor != 1.0:
         chosen, chosen_p = route_topk_general(logits, top_k, renormalize, expert_bias, score_function, num_groups, topk_groups,
                                               scaling_factor)
     else:
         chosen, chosen_p = route_topk_reference(logits, top_k, renormalize, expert_bias)
-    if aux:
-        chosen_p = _AuxLossGrad.apply(chosen_p, logits, chosen, top_k, float(load_balancing_coef), float(z_loss_coef),
-                                      float(token_loss_weight), aux_loss_sums)
-    if seq:
-        chosen_p = _SeqBalanceGrad.apply(chosen_p, logits, chosen, top_k, score_function, int(sequence_length),
-                                         float(sequence_balance_coef), float(token_loss_weight), sequence_balance_sums)
+    if losses is not None:
+        chosen_p = _BalanceLossGrad.apply(chosen_p, logits, chosen, top_k, score_function, num_seqs, losses)
     return chosen, chosen_p
 
 

@@ -776,146 +776,78 @@ static bool router_sigmoid(c10::string_view score_function) {
   return score_function == "sigmoid";
 }
 
-std::tuple<Tensor, Tensor> router_topk_fwd(const Tensor& logits, const c10::optional<Tensor>& bias, int64_t k, bool renorm,
-                                           c10::string_view score_function, int64_t num_groups, int64_t topk_groups,
-                                           double scaling_factor) {
+std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor> router_topk_fwd(const Tensor& logits, const c10::optional<Tensor>& bias,
+                                                                   int64_t k, bool renorm, c10::string_view score_function,
+                                                                   int64_t num_groups, int64_t topk_groups,
+                                                                   double scaling_factor, int64_t num_seqs) {
   CHECK_CUDA_CONTIG(logits);
   TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && logits.dim() == 2);
   const bool sigmoid = router_sigmoid(score_function);
-  c10::cuda::CUDAGuard guard(logits.device());
   const int64_t T = logits.size(0), E = logits.size(1);
+  TORCH_CHECK(num_seqs == 0 || (num_seqs > 0 && T % num_seqs == 0), "router fwd: the sequence count must be 0 (no "
+              "statistics) or a positive divisor of the token count");
   const float* b = nullptr;
   if (bias.has_value()) {
     TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->scalar_type() == at::kFloat && bias->numel() == E);
+    TORCH_CHECK(bias->device() == logits.device(), "router fwd: the bias must be on the logits' device");
     b = bias->data_ptr<float>();
   }
+  c10::cuda::CUDAGuard guard(logits.device());
   Tensor idx = at::empty({T, k}, logits.options().dtype(at::kLong));
   Tensor probs = at::empty({T, k}, logits.options().dtype(at::kFloat));
+  if (num_seqs == 0) {  // no statistics: undefined outputs (None in Python), so the plain call allocates nothing more
+    d9d::router_topk_fwd(logits.data_ptr(), b, T, static_cast<int>(E), static_cast<int>(k), renorm, sigmoid,
+                         static_cast<int>(num_groups), static_cast<int>(topk_groups), static_cast<float>(scaling_factor),
+                         reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), probs.data_ptr<float>(), 0, nullptr,
+                         nullptr, nullptr, nullptr, nullptr, nullptr, cur_stream());
+    return {idx, probs, Tensor(), Tensor(), Tensor()};
+  }
+  const int64_t parts = d9d::router_stat_parts(T, num_seqs);
+  Tensor part_counts = at::empty({parts, E}, logits.options().dtype(at::kInt));
+  Tensor part_scores = at::empty({parts, E}, logits.options().dtype(at::kFloat));
+  Tensor part_lse2 = at::empty({parts}, logits.options().dtype(at::kFloat));
+  Tensor counts = at::empty({num_seqs, E}, logits.options().dtype(at::kInt));
+  Tensor score_sum = at::empty({num_seqs, E}, logits.options().dtype(at::kFloat));
+  Tensor lse2_sum = at::empty({num_seqs}, logits.options().dtype(at::kFloat));
   d9d::router_topk_fwd(logits.data_ptr(), b, T, static_cast<int>(E), static_cast<int>(k), renorm, sigmoid,
                        static_cast<int>(num_groups), static_cast<int>(topk_groups), static_cast<float>(scaling_factor),
-                       reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), probs.data_ptr<float>(), cur_stream());
-  return {idx, probs};
+                       reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), probs.data_ptr<float>(), num_seqs,
+                       part_counts.data_ptr<int>(), part_scores.data_ptr<float>(), part_lse2.data_ptr<float>(),
+                       counts.data_ptr<int>(), score_sum.data_ptr<float>(), lse2_sum.data_ptr<float>(), cur_stream());
+  return {idx, probs, counts, score_sum, lse2_sum};
 }
 
-Tensor router_topk_bwd(const Tensor& logits, const Tensor& idx, const Tensor& dprobs, bool renorm, c10::string_view score_function,
-                       double scaling_factor) {
+// balance_grad [B, E] (B dividing T): the balance gradient row of each sequence of T / B tokens
+Tensor router_topk_bwd(const Tensor& logits, const Tensor& idx, const Tensor& dprobs, bool renorm,
+                       c10::string_view score_function, double scaling_factor, const c10::optional<Tensor>& balance_grad,
+                       double z_coef) {
   CHECK_CUDA_CONTIG(logits); CHECK_CUDA_CONTIG(idx); CHECK_CUDA_CONTIG(dprobs);
   TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && idx.scalar_type() == at::kLong && dprobs.scalar_type() == at::kFloat);
   const bool sigmoid = router_sigmoid(score_function);
-  c10::cuda::CUDAGuard guard(logits.device());
-  const int64_t T = logits.size(0), E = logits.size(1), k = idx.size(1);
-  Tensor out = at::empty_like(logits);
-  d9d::router_topk_bwd(logits.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dprobs.data_ptr<float>(), T,
-                       static_cast<int>(E), static_cast<int>(k), renorm, sigmoid, static_cast<float>(scaling_factor),
-                       out.data_ptr(), cur_stream());
-  return out;
-}
-
-std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor> router_topk_aux_fwd(const Tensor& logits, const c10::optional<Tensor>& bias,
-                                                                       int64_t k, bool renorm, int64_t num_groups,
-                                                                       int64_t topk_groups, double scaling_factor) {
-  CHECK_CUDA_CONTIG(logits);
-  TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && logits.dim() == 2);
-  c10::cuda::CUDAGuard guard(logits.device());
-  const int64_t T = logits.size(0), E = logits.size(1);
-  const float* b = nullptr;
-  if (bias.has_value()) {
-    TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->scalar_type() == at::kFloat && bias->numel() == E);
-    TORCH_CHECK(bias->device() == logits.device(), "router aux fwd: the bias must be on the logits' device");
-    b = bias->data_ptr<float>();
-  }
-  Tensor idx = at::empty({T, k}, logits.options().dtype(at::kLong));
-  Tensor probs = at::empty({T, k}, logits.options().dtype(at::kFloat));
-  const int64_t parts = d9d::router_aux_parts(T);
-  Tensor part_counts = at::empty({parts, E}, logits.options().dtype(at::kInt));
-  Tensor part_scores = at::empty({parts, E}, logits.options().dtype(at::kFloat));
-  Tensor part_lse2 = at::empty({parts}, logits.options().dtype(at::kFloat));
-  Tensor counts = at::empty({E}, logits.options().dtype(at::kInt));
-  Tensor score_sum = at::empty({E}, logits.options().dtype(at::kFloat));
-  Tensor lse2_sum = at::empty({1}, logits.options().dtype(at::kFloat));
-  d9d::router_topk_aux_fwd(logits.data_ptr(), b, T, static_cast<int>(E), static_cast<int>(k), renorm, static_cast<int>(num_groups),
-                           static_cast<int>(topk_groups), static_cast<float>(scaling_factor),
-                           reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), probs.data_ptr<float>(),
-                           part_counts.data_ptr<int>(), part_scores.data_ptr<float>(), part_lse2.data_ptr<float>(),
-                           counts.data_ptr<int>(), score_sum.data_ptr<float>(), lse2_sum.data_ptr<float>(), cur_stream());
-  return {idx, probs, counts, score_sum, lse2_sum};
-}
-
-Tensor router_topk_aux_bwd(const Tensor& logits, const Tensor& idx, const Tensor& dprobs, bool renorm, double scaling_factor,
-                           const Tensor& lb_grad, double z_coef) {
-  CHECK_CUDA_CONTIG(logits); CHECK_CUDA_CONTIG(idx); CHECK_CUDA_CONTIG(dprobs); CHECK_CUDA_CONTIG(lb_grad);
-  TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && idx.scalar_type() == at::kLong && dprobs.scalar_type() == at::kFloat);
   TORCH_CHECK(logits.dim() == 2 && idx.dim() == 2 && idx.size(0) == logits.size(0) && dprobs.sizes() == idx.sizes(),
-              "router aux bwd: idx and dprobs must be [T, k] for logits [T, E]");
-  TORCH_CHECK(lb_grad.scalar_type() == at::kFloat && lb_grad.numel() == logits.size(1),
-              "router aux bwd: the load-balancing gradient must be fp32 [E]");
-  TORCH_CHECK(idx.device() == logits.device() && dprobs.device() == logits.device() && lb_grad.device() == logits.device(),
-              "router aux bwd: all operands must be on the logits' device");
-  c10::cuda::CUDAGuard guard(logits.device());
+              "router bwd: idx and dprobs must be [T, k] for logits [T, E]");
+  TORCH_CHECK(idx.device() == logits.device() && dprobs.device() == logits.device(),
+              "router bwd: all operands must be on the logits' device");
   const int64_t T = logits.size(0), E = logits.size(1), k = idx.size(1);
-  Tensor out = at::empty_like(logits);
-  d9d::router_topk_aux_bwd(logits.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dprobs.data_ptr<float>(),
-                           T, static_cast<int>(E), static_cast<int>(k), renorm, static_cast<float>(scaling_factor),
-                           lb_grad.data_ptr<float>(), static_cast<float>(z_coef), out.data_ptr(), cur_stream());
-  return out;
-}
-
-std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor> router_topk_seq_fwd(const Tensor& logits, const c10::optional<Tensor>& bias,
-                                                                       int64_t k, bool renorm, c10::string_view score_function,
-                                                                       int64_t num_groups, int64_t topk_groups,
-                                                                       double scaling_factor, int64_t seq_len) {
-  CHECK_CUDA_CONTIG(logits);
-  TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && logits.dim() == 2);
-  const bool sigmoid = router_sigmoid(score_function);
-  const int64_t T = logits.size(0), E = logits.size(1);
-  TORCH_CHECK(seq_len > 0 && T % seq_len == 0, "router seq fwd: the sequence length must be a positive divisor of the "
-              "token count");
-  const float* b = nullptr;
-  if (bias.has_value()) {
-    TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->scalar_type() == at::kFloat && bias->numel() == E);
-    TORCH_CHECK(bias->device() == logits.device(), "router seq fwd: the bias must be on the logits' device");
-    b = bias->data_ptr<float>();
+  const float* g = nullptr;
+  int64_t B = 0;
+  if (balance_grad.has_value()) {
+    CHECK_CUDA_CONTIG((*balance_grad));
+    TORCH_CHECK(balance_grad->scalar_type() == at::kFloat && balance_grad->dim() == 2 && balance_grad->size(1) == E,
+                "router bwd: the balance gradient must be fp32 [B, E]");
+    TORCH_CHECK(balance_grad->device() == logits.device(), "router bwd: all operands must be on the logits' device");
+    B = balance_grad->size(0);
+    TORCH_CHECK(B > 0 && T % B == 0, "router bwd: the balance gradient's row count must be a positive divisor of the "
+                "token count");
+    g = balance_grad->data_ptr<float>();
   }
-  c10::cuda::CUDAGuard guard(logits.device());
-  const int64_t seqs = T / seq_len;
-  Tensor idx = at::empty({T, k}, logits.options().dtype(at::kLong));
-  Tensor probs = at::empty({T, k}, logits.options().dtype(at::kFloat));
-  const int64_t parts = seqs * d9d::router_seq_parts(T, seq_len);
-  Tensor part_counts = at::empty({parts, E}, logits.options().dtype(at::kInt));
-  Tensor part_scores = at::empty({parts, E}, logits.options().dtype(at::kFloat));
-  Tensor part_lse2 = at::empty({parts}, logits.options().dtype(at::kFloat));
-  Tensor counts = at::empty({seqs, E}, logits.options().dtype(at::kInt));
-  Tensor score_sum = at::empty({seqs, E}, logits.options().dtype(at::kFloat));
-  Tensor lse2_sum = at::empty({seqs}, logits.options().dtype(at::kFloat));
-  d9d::router_topk_seq_fwd(logits.data_ptr(), b, T, static_cast<int>(E), static_cast<int>(k), renorm, sigmoid,
-                           static_cast<int>(num_groups), static_cast<int>(topk_groups), static_cast<float>(scaling_factor),
-                           seq_len, reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), probs.data_ptr<float>(),
-                           part_counts.data_ptr<int>(), part_scores.data_ptr<float>(), part_lse2.data_ptr<float>(),
-                           counts.data_ptr<int>(), score_sum.data_ptr<float>(), lse2_sum.data_ptr<float>(), cur_stream());
-  return {idx, probs, counts, score_sum, lse2_sum};
-}
-
-Tensor router_topk_seq_bwd(const Tensor& logits, const Tensor& idx, const Tensor& dprobs, bool renorm,
-                           c10::string_view score_function, double scaling_factor, const Tensor& balance_grad,
-                           double z_coef, int64_t seq_len) {
-  CHECK_CUDA_CONTIG(logits); CHECK_CUDA_CONTIG(idx); CHECK_CUDA_CONTIG(dprobs); CHECK_CUDA_CONTIG(balance_grad);
-  TORCH_CHECK(logits.scalar_type() == at::kBFloat16 && idx.scalar_type() == at::kLong && dprobs.scalar_type() == at::kFloat);
-  const bool sigmoid = router_sigmoid(score_function);
-  TORCH_CHECK(logits.dim() == 2 && idx.dim() == 2 && idx.size(0) == logits.size(0) && dprobs.sizes() == idx.sizes(),
-              "router seq bwd: idx and dprobs must be [T, k] for logits [T, E]");
-  const int64_t T = logits.size(0), E = logits.size(1), k = idx.size(1);
-  TORCH_CHECK(seq_len > 0 && T % seq_len == 0, "router seq bwd: the sequence length must be a positive divisor of the "
-              "token count");
-  TORCH_CHECK(balance_grad.scalar_type() == at::kFloat && balance_grad.dim() == 2 && balance_grad.size(0) == T / seq_len &&
-              balance_grad.size(1) == E, "router seq bwd: the balance gradient must be fp32 [T / seq_len, E]");
-  TORCH_CHECK(!sigmoid || z_coef == 0.0, "router seq bwd: the z-loss is defined for softmax routers only");
-  TORCH_CHECK(idx.device() == logits.device() && dprobs.device() == logits.device() && balance_grad.device() == logits.device(),
-              "router seq bwd: all operands must be on the logits' device");
+  TORCH_CHECK(z_coef == 0.0 || (g && !sigmoid), "router bwd: the z-loss is defined for softmax routers only, with a "
+              "balance gradient");
   c10::cuda::CUDAGuard guard(logits.device());
   Tensor out = at::empty_like(logits);
-  d9d::router_topk_seq_bwd(logits.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dprobs.data_ptr<float>(),
-                           T, static_cast<int>(E), static_cast<int>(k), renorm, sigmoid, static_cast<float>(scaling_factor),
-                           balance_grad.data_ptr<float>(), static_cast<float>(z_coef), seq_len, out.data_ptr(), cur_stream());
+  d9d::router_topk_bwd(logits.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dprobs.data_ptr<float>(),
+                       T, static_cast<int>(E), static_cast<int>(k), renorm, sigmoid, static_cast<float>(scaling_factor), g,
+                       B, static_cast<float>(z_coef), out.data_ptr(), cur_stream());
   return out;
 }
 
@@ -1123,16 +1055,9 @@ TORCH_LIBRARY(d9d_b200, m) {
   m.def("qk_norm_rope_bwd(Tensor dq_out, Tensor dk_out, Tensor q, Tensor k, Tensor wq, Tensor wk, Tensor cos_t, Tensor sin_t, "
         "Tensor inv_rms, bool zero_centered, int style) -> (Tensor, Tensor, Tensor, Tensor)");
   m.def("router_topk_fwd(Tensor logits, Tensor? bias, int k, bool renorm, str score_function, int num_groups, int topk_groups, "
-        "float scaling_factor) -> (Tensor, Tensor)");
-  m.def("router_topk_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm, str score_function, float scaling_factor) -> Tensor");
-  m.def("router_topk_aux_fwd(Tensor logits, Tensor? bias, int k, bool renorm, int num_groups, int topk_groups, "
-        "float scaling_factor) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
-  m.def("router_topk_aux_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm, float scaling_factor, Tensor lb_grad, "
-        "float z_coef) -> Tensor");
-  m.def("router_topk_seq_fwd(Tensor logits, Tensor? bias, int k, bool renorm, str score_function, int num_groups, "
-        "int topk_groups, float scaling_factor, int seq_len) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
-  m.def("router_topk_seq_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm, str score_function, float scaling_factor, "
-        "Tensor balance_grad, float z_coef, int seq_len) -> Tensor");
+        "float scaling_factor, int num_seqs) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
+  m.def("router_topk_bwd(Tensor logits, Tensor idx, Tensor dprobs, bool renorm, str score_function, float scaling_factor, "
+        "Tensor? balance_grad, float z_coef) -> Tensor");
   m.def("gemm_ag_a(int[] a_peer_ptrs, int rows_local, int lda, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int block_n=0) -> ()");
   m.def("gemm_wait_a(Tensor a, Tensor flags, int rank, int block_rows, Tensor b, Tensor(a!) d, bool b_mn, int spare_sms=0, "
         "int block_n=0) -> ()");
@@ -1184,10 +1109,6 @@ TORCH_LIBRARY_IMPL(d9d_b200, CUDA, m) {
   m.impl("qk_norm_rope_bwd", &qk_norm_rope_bwd);
   m.impl("router_topk_fwd", &router_topk_fwd);
   m.impl("router_topk_bwd", &router_topk_bwd);
-  m.impl("router_topk_aux_fwd", &router_topk_aux_fwd);
-  m.impl("router_topk_aux_bwd", &router_topk_aux_bwd);
-  m.impl("router_topk_seq_fwd", &router_topk_seq_fwd);
-  m.impl("router_topk_seq_bwd", &router_topk_seq_bwd);
   m.impl("gemm_ag_a", &gemm_ag_a);
   m.impl("gemm_wait_a", &gemm_wait_a);
   m.impl("gemm_rs_d", &gemm_rs_d);

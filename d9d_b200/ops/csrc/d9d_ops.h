@@ -209,38 +209,24 @@ void qk_norm_rope_bwd(const void* dq_out, const void* dk_out, const void* q, con
 // ------------------------------------------------------------------ MoE router -----------------------------
 // logits [T, E] bf16 -> scores (fp32 softmax, or sigmoid) -> top-k by (score + bias), optionally only among the
 // topk_groups best of num_groups expert groups (group score: sum of its two best keys; dropped experts get key 0) ->
-// idx [T, k] int64, probs [T, k] fp32 = scale * score (renormalised over the k when renorm)
+// idx [T, k] int64, probs [T, k] fp32 = scale * score (renormalised over the k when renorm).
+// With num_seqs > 0 (a divisor of T) also the auxiliary-loss statistics of the num_seqs sequences of T / num_seqs
+// consecutive tokens, deterministic (no atomics): counts [num_seqs, E] int32 (selections per expert),
+// score_sum [num_seqs, E] = sum_{t in seq} s[t] (softmax: s = softmax(x_t); sigmoid: s = sigma(x_t) / sum_j sigma(x_t)_j)
+// and lse2_sum [num_seqs] = sum_{t in seq} lse_t^2 (softmax; zeros for sigmoid), via part_counts [P, E],
+// part_scores [P, E], part_lse2 [P] with P = router_stat_parts(T, num_seqs) (0 when T = 0: zeros are written).
+// With num_seqs = 0 the statistics pointers are unused (may be null).
+int router_stat_parts(long long T, long long num_seqs);
 void router_topk_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
-                     int num_groups, int topk_groups, float scale, long long* idx, float* probs, cudaStream_t stream);
+                     int num_groups, int topk_groups, float scale, long long* idx, float* probs, long long num_seqs,
+                     int* part_counts, float* part_scores, float* part_lse2, int* counts, float* score_sum,
+                     float* lse2_sum, cudaStream_t stream);
+// With g != nullptr, plus the balance gradient of g [num_seqs, E] fp32 (num_seqs a divisor of T), row t / (T / num_seqs)
+// for token t: softmax dlogits[t, e] += s_e (g_e - s.g) + z_coef lse_t s_e (z_coef = 2 w_tok coef_z); sigmoid
+// dlogits[t, e] += sigma_e (1 - sigma_e) (g_e - s.g) / sum_j sigma_j
 void router_topk_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                     bool renorm, bool sigmoid, float scale, void* dlogits, cudaStream_t stream);
-// Softmax routing with the auxiliary-loss statistics, deterministic (no atomics): the same idx / probs, plus
-// counts [E] int32 (selections per expert), score_sum [E] = sum_t softmax(x_t)[e] and lse2_sum [1] = sum_t lse_t^2, via
-// part_counts [P, E], part_scores [P, E], part_lse2 [P] with P = router_aux_parts(T) (0 when T = 0: zeros are written).
-int router_aux_parts(long long T);
-void router_topk_aux_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, int num_groups,
-                         int topk_groups, float scale, long long* idx, float* probs, int* part_counts,
-                         float* part_scores, float* part_lse2, int* counts, float* score_sum, float* lse2_sum,
-                         cudaStream_t stream);
-// router_topk_bwd for softmax, plus the auxiliary gradients: dlogits[t, e] += s_e (g_e - sum_j s_j g_j) + z_coef lse_t s_e
-// with g [E] fp32 (load-balancing term) and z_coef = 2 w_tok coef_z (z-loss term)
-void router_topk_aux_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                         bool renorm, float scale, const float* g, float z_coef, void* dlogits, cudaStream_t stream);
-// Routing with per-sequence statistics for the sequence-wise balance loss (softmax or sigmoid), deterministic: the same
-// idx / probs, plus for each of the T / seq_len sequences of seq_len consecutive tokens counts [T / seq_len, E] int32,
-// score_sum [T / seq_len, E] = sum_{t in seq} s[t] (softmax: s = softmax(x_t); sigmoid: s = sigma(x_t) / sum_j sigma(x_t)_j)
-// and lse2_sum [T / seq_len] = sum_{t in seq} lse_t^2 (softmax; zeros for sigmoid), via part_counts [P, E],
-// part_scores [P, E], part_lse2 [P] with P = T / seq_len * router_seq_parts(T, seq_len).  seq_len must divide T.
-int router_seq_parts(long long T, long long seq_len);
-void router_topk_seq_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
-                         int num_groups, int topk_groups, float scale, long long seq_len, long long* idx, float* probs,
-                         int* part_counts, float* part_scores, float* part_lse2, int* counts, float* score_sum,
-                         float* lse2_sum, cudaStream_t stream);
-// router_topk_bwd plus the balance gradient of g [T / seq_len, E] fp32, row t / seq_len for token t: softmax
-// dlogits[t, e] += s_e (g_e - s.g) + z_coef lse_t s_e; sigmoid dlogits[t, e] += sigma_e (1 - sigma_e) (g_e - s.g) / sum_j sigma_j
-void router_topk_seq_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                         bool renorm, bool sigmoid, float scale, const float* g, float z_coef, long long seq_len,
-                         void* dlogits, cudaStream_t stream);
+                     bool renorm, bool sigmoid, float scale, const float* g, long long num_seqs, float z_coef,
+                     void* dlogits, cudaStream_t stream);
 
 // ------------------------------------------------------------------ expert-parallel exchange over NVLink ----
 // peer_base: device array [world] of symmetric-arena base pointers; off_* are byte offsets of regions inside the arena.

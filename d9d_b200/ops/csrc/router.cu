@@ -2,17 +2,15 @@
 // selection bias, + optional DeepSeek-V3 group-limited selection, + optional renormalisation and scaling of the selected
 // scores) in one pass, one warp per token; and its backward.
 // Replaces softmax / topk (radix select + sort) / gather / div / sum launches of the eager path.
-// The options are template parameters: the plain softmax instantiations (<VPL, false, false, false, false, false> forward,
-// <VPL, false, false, false, false> backward) compile to the same instructions as before the options existed.
-// AUX (softmax only) adds the router's auxiliary losses: the forward also produces the per-expert selection counts,
-// sum_t s[t, e] and sum_t lse_t^2 (per-warp registers -> per-block partials in a fixed order -> router_aux_finalize_kernel,
-// no atomics, so two passes over the same logits agree bit for bit); the backward adds the load-balancing and z-loss
-// gradients to dlogits before its bf16 rounding.
-// SEQ (with AUX, softmax or sigmoid) keeps the statistics per sequence of seq_len consecutive tokens for the
-// sequence-wise balance loss: each block owns a contiguous range of at most `chunk` tokens inside one sequence, so its
-// partials belong to that sequence, and router_aux_finalize_kernel<true> sums each sequence's partials in the same fixed
-// order.  Sigmoid scores enter the statistics normalised over the experts (s = sigma / sum_j sigma_j), softmax ones as they
-// are (and with lse^2 per sequence); the backward reads the balance gradient row g[t / seq_len].
+// The options are template parameters: the plain softmax instantiations (<VPL, false, false, false, false> forward,
+// <VPL, false, false, false> backward) compile to the same instructions as before the options existed.
+// STATS adds the statistics of the router's auxiliary losses, per sequence of seq_len consecutive tokens (the batch
+// losses use one sequence of all T tokens): the per-expert selection counts, sum_t s[t, e] and sum_t lse_t^2.  Each block
+// owns a contiguous range of at most `chunk` tokens inside one sequence and writes its partials (per-warp registers ->
+// per-block partials in a fixed order), and router_aux_finalize_kernel sums each sequence's partials in a fixed order: no
+// atomics, so two passes over the same logits agree bit for bit.  Sigmoid scores enter the statistics normalised over the
+// experts (s = sigma / sum_j sigma_j), softmax ones as they are (and with lse^2).
+// BALANCE adds the balance and z-loss gradients to dlogits before its bf16 rounding, from the gradient row g[t / seq_len].
 #include <stdexcept>
 
 #include "common.cuh"
@@ -114,44 +112,42 @@ __device__ __forceinline__ void mask_dropped_groups(float (&key)[VPL], float* __
 
 // The new option instantiations declare a minimum of one block per SM: without it ptxas caps some of them at 64 registers
 // and spills.  A minimum of 0 is the plain __launch_bounds__(256) of the softmax path.
-// AUX: block b writes part_counts[b, E], part_scores[b, E] and part_lse2[b] (sums over the block's tokens).
-// SEQ: block b covers tokens [q S + c chunk, q S + min(S, (c + 1) chunk)) of sequence q = b / seq_parts, c = b % seq_parts
-// (S = seq_len), a warp every ROUTER_WARPS tokens; the grid has (T / S) seq_parts blocks.
-template <int VPL, bool SIGMOID, bool GROUPED, bool SCALED, bool AUX, bool SEQ>
-__global__ void __launch_bounds__(256, (GROUPED || AUX) ? 1 : 0)
+// STATS: block b covers tokens [q S + c chunk, q S + min(S, (c + 1) chunk)) of sequence q = b / seq_parts,
+// c = b % seq_parts (S = seq_len), a warp every ROUTER_WARPS tokens; the grid has (T / S) seq_parts blocks.  It writes
+// part_counts[b, E], part_scores[b, E] and part_lse2[b] (sums over its tokens).
+template <int VPL, bool SIGMOID, bool GROUPED, bool SCALED, bool STATS>
+__global__ void __launch_bounds__(256, (GROUPED || STATS) ? 1 : 0)
     router_fwd_kernel(const __nv_bfloat16* __restrict__ logits, const float* __restrict__ bias, long long T, int E, int k,
                       bool renorm, long long* __restrict__ idx_out, float* __restrict__ probs_out, int G,
                       int topk_groups, float scale, int* __restrict__ part_counts, float* __restrict__ part_scores,
                       float* __restrict__ part_lse2, long long seq_len, int chunk, int seq_parts) {
-  static_assert(!(AUX && SIGMOID && !SEQ), "the batch auxiliary losses are defined for softmax routers only");
-  static_assert(!SEQ || AUX, "per-sequence statistics use the AUX accumulators");
   const int lane = threadIdx.x & 31;
   long long t_begin = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5, t_end = T;
   long long t_step = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  if constexpr (SEQ) {
+  if constexpr (STATS) {
     const long long first = static_cast<long long>(blockIdx.x / seq_parts) * seq_len;
     const long long c = static_cast<long long>(blockIdx.x % seq_parts) * chunk;
     t_begin = first + c + (threadIdx.x >> 5);
     t_end = first + min(seq_len, c + chunk);
     t_step = ROUTER_WARPS;
   }
-  float acc_s[VPL], acc_lse2 = 0.f;  // AUX: lane-owned sum_t s[t, e] and (warp-uniform) sum_t lse_t^2
-  int acc_c[VPL];                    // AUX: lane-owned selection counts
-  if constexpr (AUX) {
+  float acc_s[VPL], acc_lse2 = 0.f;  // STATS: lane-owned sum_t s[t, e] and (warp-uniform) sum_t lse_t^2
+  int acc_c[VPL];                    // STATS: lane-owned selection counts
+  if constexpr (STATS) {
 #pragma unroll
     for (int i = 0; i < VPL; ++i) { acc_s[i] = 0.f; acc_c[i] = 0; }
   }
   for (long long t = t_begin; t < t_end; t += t_step) {
     float p[VPL], key[VPL], mx, sum;
     load_row_scores<VPL, SIGMOID>(logits + t * E, E, lane, p, mx, sum);
-    if constexpr (AUX && SIGMOID) {  // normalised affinities; padding lanes hold sigma(0) and are left out
+    if constexpr (STATS && SIGMOID) {  // normalised affinities; padding lanes hold sigma(0) and are left out
       float ssum = 0.f;
 #pragma unroll
       for (int i = 0; i < VPL; ++i) ssum += (lane + i * 32 < E) ? p[i] : 0.f;
       const float inv = 1.f / warp_sum(ssum);
 #pragma unroll
       for (int i = 0; i < VPL; ++i) acc_s[i] += p[i] * inv;
-    } else if constexpr (AUX) {
+    } else if constexpr (STATS) {
 #pragma unroll
       for (int i = 0; i < VPL; ++i) acc_s[i] += p[i];  // padding lanes hold 0
       const float lse = mx + __logf(sum);
@@ -169,7 +165,7 @@ __global__ void __launch_bounds__(256, (GROUPED || AUX) ? 1 : 0)
     float sel_p = 0.f;   // lane j keeps the j-th selection
     int sel_e = 0;
     float total = 0.f;
-    unsigned picked = 0u;  // AUX: bit i set when this lane's expert lane + 32 i was selected
+    unsigned picked = 0u;  // STATS: bit i set when this lane's expert lane + 32 i was selected
     for (int j = 0; j < k; ++j) {
       // arg-max over the warp; ties go to the lower expert index
       float best = -INFINITY;
@@ -189,7 +185,7 @@ __global__ void __launch_bounds__(256, (GROUPED || AUX) ? 1 : 0)
       }
       if ((best_e & 31) == lane) {  // owner retires the winner
         key[best_e >> 5] = -INFINITY;
-        if constexpr (AUX) picked |= 1u << (best_e >> 5);
+        if constexpr (STATS) picked |= 1u << (best_e >> 5);
       }
       if (lane == j) { sel_p = best_p; sel_e = best_e; }
       total += best_p;
@@ -200,12 +196,12 @@ __global__ void __launch_bounds__(256, (GROUPED || AUX) ? 1 : 0)
       if constexpr (SCALED) w *= scale;
       probs_out[t * k + lane] = w;
     }
-    if constexpr (AUX) {
+    if constexpr (STATS) {
 #pragma unroll
       for (int i = 0; i < VPL; ++i) acc_c[i] += (picked >> i) & 1u;
     }
   }
-  if constexpr (AUX) {
+  if constexpr (STATS) {
     // block reduction in warp order: s_*[e] = ((w0 + w1) + w2) + ...
     __shared__ float s_scores[32 * VPL];
     __shared__ int s_counts[32 * VPL];
@@ -238,7 +234,7 @@ __global__ void __launch_bounds__(256, (GROUPED || AUX) ? 1 : 0)
   }
 }
 
-// Sums the forward's [parts, E] partials in a fixed order.  Blocks of 32 x 32 threads: block b < ceil(E / 32) owns
+// Sums one sequence's [parts, E] partials in a fixed order.  Blocks of 32 x 32 threads: block b < ceil(E / 32) owns
 // experts 32 b + x, thread row y sums parts y, y + 32, ... and row 0 then adds the 32 row sums in order; the last block
 // sums part_lse2 the same way.  With no parts (T = 0) it writes zeros.
 __device__ __forceinline__ void router_aux_finalize(const int* __restrict__ part_counts, const float* __restrict__ part_scores,
@@ -283,51 +279,40 @@ __device__ __forceinline__ void router_aux_finalize(const int* __restrict__ part
   }
 }
 
-// SEQ: the partials are [seqs, parts, E] / [seqs, parts] and the outputs [seqs, E] / [seqs]; blockIdx.y strides over the
-// sequences, each summed exactly like the single sequence of the batch statistics.
-template <bool SEQ>
+// The partials are [seqs, parts, E] / [seqs, parts] and the outputs [seqs, E] / [seqs]; blockIdx.y strides over the
+// sequences.
 __global__ void __launch_bounds__(1024)
     router_aux_finalize_kernel(const int* __restrict__ part_counts, const float* __restrict__ part_scores,
                                const float* __restrict__ part_lse2, int parts, int E, int* __restrict__ counts,
                                float* __restrict__ score_sum, float* __restrict__ lse2_sum, long long seqs) {
-  if constexpr (SEQ) {
-    for (long long q = blockIdx.y; q < seqs; q += gridDim.y) {
-      const long long off = q * parts;
-      router_aux_finalize(part_counts + off * E, part_scores + off * E, part_lse2 + off, parts, E, counts + q * E,
-                          score_sum + q * E, lse2_sum + q);
-      __syncthreads();  // the next sequence reuses the shared row sums
-    }
-  } else {
-    router_aux_finalize(part_counts, part_scores, part_lse2, parts, E, counts, score_sum, lse2_sum);
+  for (long long q = blockIdx.y; q < seqs; q += gridDim.y) {
+    const long long off = q * parts;
+    router_aux_finalize(part_counts + off * E, part_scores + off * E, part_lse2 + off, parts, E, counts + q * E,
+                        score_sum + q * E, lse2_sum + q);
+    __syncthreads();  // the next sequence reuses the shared row sums
   }
 }
 
 // r_j = scale * s_j (/ (S + eps) when renorm).  With dr' = scale * dr: ds_j = (dr'_j - sum_i dr'_i r_i) / (S + eps) when
 // renorm, else dr'_j; dp = scatter(ds).  softmax: dlogits[e] = p_e * (dp_e - sum_j ds_j s_j); sigmoid: s_e (1 - s_e) dp_e.
-// AUX (softmax): dlogits[e] += p_e * (g_e - sum_j p_j g_j) + z_coef * lse * p_e, folded in as dp_e += g_e and
-// inner += sum_j p_j g_j - z_coef * lse (g: load-balancing gradient per expert, z_coef = 2 w_tok coef_z).
-// SEQ: g is [T / seq_len, E] and token t uses row t / seq_len.  Sigmoid (s_e = p_e / sum_j p_j, the balance scores):
+// BALANCE: g is [T / seq_len, E] (balance gradient per sequence and expert) and token t uses row t / seq_len.  Softmax:
+// dlogits[e] += p_e * (g_e - sum_j p_j g_j) + z_coef * lse * p_e (z_coef = 2 w_tok coef_z), folded in as dp_e += g_e and
+// inner += sum_j p_j g_j - z_coef * lse.  Sigmoid (s_e = p_e / sum_j p_j, the balance scores):
 // dlogits[e] += p_e (1 - p_e) (g_e - sum_j s_j g_j) / sum_j p_j, folded in as dp_e += (g_e - s.g) / sum_j p_j.
-template <int VPL, bool SIGMOID, bool SCALED, bool AUX, bool SEQ>
-__global__ void __launch_bounds__(256, (SIGMOID || SCALED || AUX) ? 1 : 0)
+template <int VPL, bool SIGMOID, bool SCALED, bool BALANCE>
+__global__ void __launch_bounds__(256, (SIGMOID || SCALED || BALANCE) ? 1 : 0)
     router_bwd_kernel(const __nv_bfloat16* __restrict__ logits, const long long* __restrict__ idx,
                       const float* __restrict__ dprobs, long long T, int E, int k, bool renorm,
                       __nv_bfloat16* __restrict__ dlogits, float scale, const float* __restrict__ g, float z_coef,
                       long long seq_len) {
-  static_assert(!(AUX && SIGMOID && !SEQ), "the batch auxiliary losses are defined for softmax routers only");
-  static_assert(!SEQ || AUX, "the sequence-wise gradient uses the AUX terms");
   const int lane = threadIdx.x & 31;
   const long long warp = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  float gv[VPL];  // AUX: this lane's g_e, loaded once (SEQ: per token, from its sequence's row)
-  if constexpr (AUX && !SEQ) {
-#pragma unroll
-    for (int i = 0; i < VPL; ++i) gv[i] = (lane + i * 32 < E) ? g[lane + i * 32] : 0.f;
-  }
+  float gv[VPL];  // BALANCE: this lane's g_e, per token from its sequence's row
   for (long long t = warp; t < T; t += warps) {
     float p[VPL], mx, sum;
     load_row_scores<VPL, SIGMOID>(logits + t * E, E, lane, p, mx, sum);
-    if constexpr (SEQ) {
+    if constexpr (BALANCE) {
       const float* __restrict__ row = g + (t / seq_len) * E;
 #pragma unroll
       for (int i = 0; i < VPL; ++i) gv[i] = (lane + i * 32 < E) ? row[lane + i * 32] : 0.f;
@@ -355,7 +340,7 @@ __global__ void __launch_bounds__(256, (SIGMOID || SCALED || AUX) ? 1 : 0)
       my_ds = (lane < k) ? (my_dr - dot) / S : 0.f;
     }
     float inner = 0.f;
-    if constexpr (AUX && !SIGMOID) {
+    if constexpr (BALANCE && !SIGMOID) {
       float pg = 0.f;
 #pragma unroll
       for (int i = 0; i < VPL; ++i) pg += p[i] * gv[i];
@@ -364,7 +349,7 @@ __global__ void __launch_bounds__(256, (SIGMOID || SCALED || AUX) ? 1 : 0)
       inner = warp_sum(my_ds * my_s);
     }
     float dp[VPL];
-    if constexpr (AUX && SIGMOID) {
+    if constexpr (BALANCE && SIGMOID) {
       float psum = 0.f, pg = 0.f;
 #pragma unroll
       for (int i = 0; i < VPL; ++i) {
@@ -378,7 +363,7 @@ __global__ void __launch_bounds__(256, (SIGMOID || SCALED || AUX) ? 1 : 0)
     } else {
 #pragma unroll
       for (int i = 0; i < VPL; ++i) {
-        if constexpr (AUX) dp[i] = gv[i];
+        if constexpr (BALANCE) dp[i] = gv[i];
         else dp[i] = 0.f;
       }
     }
@@ -415,60 +400,55 @@ inline int grid_for(long long T) {
   return static_cast<int>(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
 }
 
-// SEQ: tokens per block, a multiple of ROUTER_WARPS giving each warp the token count of the grid-stride walk over
-// grid_for(T) blocks, so long sequences get about as many blocks as the batch kernels
+// STATS: tokens per block, a multiple of ROUTER_WARPS giving each warp the token count of a grid-stride walk over
+// grid_for(T) blocks, so long sequences get about as many blocks as the plain kernels
 inline int seq_chunk(long long T) {
   const long long warps = static_cast<long long>(grid_for(T)) * ROUTER_WARPS;
   return static_cast<int>((T + warps - 1) / warps) * ROUTER_WARPS;
 }
 
-// aux: with part_* sized [grid_for(T), E] / [grid_for(T)] (softmax only), or, with seq_len > 0, per-sequence statistics
-// (softmax or sigmoid) with part_* sized [T / seq_len * seq_parts, E] / [T / seq_len * seq_parts]
+// stats: per-sequence statistics with part_* sized [num_seqs * seq_parts, E] / [num_seqs * seq_parts]
 template <int VPL>
 void launch_fwd(const __nv_bfloat16* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
-                int G, int topk_groups, float scale, long long* idx, float* probs, bool aux, int* part_counts,
-                float* part_scores, float* part_lse2, cudaStream_t stream, long long seq_len = 0, int chunk = 0,
-                int seq_parts = 1) {
-  const bool grouped = G > 1, scaled = scale != 1.f, seq = seq_len > 0;
+                int G, int topk_groups, float scale, long long* idx, float* probs, bool stats, int* part_counts,
+                float* part_scores, float* part_lse2, cudaStream_t stream, long long seq_len, int chunk,
+                int seq_parts) {
+  const bool grouped = G > 1, scaled = scale != 1.f;
   const size_t smem = grouped ? sizeof(float) * ROUTER_WARPS * E : 0;  // <= 32 KiB for E <= 1024
-#define D9D_ROUTER_FWD(SIG, GRP, SCL, AUX, SEQ)                                                                        \
-  if (sigmoid == SIG && grouped == GRP && scaled == SCL && aux == AUX && seq == SEQ) {                                 \
-    const int grid = SEQ ? static_cast<int>(T / seq_len) * seq_parts : grid_for(T);                                   \
-    router_fwd_kernel<VPL, SIG, GRP, SCL, AUX, SEQ><<<grid, 256, smem, stream>>>(                                      \
+#define D9D_ROUTER_FWD(SIG, GRP, SCL, STATS)                                                                          \
+  if (sigmoid == SIG && grouped == GRP && scaled == SCL && stats == STATS) {                                         \
+    const int grid = STATS ? static_cast<int>(T / seq_len) * seq_parts : grid_for(T);                                 \
+    router_fwd_kernel<VPL, SIG, GRP, SCL, STATS><<<grid, 256, smem, stream>>>(                                       \
         logits, bias, T, E, k, renorm, idx, probs, G, topk_groups, scale, part_counts, part_scores, part_lse2, seq_len, \
         chunk, seq_parts);                                                                                             \
     return;                                                                                                            \
   }
-  D9D_ROUTER_FWD(false, false, false, false, false) D9D_ROUTER_FWD(false, false, true, false, false)
-  D9D_ROUTER_FWD(false, true, false, false, false) D9D_ROUTER_FWD(false, true, true, false, false)
-  D9D_ROUTER_FWD(true, false, false, false, false) D9D_ROUTER_FWD(true, false, true, false, false)
-  D9D_ROUTER_FWD(true, true, false, false, false) D9D_ROUTER_FWD(true, true, true, false, false)
-  D9D_ROUTER_FWD(false, false, false, true, false) D9D_ROUTER_FWD(false, false, true, true, false)
-  D9D_ROUTER_FWD(false, true, false, true, false) D9D_ROUTER_FWD(false, true, true, true, false)
-  D9D_ROUTER_FWD(false, false, false, true, true) D9D_ROUTER_FWD(false, false, true, true, true)
-  D9D_ROUTER_FWD(false, true, false, true, true) D9D_ROUTER_FWD(false, true, true, true, true)
-  D9D_ROUTER_FWD(true, false, false, true, true) D9D_ROUTER_FWD(true, false, true, true, true)
-  D9D_ROUTER_FWD(true, true, false, true, true) D9D_ROUTER_FWD(true, true, true, true, true)
+  D9D_ROUTER_FWD(false, false, false, false) D9D_ROUTER_FWD(false, false, true, false)
+  D9D_ROUTER_FWD(false, true, false, false) D9D_ROUTER_FWD(false, true, true, false)
+  D9D_ROUTER_FWD(true, false, false, false) D9D_ROUTER_FWD(true, false, true, false)
+  D9D_ROUTER_FWD(true, true, false, false) D9D_ROUTER_FWD(true, true, true, false)
+  D9D_ROUTER_FWD(false, false, false, true) D9D_ROUTER_FWD(false, false, true, true)
+  D9D_ROUTER_FWD(false, true, false, true) D9D_ROUTER_FWD(false, true, true, true)
+  D9D_ROUTER_FWD(true, false, false, true) D9D_ROUTER_FWD(true, false, true, true)
+  D9D_ROUTER_FWD(true, true, false, true) D9D_ROUTER_FWD(true, true, true, true)
 #undef D9D_ROUTER_FWD
 }
 
 template <int VPL>
 void launch_bwd(const __nv_bfloat16* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
                 bool renorm, bool sigmoid, float scale, __nv_bfloat16* dlogits, const float* g, float z_coef,
-                cudaStream_t stream, long long seq_len = 0) {
-  const bool scaled = scale != 1.f, aux = g != nullptr, seq = seq_len > 0;
-#define D9D_ROUTER_BWD(SIG, SCL, AUX, SEQ)                                                                           \
-  if (sigmoid == SIG && scaled == SCL && aux == AUX && seq == SEQ) {                                                 \
-    router_bwd_kernel<VPL, SIG, SCL, AUX, SEQ><<<grid_for(T), 256, 0, stream>>>(logits, idx, dprobs, T, E, k,       \
-                                                                                renorm, dlogits, scale, g, z_coef,  \
-                                                                                seq_len);                           \
-    return;                                                                                                          \
+                cudaStream_t stream, long long seq_len) {
+  const bool scaled = scale != 1.f, balance = g != nullptr;
+#define D9D_ROUTER_BWD(SIG, SCL, BAL)                                                                             \
+  if (sigmoid == SIG && scaled == SCL && balance == BAL) {                                                        \
+    router_bwd_kernel<VPL, SIG, SCL, BAL><<<grid_for(T), 256, 0, stream>>>(logits, idx, dprobs, T, E, k, renorm, \
+                                                                           dlogits, scale, g, z_coef, seq_len);   \
+    return;                                                                                                       \
   }
-  D9D_ROUTER_BWD(false, false, false, false) D9D_ROUTER_BWD(false, true, false, false)
-  D9D_ROUTER_BWD(true, false, false, false) D9D_ROUTER_BWD(true, true, false, false)
-  D9D_ROUTER_BWD(false, false, true, false) D9D_ROUTER_BWD(false, true, true, false)
-  D9D_ROUTER_BWD(false, false, true, true) D9D_ROUTER_BWD(false, true, true, true)
-  D9D_ROUTER_BWD(true, false, true, true) D9D_ROUTER_BWD(true, true, true, true)
+  D9D_ROUTER_BWD(false, false, false) D9D_ROUTER_BWD(false, true, false)
+  D9D_ROUTER_BWD(true, false, false) D9D_ROUTER_BWD(true, true, false)
+  D9D_ROUTER_BWD(false, false, true) D9D_ROUTER_BWD(false, true, true)
+  D9D_ROUTER_BWD(true, false, true) D9D_ROUTER_BWD(true, true, true)
 #undef D9D_ROUTER_BWD
 }
 
@@ -493,83 +473,46 @@ static void check_router_groups(int E, int num_groups, int topk_groups) {
     throw std::runtime_error("d9d router: 1 <= num_groups <= 32 dividing E and 1 <= topk_groups <= num_groups required");
 }
 
+static void check_num_seqs(long long T, long long num_seqs) {
+  if (num_seqs < 1 || T % num_seqs != 0)
+    throw std::runtime_error("d9d router: the sequence count must be a positive divisor of the token count");
+}
+
+int router_stat_parts(long long T, long long num_seqs) {
+  if (num_seqs == 0) return 0;
+  check_num_seqs(T, num_seqs);
+  if (T == 0) return 0;
+  const long long chunk = seq_chunk(T), seq_len = T / num_seqs;
+  return static_cast<int>(num_seqs * ((seq_len + chunk - 1) / chunk));
+}
+
 void router_topk_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
-                     int num_groups, int topk_groups, float scale, long long* idx, float* probs, cudaStream_t stream) {
-  if (T == 0) return;
+                     int num_groups, int topk_groups, float scale, long long* idx, float* probs, long long num_seqs,
+                     int* part_counts, float* part_scores, float* part_lse2, int* counts, float* score_sum,
+                     float* lse2_sum, cudaStream_t stream) {
+  if (T == 0 && num_seqs == 0) return;
   check_router_shape(E, k);
   check_router_groups(E, num_groups, topk_groups);
-  D9D_ROUTER_DISPATCH(launch_fwd, static_cast<const __nv_bfloat16*>(logits), bias, T, E, k, renorm, sigmoid,
-                      num_groups, topk_groups, scale, idx, probs, false, nullptr, nullptr, nullptr, stream);
+  const int parts = router_stat_parts(T, num_seqs);
+  const int seq_parts = num_seqs ? static_cast<int>(parts / num_seqs) : 1;
+  if (T > 0)
+    D9D_ROUTER_DISPATCH(launch_fwd, static_cast<const __nv_bfloat16*>(logits), bias, T, E, k, renorm, sigmoid,
+                        num_groups, topk_groups, scale, idx, probs, num_seqs > 0, part_counts, part_scores, part_lse2,
+                        stream, num_seqs ? T / num_seqs : 0, num_seqs ? seq_chunk(T) : 0, seq_parts);
+  if (num_seqs > 0)
+    router_aux_finalize_kernel<<<dim3((E + 31) / 32 + 1, static_cast<unsigned>(num_seqs < 65535 ? num_seqs : 65535)),
+                                 dim3(32, 32), 0, stream>>>(part_counts, part_scores, part_lse2, seq_parts, E, counts,
+                                                            score_sum, lse2_sum, num_seqs);
 }
 
 void router_topk_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                     bool renorm, bool sigmoid, float scale, void* dlogits, cudaStream_t stream) {
+                     bool renorm, bool sigmoid, float scale, const float* g, long long num_seqs, float z_coef,
+                     void* dlogits, cudaStream_t stream) {
   if (T == 0) return;
   check_router_shape(E, k);
+  if (g) check_num_seqs(T, num_seqs);
   D9D_ROUTER_DISPATCH(launch_bwd, static_cast<const __nv_bfloat16*>(logits), idx, dprobs, T, E, k, renorm, sigmoid,
-                      scale, static_cast<__nv_bfloat16*>(dlogits), nullptr, 0.f, stream);
-}
-
-int router_aux_parts(long long T) { return T > 0 ? grid_for(T) : 0; }
-
-void router_topk_aux_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, int num_groups,
-                         int topk_groups, float scale, long long* idx, float* probs, int* part_counts,
-                         float* part_scores, float* part_lse2, int* counts, float* score_sum, float* lse2_sum,
-                         cudaStream_t stream) {
-  check_router_shape(E, k);
-  check_router_groups(E, num_groups, topk_groups);
-  if (T > 0)
-    D9D_ROUTER_DISPATCH(launch_fwd, static_cast<const __nv_bfloat16*>(logits), bias, T, E, k, renorm, false,
-                        num_groups, topk_groups, scale, idx, probs, true, part_counts, part_scores, part_lse2, stream);
-  router_aux_finalize_kernel<false><<<(E + 31) / 32 + 1, dim3(32, 32), 0, stream>>>(
-      part_counts, part_scores, part_lse2, router_aux_parts(T), E, counts, score_sum, lse2_sum, 1);
-}
-
-void router_topk_aux_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                         bool renorm, float scale, const float* g, float z_coef, void* dlogits, cudaStream_t stream) {
-  if (T == 0) return;
-  check_router_shape(E, k);
-  D9D_ROUTER_DISPATCH(launch_bwd, static_cast<const __nv_bfloat16*>(logits), idx, dprobs, T, E, k, renorm, false,
-                      scale, static_cast<__nv_bfloat16*>(dlogits), g, z_coef, stream);
-}
-
-static void check_seq_len(long long T, long long seq_len) {
-  if (seq_len < 1 || T % seq_len != 0)
-    throw std::runtime_error("d9d router: the sequence length must be a positive divisor of the token count");
-}
-
-int router_seq_parts(long long T, long long seq_len) {
-  check_seq_len(T, seq_len);
-  if (T == 0) return 0;
-  const long long chunk = seq_chunk(T);
-  return static_cast<int>((seq_len + chunk - 1) / chunk);
-}
-
-void router_topk_seq_fwd(const void* logits, const float* bias, long long T, int E, int k, bool renorm, bool sigmoid,
-                         int num_groups, int topk_groups, float scale, long long seq_len, long long* idx, float* probs,
-                         int* part_counts, float* part_scores, float* part_lse2, int* counts, float* score_sum,
-                         float* lse2_sum, cudaStream_t stream) {
-  check_router_shape(E, k);
-  check_router_groups(E, num_groups, topk_groups);
-  const int parts = router_seq_parts(T, seq_len);
-  if (T == 0) return;
-  D9D_ROUTER_DISPATCH(launch_fwd, static_cast<const __nv_bfloat16*>(logits), bias, T, E, k, renorm, sigmoid,
-                      num_groups, topk_groups, scale, idx, probs, true, part_counts, part_scores, part_lse2, stream,
-                      seq_len, seq_chunk(T), parts);
-  const long long seqs = T / seq_len;
-  router_aux_finalize_kernel<true><<<dim3((E + 31) / 32 + 1, static_cast<unsigned>(seqs < 65535 ? seqs : 65535)),
-                                     dim3(32, 32), 0, stream>>>(part_counts, part_scores, part_lse2, parts, E, counts,
-                                                                score_sum, lse2_sum, seqs);
-}
-
-void router_topk_seq_bwd(const void* logits, const long long* idx, const float* dprobs, long long T, int E, int k,
-                         bool renorm, bool sigmoid, float scale, const float* g, float z_coef, long long seq_len,
-                         void* dlogits, cudaStream_t stream) {
-  check_seq_len(T, seq_len);
-  if (T == 0) return;
-  check_router_shape(E, k);
-  D9D_ROUTER_DISPATCH(launch_bwd, static_cast<const __nv_bfloat16*>(logits), idx, dprobs, T, E, k, renorm, sigmoid,
-                      scale, static_cast<__nv_bfloat16*>(dlogits), g, z_coef, stream, seq_len);
+                      scale, static_cast<__nv_bfloat16*>(dlogits), g, z_coef, stream, g ? T / num_seqs : 0);
 }
 
 }  // namespace d9d
