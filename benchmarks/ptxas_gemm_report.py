@@ -1,4 +1,4 @@
-"""Register, stack and spill report of every bf16 wgmma GEMM instance, or of the flash attention kernels (no GPU needed).
+"""Register, stack and spill report of every bf16 and fp8 wgmma GEMM instance, or of the flash attention kernels (no GPU needed).
 
 Compiles the GEMM translation units (or ``flash_attn.cu`` with ``--units attention``) for sm_90a with ``-Xptxas -v`` (the
 flags of ``d9d_b200/ops/build.py``) and prints one row per kernel instance: registers, stack frame, spill stores / loads,
@@ -27,17 +27,24 @@ sys.path.insert(0, str(ROOT))
 
 from d9d_b200.ops import build as ops_build  # noqa: E402
 
-UNITS = ["gemm_dense.cu", "gemm_dense_pair.cu", "gemm_grouped.cu", "gemm_ce.cu", "gemm_comm_fwd.cu", "gemm_comm_wgrad.cu"]
+UNITS = ["gemm_dense.cu", "gemm_dense_pair.cu", "gemm_grouped.cu", "gemm_ce.cu", "gemm_comm_fwd.cu", "gemm_comm_wgrad.cu",
+         "gemm_fp8.cu"]
 MODES = {0: "DENSE", 1: "GROUPED_M", 2: "GROUPED_K"}
 EPIS = {0: "BF16", 1: "F32", 2: "F32_ACC", 3: "BF16_ACC", 4: "CE_LSE", 5: "CE_DLOGITS", 6: "CE_LSE_SUM",
         7: "CE_DLOGITS_REG"}
 COMMS = {0: "-", 1: "AG_A", 2: "RS_D", 3: "AG_KA", 4: "AG_KB", 5: "WAIT_A"}
 _GEMM = re.compile(r"gemm_kernelILi(\d+)ELi(\d+)ELb([01])ELb([01])ELi(\d+)ELi(\d+)ELi(\d+)EE")
+_FP8 = re.compile(r"gemm_fp8_kernelILi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)EE")
+SCALINGS = {0: "ROWCOL", 1: "MX"}
 _ATTN_FWD = re.compile(r"flash_attn_fwd_kernelILi(\d+)ELi(\d+)EE")
 _ATTN_BWD = re.compile(r"flash_attn_bwd_kernelILi(\d+)ELi(\d+)ELb([01])EE")
 
 
 def _name(mangled: str) -> str | None:
+    m = _FP8.search(mangled)
+    if m is not None:
+        bn, scaling, mode, epi = (int(x) for x in m.groups())
+        return f"fp8 {MODES[mode]:<9} BN {bn:<3} {SCALINGS[scaling]:<6} {EPIS[epi]}"
     m = _GEMM.search(mangled)
     if m is None:
         return None

@@ -11,6 +11,8 @@ _KERNELS_PER_OP = {
     "ce_forward_ex": 3,
     "ce_forward_reg": 3,
     "flash_attn_bwd": 3,  # delta pre-pass + dK/dV kernel + dQ kernel
+    "quantize_colwise_t_batched": 2,  # column amax + transposing quantiser
+    "quantize_segments_t": 2,
 }
 
 

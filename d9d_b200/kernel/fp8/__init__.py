@@ -44,6 +44,25 @@ def quantize_colwise_t_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.T
     return q, scale
 
 
+def quantize_colwise_t_batched_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [E, R, C]`` -> ``(qT [E, C, R], scale [E, C])``: the transposing quantiser applied to every ``x[e]``."""
+    parts = [quantize_colwise_t_reference(xe) for xe in x]
+    return torch.stack([q for q, _ in parts]), torch.stack([s for _, s in parts])
+
+
+def quantize_segments_t_reference(x: torch.Tensor, starts, counts) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [R, C]`` with expert ``e`` on rows ``[starts[e], starts[e] + counts[e])`` -> ``(qT [C, R], scale [E, C])``: one
+    scale per (expert, column) over the expert's rows (1 for an expert without rows or with all-zero values); every row of
+    ``x`` outside the experts' ranges comes out as zero in ``qT``."""
+    starts, counts = [int(v) for v in starts], [int(v) for v in counts]
+    qt = torch.zeros(x.shape[1], x.shape[0], dtype=FP8, device=x.device)
+    scale = torch.ones(len(counts), x.shape[1], dtype=torch.float32, device=x.device)
+    for e, (s0, n) in enumerate(zip(starts, counts)):
+        if n > 0:
+            qt[:, s0 : s0 + n], scale[e] = quantize_colwise_t_reference(x[s0 : s0 + n])
+    return qt, scale
+
+
 def mx_scale_exponent(amax: torch.Tensor) -> torch.Tensor:
     """Smallest integer ``e`` with ``amax / 2**e <= 448`` (``-127`` for all-zero groups), clamped to [-126, 126]."""
     # 448 = 1.75 * 2**8: with amax = m * 2**x (1 <= m < 2) the answer is x - 8 (+1 if m > 1.75) - exact, no logarithms
@@ -232,6 +251,7 @@ def convert_linears_to_fp8(module: nn.Module, predicate=lambda name, m: True, re
 
 __all__ = [
     "Fp8Linear", "Fp8LinearFunction", "MxFp8LinearFunction", "convert_linears_to_fp8", "dequantize_mx", "fp8_linear", "mx_mm", "mx_scale_exponent",
-    "quantize_colwise_t", "quantize_colwise_t_reference", "quantize_mx_reference", "quantize_rowwise", "quantize_rowwise_reference",
+    "quantize_colwise_t", "quantize_colwise_t_batched_reference", "quantize_colwise_t_reference", "quantize_mx_reference",
+    "quantize_segments_t_reference", "quantize_rowwise", "quantize_rowwise_reference",
     "scaled_mm", "unpack_mx_scales",
 ]

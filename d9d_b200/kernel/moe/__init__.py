@@ -9,15 +9,17 @@ Compatibility surface (``compat.py``): ``fused_indices_to_multihot``, ``moe_perm
 """
 
 from .compat import fused_indices_to_multihot, moe_permute_with_probs, moe_unpermute_mask
-from .experts import grouped_swiglu
+from .experts import fp8_grouped_linear_reference, grouped_swiglu, grouped_swiglu_fp8_reference
 from .layout import MoELayout, build_moe_layout, grouped_linear, moe_permute, moe_unpermute
 
 __all__ = [
     "MoELayout",
     "build_moe_layout",
+    "fp8_grouped_linear_reference",
     "fused_indices_to_multihot",
     "grouped_linear",
     "grouped_swiglu",
+    "grouped_swiglu_fp8_reference",
     "moe_permute",
     "moe_permute_with_probs",
     "moe_unpermute",

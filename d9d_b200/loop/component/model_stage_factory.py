@@ -77,6 +77,7 @@ class ModelStageFactory:
         if not isinstance(model, nn.Module) or not isinstance(model, ModuleLateInit):
             raise ValueError("Model stage is required to be nn.Module instance implementing ModuleLateInit protocol")
         self._apply_fp8(model)
+        self._apply_fp8_experts(model)
         if self._ctx.mesh_params.is_distributed:
             self._provider.parallelize_model_stage(ParallelizeModelStageContext(model=model, stage=stage, dist_context=self._ctx))
         model.to_empty(device=self._ctx.current_device)
@@ -102,6 +103,18 @@ class ModelStageFactory:
         n = convert_linears_to_fp8(model, lambda name, _m: bool(include.search(name)) and not (exclude and exclude.search(name)),
                                    recipe=cfg.recipe)
         self._ctx.logger.info(f"fp8: {n} linear layers of this stage run in e4m3")
+
+    def _apply_fp8_experts(self, model: nn.Module) -> None:
+        if not self._config_model.fp8_experts:
+            return
+        if self._ctx.mesh_params.tensor_parallel > 1:
+            raise NotImplementedError("model_stage_factory.fp8_experts is not combined with tensor parallelism")
+        from d9d_b200.module.block.moe import GroupedSwiGLU
+
+        blocks = [m for m in model.modules() if isinstance(m, GroupedSwiGLU)]
+        for block in blocks:
+            block.enable_fp8()  # refuses LoRA-wrapped projections and sizes that are not multiples of 16
+        self._ctx.logger.info(f"fp8: {len(blocks)} expert blocks of this stage run in e4m3")
 
     def build_pipeline_and_modules(self) -> tuple[PipelineScheduleInfo, TrackedModules]:
         if self._config_model.checkpoint_only_trainable_parameters:

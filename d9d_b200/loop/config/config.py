@@ -46,7 +46,8 @@ class Fp8LinearConfig(BaseModel):
     weight-gradient GEMMs - ``d9d_b200.kernel.fp8.Fp8Linear``).  Net-new: the reference has no fp8 path.
 
     ``include`` / ``exclude`` are regular expressions searched in the module names of a model stage; only plain linear
-    layers whose feature sizes are multiples of 16 are converted (LoRA wrappers, grouped expert weights, norms are not)."""
+    layers whose feature sizes are multiples of 16 are converted (LoRA wrappers, grouped expert weights, norms are not;
+    ``ModelStageFactoryConfig.fp8_experts`` runs the expert blocks in fp8)."""
 
     include: str = r".*"
     exclude: str | None = r"lm_head|cls_head|embedding_head|router|\.gate$"
@@ -57,6 +58,9 @@ class ModelStageFactoryConfig(BaseModel):
     source_checkpoint: Path | None
     checkpoint_only_trainable_parameters: bool
     fp8_linear: Fp8LinearConfig | None = None
+    # run every MoE expert block (GroupedSwiGLU) of the stage in fp8: e4m3 grouped GEMMs with per-expert row / column
+    # scales for the forward, input gradient and weight gradient; the weights stay bf16 masters
+    fp8_experts: bool = False
 
 
 class GradientClippingConfig(BaseModel):

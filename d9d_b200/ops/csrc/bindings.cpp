@@ -299,6 +299,48 @@ std::tuple<Tensor, Tensor> quantize_rowwise(const Tensor& x) {
   return {q, scale};
 }
 
+// x[E,R,C] bf16 (R a multiple of 16) -> (qt[E,C,R] e4m3, scale[E,C] fp32) with x[e,r,c] ~= qt[e,c,r] * scale[e,c]
+std::tuple<Tensor, Tensor> quantize_colwise_t_batched(const Tensor& x) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 3 && x.is_contiguous() && x.scalar_type() == at::kBFloat16,
+              "quantize_colwise_t_batched: contiguous 3-D bf16 CUDA tensor required");
+  TORCH_CHECK(x.size(1) % 16 == 0, "quantize_colwise_t_batched: R must be a multiple of 16 (16-byte rows of the transposed copy)");
+  TORCH_CHECK(x.size(0) < (int64_t(1) << 16) && x.size(2) < (int64_t(1) << 31), "quantize_colwise_t_batched: too many planes / columns");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t E = x.size(0), R = x.size(1), C = x.size(2);
+  Tensor qt = at::empty({E, C, R}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor scale = at::empty({E, C}, x.options().dtype(at::kFloat));
+  Tensor amax = at::empty({E, C}, x.options().dtype(at::kFloat));
+  d9d::quantize_colwise_t_e4m3(x.data_ptr(), qt.data_ptr(), scale.data_ptr<float>(), amax.data_ptr<float>(), R, static_cast<int>(C),
+                               C, R, cur_stream(), static_cast<int>(E));
+  return {qt, scale};
+}
+
+// x[cap,C] bf16 in the MoE layout (cap a multiple of 128) -> (qt[C,cap] e4m3, scale[E,C] fp32): expert e's rows
+// [seg_offsets[e], seg_offsets[e] + counts[e]) with one scale per (e, c) over them; all other rows of qt are zero
+std::tuple<Tensor, Tensor> quantize_segments_t(const Tensor& x, const Tensor& tile_group, const Tensor& seg_offsets,
+                                               const Tensor& counts) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.stride(1) == 1 && x.scalar_type() == at::kBFloat16,
+              "quantize_segments_t: 2-D bf16 CUDA tensor with unit column stride required");
+  CHECK_CUDA_CONTIG(tile_group); CHECK_CUDA_CONTIG(seg_offsets); CHECK_CUDA_CONTIG(counts);
+  TORCH_CHECK(tile_group.scalar_type() == at::kInt && seg_offsets.scalar_type() == at::kInt && counts.scalar_type() == at::kInt,
+              "quantize_segments_t: tile_group, seg_offsets and counts must be int32");
+  TORCH_CHECK(tile_group.device() == x.device() && seg_offsets.device() == x.device() && counts.device() == x.device(),
+              "quantize_segments_t: operands must be on one device");
+  TORCH_CHECK(x.size(0) % 128 == 0 && tile_group.numel() == x.size(0) / 128,
+              "quantize_segments_t: rows must be a multiple of 128 with one tile_group entry per 128 rows");
+  TORCH_CHECK(counts.numel() > 0 && seg_offsets.numel() == counts.numel() + 1, "quantize_segments_t: seg_offsets must be [E + 1], counts [E]");
+  TORCH_CHECK(x.size(0) < (int64_t(1) << 31) && x.size(1) < (int64_t(1) << 31), "quantize_segments_t: too large");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t R = x.size(0), C = x.size(1), E = counts.numel();
+  Tensor qt = at::empty({C, R}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor scale = at::empty({E, C}, x.options().dtype(at::kFloat));
+  Tensor amax = at::empty({E, C}, x.options().dtype(at::kFloat));
+  d9d::quantize_segments_t_e4m3(x.data_ptr(), qt.data_ptr(), scale.data_ptr<float>(), amax.data_ptr<float>(), tile_group.data_ptr<int>(),
+                                seg_offsets.data_ptr<int>(), counts.data_ptr<int>(), static_cast<int>(E), R, static_cast<int>(C),
+                                x.stride(0), R, cur_stream());
+  return {qt, scale};
+}
+
 // x[R,C] bf16 -> (qt[C,R] e4m3 (row pitch padded to 16 bytes), scale[C] fp32) with x[r,c] ~= qt[c,r] * scale[c]
 std::tuple<Tensor, Tensor> quantize_colwise_t(const Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.stride(1) == 1 && x.scalar_type() == at::kBFloat16, "quantize_colwise_t: 2-D bf16 CUDA tensor required");
@@ -369,6 +411,77 @@ void gemm_mxfp8(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tenso
   TORCH_CHECK(sfb.scalar_type() == at::kByte && sfb.numel() >= (static_cast<int64_t>(g.N) + 255) / 256 * 2 * kb * 512, "gemm_mxfp8: sfb too small");
   g.block_scaled = true;
   g.sfa = sfa.data_ptr<uint8_t>(); g.sfb = sfb.data_ptr<uint8_t>();
+  d9d::gemm_fp8(g, cur_stream());
+}
+
+// Operand checks of the grouped fp8 GEMMs, before anything touches the device: e4m3 K-major operands with 16-byte rows,
+// fp32 scales of the stated lengths, int32 tables, one device
+void check_fp8_grouped(const char* op, const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, const Tensor& d,
+                       const Tensor& table) {
+  for (const Tensor* t : {&a, &sa, &b, &sb, &d, &table}) {
+    TORCH_CHECK(t->is_cuda() && t->device() == a.device(), op, ": all operands must be CUDA tensors on one device");
+    TORCH_CHECK(t->is_contiguous(), op, ": operands must be contiguous");
+  }
+  CHECK_ALIGNED16(a); CHECK_ALIGNED16(b); CHECK_ALIGNED16(d);
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn, op, ": a and b must be float8_e4m3fn");
+  TORCH_CHECK(sa.scalar_type() == at::kFloat && sb.scalar_type() == at::kFloat, op, ": scales must be fp32");
+  TORCH_CHECK(table.scalar_type() == at::kInt, op, ": the expert table must be int32");
+  TORCH_CHECK(a.dim() == 2 && a.size(1) % 16 == 0 && a.size(1) > 0, op, ": a must be 2-D with rows of a positive multiple of 16 bytes");
+  TORCH_CHECK(a.size(0) < (int64_t(1) << 31) && a.size(1) < (int64_t(1) << 31), op, ": a is too large");
+}
+
+// d[R,N] (+)= (a[R,K] · b[e(r)]^T) * sa[r] * sb[e(r), n]: the MoE forward / input gradient in fp8.  a: the expert-sorted
+// rows (R a multiple of 128), b: [E, N, K], tile_group: [R/128] expert of every 128-row tile (-1: never written)
+void gemm_fp8_grouped_m(const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, Tensor d, const Tensor& tile_group,
+                        bool accumulate) {
+  check_fp8_grouped("gemm_fp8_grouped_m", a, sa, b, sb, d, tile_group);
+  TORCH_CHECK(b.dim() == 3 && b.size(2) == a.size(1), "gemm_fp8_grouped_m: b must be [E, N, K] with the K of a");
+  TORCH_CHECK(b.size(0) > 0 && b.size(1) > 0 && b.size(1) < (int64_t(1) << 31), "gemm_fp8_grouped_m: b must have experts and N > 0");
+  TORCH_CHECK(a.size(0) % 128 == 0 && tile_group.numel() == a.size(0) / 128,
+              "gemm_fp8_grouped_m: rows must be a multiple of 128 with one tile_group entry per 128 rows");
+  TORCH_CHECK(sa.numel() == a.size(0), "gemm_fp8_grouped_m: sa must be [R]");
+  TORCH_CHECK(sb.numel() == b.size(0) * b.size(1), "gemm_fp8_grouped_m: sb must be [E * N]");
+  TORCH_CHECK(d.dim() == 2 && d.size(0) == a.size(0) && d.size(1) == b.size(1) && d.scalar_type() == at::kBFloat16,
+              "gemm_fp8_grouped_m: d must be bf16 [R, N]");
+  TORCH_CHECK(d.size(1) % 8 == 0, "gemm_fp8_grouped_m: N must be a multiple of 8 (16-byte output rows)");
+  c10::cuda::CUDAGuard guard(a.device());
+  d9d::Fp8GemmArgs g;
+  g.mode = 1; g.epi = accumulate ? 3 : 0;
+  g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1)); g.N = static_cast<int>(b.size(1));
+  g.num_groups = static_cast<int>(b.size(0));
+  g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
+  g.lda = a.stride(0); g.ldb = b.stride(1); g.b_group_stride = b.stride(0); g.ldd = d.stride(0);
+  g.scale_a = sa.data_ptr<float>(); g.scale_b = sb.data_ptr<float>();
+  g.tile_group = tile_group.data_ptr<int>();
+  d9d::gemm_fp8(g, cur_stream());
+}
+
+// d[e] (+)= (a[:, rows_e] · b[:, rows_e]^T) * sa[e, m] * sb[e, n] over expert e's rows group_offsets[e] .. [e+1]: the MoE
+// weight gradient in fp8.  a: [M, R], b: [N, R] (the transposed, per-expert quantised activations / output gradients),
+// d: [E, M, N] fp32 or bf16 (an expert without rows: zeros when storing, untouched when accumulating)
+void gemm_fp8_grouped_k(const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, Tensor d, const Tensor& group_offsets,
+                        bool accumulate) {
+  check_fp8_grouped("gemm_fp8_grouped_k", a, sa, b, sb, d, group_offsets);
+  TORCH_CHECK(b.dim() == 2 && b.size(1) == a.size(1) && b.size(0) > 0 && b.size(0) < (int64_t(1) << 31),
+              "gemm_fp8_grouped_k: b must be [N, R] with the R of a");
+  TORCH_CHECK(a.size(1) % 128 == 0, "gemm_fp8_grouped_k: R must be a multiple of 128 (the expert segments' alignment)");
+  TORCH_CHECK(d.dim() == 3 && d.size(0) > 0 && d.size(1) == a.size(0) && d.size(2) == b.size(0),
+              "gemm_fp8_grouped_k: d must be [E, M, N]");
+  TORCH_CHECK(d.scalar_type() == at::kFloat || d.scalar_type() == at::kBFloat16, "gemm_fp8_grouped_k: d must be fp32 or bf16");
+  TORCH_CHECK(d.size(2) * d.element_size() % 16 == 0, "gemm_fp8_grouped_k: rows of d must be a multiple of 16 bytes");
+  TORCH_CHECK(group_offsets.numel() == d.size(0) + 1, "gemm_fp8_grouped_k: group_offsets must be [E + 1]");
+  TORCH_CHECK(sa.numel() == d.size(0) * d.size(1), "gemm_fp8_grouped_k: sa must be [E * M]");
+  TORCH_CHECK(sb.numel() == d.size(0) * d.size(2), "gemm_fp8_grouped_k: sb must be [E * N]");
+  c10::cuda::CUDAGuard guard(a.device());
+  d9d::Fp8GemmArgs g;
+  g.mode = 2; g.epi = epi_for(d, accumulate);
+  g.M = static_cast<int>(a.size(0)); g.N = static_cast<int>(b.size(0)); g.K = 0;
+  g.k_total = a.size(1);
+  g.num_groups = static_cast<int>(d.size(0));
+  g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
+  g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(1); g.d_group_stride = d.stride(0);
+  g.scale_a = sa.data_ptr<float>(); g.scale_b = sb.data_ptr<float>();
+  g.group_offsets = group_offsets.data_ptr<int>();
   d9d::gemm_fp8(g, cur_stream());
 }
 
@@ -1032,6 +1145,10 @@ TORCH_LIBRARY(d9d_b200, m) {
   m.def("quantize_mx(Tensor x) -> (Tensor, Tensor)");
   m.def("gemm_fp8(Tensor a, Tensor b, Tensor? scale_a, Tensor? scale_b, float scalar, Tensor(a!) d) -> ()");
   m.def("gemm_mxfp8(Tensor a, Tensor sfa, Tensor b, Tensor sfb, Tensor(a!) d) -> ()");
+  m.def("quantize_colwise_t_batched(Tensor x) -> (Tensor, Tensor)");
+  m.def("quantize_segments_t(Tensor x, Tensor tile_group, Tensor seg_offsets, Tensor counts) -> (Tensor, Tensor)");
+  m.def("gemm_fp8_grouped_m(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d, Tensor tile_group, bool accumulate=False) -> ()");
+  m.def("gemm_fp8_grouped_k(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d, Tensor group_offsets, bool accumulate) -> ()");
   m.def("rms_norm_fwd(Tensor x, Tensor w, float eps, bool zero_centered) -> (Tensor, Tensor)");
   m.def("rms_norm_bwd(Tensor dout, Tensor x, Tensor w, Tensor inv_rms, bool zero_centered) -> (Tensor, Tensor)");
   m.def("silu_mul_fwd(Tensor x, Tensor y) -> Tensor");
@@ -1089,6 +1206,10 @@ TORCH_LIBRARY_IMPL(d9d_b200, CUDA, m) {
   m.impl("quantize_mx", &quantize_mx);
   m.impl("gemm_fp8", &gemm_fp8);
   m.impl("gemm_mxfp8", &gemm_mxfp8);
+  m.impl("quantize_colwise_t_batched", &quantize_colwise_t_batched);
+  m.impl("quantize_segments_t", &quantize_segments_t);
+  m.impl("gemm_fp8_grouped_m", &gemm_fp8_grouped_m);
+  m.impl("gemm_fp8_grouped_k", &gemm_fp8_grouped_k);
   m.impl("rms_norm_fwd", &rms_norm_fwd);
   m.impl("rms_norm_bwd", &rms_norm_bwd);
   m.impl("silu_mul_fwd", &silu_mul_fwd);

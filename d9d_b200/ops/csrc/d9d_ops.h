@@ -75,23 +75,37 @@ void ce_finalize_zsum(const float* part_max, const float* part_sum, const float*
 
 // ------------------------------------------------------------------ fp8 GEMM (wgmma e4m3, MX block scales) -----
 struct Fp8GemmArgs {
-  const void* A = nullptr;   // [M, K] e4m3, K contiguous (row pitch lda bytes)
-  const void* B = nullptr;   // [N, K] e4m3
-  void* D = nullptr;         // [M, N] bf16
+  int mode = 0;              // gemm::Mode: DENSE, GROUPED_M (MoE forward / dgrad), GROUPED_K (MoE wgrad)
+  int epi = 0;               // gemm::Epi: bf16 store (dense); GROUPED_M: + bf16 accumulate; GROUPED_K: fp32 / bf16 store / accumulate
+  const void* A = nullptr;   // [M, K] e4m3, K contiguous (row pitch lda bytes); GROUPED_K: [M, k_total]
+  const void* B = nullptr;   // [N, K] e4m3; GROUPED_M: [E, N, K] (expert pitch b_group_stride bytes); GROUPED_K: [N, k_total]
+  void* D = nullptr;         // [M, N] bf16; GROUPED_K: [E, M, N] (expert pitch d_group_stride elements)
   long long lda = 0, ldb = 0, ldd = 0;
+  long long b_group_stride = 0, d_group_stride = 0;
   int M = 0, N = 0, K = 0;
+  int num_groups = 1;
+  long long k_total = 0;               // GROUPED_K: rows of the grouped reduction dim
+  const int* tile_group = nullptr;     // GROUPED_M: [M/128] expert per m-tile or -1
+  const int* group_offsets = nullptr;  // GROUPED_K: [E+1] row offsets, multiples of 128
   bool block_scaled = false;          // true: MXFP8 (UE8M0 scale per 32 K-elements), false: row / column scales in the epilogue
-  const float* scale_a = nullptr;     // [M] or nullptr
-  const float* scale_b = nullptr;     // [N] or nullptr
+  const float* scale_a = nullptr;     // [M] or nullptr; GROUPED_K: [E, M]
+  const float* scale_b = nullptr;     // [N] or nullptr; grouped: [E, N]
   float scale_scalar = 1.f;
   const uint8_t* sfa = nullptr;       // [ceil(M/128), K/128, 512]
   const uint8_t* sfb = nullptr;       // [2*ceil(N/256), K/128, 512]
 };
 void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream);
 void quantize_rowwise_e4m3(const void* x, void* q, float* scale, long long M, int K, long long ldx, cudaStream_t stream);
-// qt[C, R] (row pitch ldq bytes) = e4m3(x[R, C]^T / scale[c]); amax_scratch: [C] fp32
+// qt[e, C, R] (row pitch ldq bytes, planes C * ldq apart) = e4m3(x[e, R, C]^T / scale[e, c]) for E planes of x
+// (R * ldx elements apart); amax_scratch: [E, C] fp32
 void quantize_colwise_t_e4m3(const void* x, void* qt, float* scale, float* amax_scratch, long long R, int C, long long ldx,
-                             long long ldq, cudaStream_t stream);
+                             long long ldq, cudaStream_t stream, int E = 1);
+// x[R, C] with R a multiple of 128 (the MoE layout's capacity) -> qt[C, R] (row pitch ldq bytes), scale[E, C]:
+// expert e's rows [seg_offsets[e], seg_offsets[e] + counts[e]) are quantised with one scale per (e, c) over them (1 when
+// they are all zero or there are none); every other row of qt is zero.  No host synchronisation.
+void quantize_segments_t_e4m3(const void* x, void* qt, float* scale, float* amax_scratch, const int* tile_group,
+                              const int* seg_offsets, const int* counts, int E, long long R, int C, long long ldx, long long ldq,
+                              cudaStream_t stream);
 // sf must be zero-initialised by the caller when M is not a multiple of 256 (pad blocks)
 void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long long ldx, cudaStream_t stream);
 

@@ -1,8 +1,11 @@
 // fp8 (e4m3) GEMM launchers + the quantisation kernels that produce their operands.
 //   quantize_rowwise     x[M,K] bf16 -> q[M,K] e4m3, scale[M]            (scale = amax / 448 per row)
-//   quantize_colwise_t   x[R,C] bf16 -> qT[C,R] e4m3, scale[C]           (transposed copy, scale per column of x)
+//   quantize_colwise_t   x[E,R,C] bf16 -> qT[E,C,R] e4m3, scale[E,C]   (transposed copy, scale per column of every x[e])
+//   quantize_segments_t  x[cap,C] bf16 -> qT[C,cap] e4m3, scale[E,C]   (transposed copy, scale per column of every expert's
+//                                                                      rows; pad rows come out as zeros)
 //   quantize_mx          x[M,K] bf16 -> q[M,K] e4m3, UE8M0 scale blocks  (one scale per 32 K-elements, 128-row x 4-group blocks)
-//   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on wgmma e4m3 (MX: per-32-K scales applied in registers)
+//   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on wgmma e4m3 (MX: per-32-K scales applied in registers), and the
+//                          grouped expert GEMMs (GROUPED_M / GROUPED_K, see gemm_fp8_sm90.cuh)
 #include <cuda_fp8.h>
 
 #include "gemm_fp8_sm90.cuh"
@@ -57,37 +60,86 @@ __global__ void quant_rowwise_kernel(const __nv_bfloat16* __restrict__ x, uint8_
 }
 
 // ---- column-wise + transpose -----------------------------------------------------------------------------------
+// Which rows of x form one scale group ("plane") and where they go in qT:
+//   batched  (tile_group == nullptr): plane e = blockIdx.z is x + e * x_plane [R, C] -> qt + e * q_plane [C, R]
+//   segments (tile_group != nullptr): one x [R = cap, C] -> qt [C, cap]; row r belongs to expert g = tile_group[r / 128]
+//            and is quantised with expert g's scales when r < seg_offsets[g] + counts[g]; every other row is written as
+//            a zero (and never read).  Scale groups start on 128-row boundaries, so a 64- or 128-row tile has one expert.
+struct ColTPlanes {
+  long long x_plane, q_plane;
+  const int* tile_group;
+  const int* seg_offsets;
+  const int* counts;
+  int num_planes;  // E: planes of amax / scale ([E, C])
+};
+
+// expert of the 128-row-aligned tile starting at row r0 and the end of its valid rows (-1 / r0: no valid rows)
+__device__ __forceinline__ int segment_of(const ColTPlanes& pl, long long r0, long long& valid_end) {
+  const int g = pl.tile_group[r0 / 128];
+  valid_end = g >= 0 ? static_cast<long long>(pl.seg_offsets[g]) + pl.counts[g] : r0;
+  return g;
+}
+
 // pass 1: amax per column (non-negative floats order like their bit patterns: atomicMax on the int view)
 __global__ void col_amax_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ amax, long long R, int C, long long ldx,
-                                int rows_per_block) {
+                                int rows_per_block, ColTPlanes pl) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const long long r0 = static_cast<long long>(blockIdx.y) * rows_per_block;
-  const long long r1 = min(R, r0 + rows_per_block);
+  long long r1 = min(R, r0 + rows_per_block);
+  int g = blockIdx.z;
+  if (pl.tile_group != nullptr) {
+    long long valid_end;
+    g = segment_of(pl, r0, valid_end);
+    if (g < 0) return;
+    r1 = min(r1, valid_end);
+  } else {
+    x += g * pl.x_plane;
+  }
   float m = 0.f;
   for (long long r = r0; r < r1; ++r) m = fmaxf(m, fabsf(__bfloat162float(x[r * ldx + c])));
-  atomicMax(reinterpret_cast<int*>(amax) + c, __float_as_int(m));
+  atomicMax(reinterpret_cast<int*>(amax) + static_cast<long long>(g) * C + c, __float_as_int(m));
 }
 
-// pass 2: 64 x 64 tile through shared memory; amax[c] is turned into the scale in place by the blocks of the first tile row
+// pass 2: 64 x 64 tile through shared memory; amax is turned into the scales by the blocks of the first tile row
 __global__ void quant_colwise_t_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ amax, uint8_t* __restrict__ qt,
-                                       float* __restrict__ scale, long long R, int C, long long ldx, long long ldq) {
+                                       float* __restrict__ scale, long long R, int C, long long ldx, long long ldq, ColTPlanes pl) {
   __shared__ uint8_t tile[64][64 + 4];
   const int c0 = blockIdx.x * 64;
   const long long r0 = static_cast<long long>(blockIdx.y) * 64;
   const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;  // 256 threads: 64 columns x 4 row phases
   const int c = c0 + tx;
+  const bool segments = pl.tile_group != nullptr;
+  int g = blockIdx.z;
+  long long r_end = R;
+  if (segments) {
+    g = -1;
+    r_end = r0;
+    if (r0 < R) g = segment_of(pl, r0, r_end);
+  } else {
+    x += g * pl.x_plane;
+    qt += g * pl.q_plane;
+  }
+  auto put_scale = [&](int e) {
+    const float a = amax[static_cast<long long>(e) * C + c];
+    scale[static_cast<long long>(e) * C + c] = a > 0.f ? a / E4M3_MAX : 1.f;
+  };
+  if (blockIdx.y == 0 && c < C) {
+    if (segments) {
+      for (int e = ty; e < pl.num_planes; e += 4) put_scale(e);  // every expert's, also of those without rows
+    } else if (ty == 0) {
+      put_scale(g);
+    }
+  }
   float inv = 0.f;
-  if (c < C) {
-    const float a = amax[c];
-    const float s = a > 0.f ? a / E4M3_MAX : 1.f;
-    inv = 1.f / s;
-    if (blockIdx.y == 0 && ty == 0) scale[c] = s;
+  if (c < C && g >= 0) {
+    const float a = amax[static_cast<long long>(g) * C + c];
+    inv = 1.f / (a > 0.f ? a / E4M3_MAX : 1.f);
   }
   for (int i = ty; i < 64; i += 4) {
     const long long r = r0 + i;
     float v = 0.f;
-    if (r < R && c < C) v = __bfloat162float(x[r * ldx + c]) * inv;
+    if (r < r_end && c < C) v = __bfloat162float(x[r * ldx + c]) * inv;
     tile[tx][i] = static_cast<uint8_t>(__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3));
   }
   __syncthreads();
@@ -132,40 +184,50 @@ __global__ void quant_mx_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __
   sf[blk * 512 + (r % 32) * 16 + (r / 32) * 4 + (g % 4)] = static_cast<uint8_t>(e + 127);
 }
 
-CUtensorMap make_tmap_u8_2d(const void* base, uint64_t d0, uint64_t d1, uint64_t stride1_bytes, uint32_t box0, uint32_t box1) {
+// 2-D map, or 3-D ([d2, d1, d0], box depth 1) when d2 > 0
+CUtensorMap make_tmap_u8(const void* base, uint64_t d0, uint64_t d1, uint64_t stride1_bytes, uint32_t box0, uint32_t box1,
+                         uint64_t d2 = 0, uint64_t stride2_bytes = 0) {
   CUtensorMap m;
-  cuuint64_t dims[2] = {d0, d1};
-  cuuint64_t strides[1] = {stride1_bytes};
-  cuuint32_t box[2] = {box0, box1};
-  cuuint32_t estr[2] = {1, 1};
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (strides[0] & 15) != 0)
+  const cuuint32_t rank = d2 > 0 ? 3 : 2;
+  cuuint64_t dims[3] = {d0, d1, d2};
+  cuuint64_t strides[2] = {stride1_bytes, stride2_bytes};
+  cuuint32_t box[3] = {box0, box1, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (strides[0] & 15) != 0 || (rank == 3 && (strides[1] & 15) != 0))
     throw std::runtime_error("d9d gemm_fp8: operand base / row pitch must be 16-byte aligned for TMA");
-  CUresult r = gemm::get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr,
+  CUresult r = gemm::get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, rank, const_cast<void*>(base), dims, strides, box, estr,
                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("d9d gemm_fp8: cuTensorMapEncodeTiled failed: " + std::to_string(r));
   return m;
 }
 
-template <int BLOCK_N, int SCALING>
+template <int BLOCK_N, int SCALING, int MODE = gemm::DENSE, int EPI = gemm::EPI_BF16>
 void launch_fp8(const Fp8GemmArgs& a, cudaStream_t stream) {
   using C = fp8::Cfg<BLOCK_N, SCALING>;
-  auto kern = fp8::gemm_fp8_kernel<BLOCK_N, SCALING>;
+  auto kern = fp8::gemm_fp8_kernel<BLOCK_N, SCALING, MODE, EPI>;
   static bool configured = false;
   if (!configured) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     configured = true;
   }
-  CUtensorMap ta = make_tmap_u8_2d(a.A, a.K, a.M, a.lda, fp8::BLOCK_K, fp8::BLOCK_M);
-  CUtensorMap tb = make_tmap_u8_2d(a.B, a.K, a.N, a.ldb, fp8::BLOCK_K, BLOCK_N);
+  // GROUPED_K: A [M, k_total] and B [N, k_total], the reduction over the grouped rows; GROUPED_M: B [E, N, K]
+  const uint64_t k_dim = MODE == gemm::GROUPED_K ? static_cast<uint64_t>(a.k_total) : static_cast<uint64_t>(a.K);
+  CUtensorMap ta = make_tmap_u8(a.A, k_dim, a.M, a.lda, fp8::BLOCK_K, fp8::BLOCK_M);
+  CUtensorMap tb = MODE == gemm::GROUPED_M ? make_tmap_u8(a.B, a.K, a.N, a.ldb, fp8::BLOCK_K, BLOCK_N, a.num_groups, a.b_group_stride)
+                                           : make_tmap_u8(a.B, k_dim, a.N, a.ldb, fp8::BLOCK_K, BLOCK_N);
   CUtensorMap td;
-  if (!gemm::make_tmap_out(&td, a.D, true, a.N, a.M, 1, a.ldd, 0))
-    throw std::runtime_error("d9d gemm_fp8: output must be 16-byte aligned with a row pitch that is a multiple of 8 elements");
+  constexpr bool out_bf16 = (EPI == gemm::EPI_BF16 || EPI == gemm::EPI_BF16_ACC);
+  const uint64_t groups = MODE == gemm::GROUPED_K ? a.num_groups : 1;
+  if (!gemm::make_tmap_out(&td, a.D, out_bf16, a.N, a.M, groups, a.ldd, a.d_group_stride))
+    throw std::runtime_error("d9d gemm_fp8: output must be 16-byte aligned with 16-byte row (and expert) pitches");
   fp8::Params p{};
   p.M = a.M; p.N = a.N; p.K = a.K;
   p.scale_a = a.scale_a; p.scale_b = a.scale_b; p.scale_scalar = a.scale_scalar;
   p.sfa = a.sfa; p.sfb = a.sfb;
-  const long long tiles = static_cast<long long>((a.M + fp8::BLOCK_M - 1) / fp8::BLOCK_M) * ((a.N + BLOCK_N - 1) / BLOCK_N);
+  p.num_groups = a.num_groups; p.tile_group = a.tile_group; p.group_offsets = a.group_offsets;
+  const long long tiles = static_cast<long long>((a.M + fp8::BLOCK_M - 1) / fp8::BLOCK_M) * ((a.N + BLOCK_N - 1) / BLOCK_N) *
+                          (MODE == gemm::GROUPED_K ? a.num_groups : 1);
   if (tiles <= 0) return;
   const int grid = static_cast<int>(tiles < gemm::sm_count() ? tiles : gemm::sm_count());
   kern<<<grid, fp8::NUM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, td, p);
@@ -182,15 +244,33 @@ void quantize_rowwise_e4m3(const void* x, void* q, float* scale, long long M, in
 }
 
 void quantize_colwise_t_e4m3(const void* x, void* qt, float* scale, float* amax_scratch, long long R, int C, long long ldx,
-                             long long ldq, cudaStream_t stream) {
-  if (R <= 0 || C <= 0) return;
-  cudaMemsetAsync(amax_scratch, 0, sizeof(float) * C, stream);
+                             long long ldq, cudaStream_t stream, int E) {
+  if (R <= 0 || C <= 0 || E <= 0) return;
+  cudaMemsetAsync(amax_scratch, 0, sizeof(float) * C * E, stream);
+  const ColTPlanes pl{R * ldx, C * ldq, nullptr, nullptr, nullptr, E};
   const int rows_per_block = 256;
-  dim3 g1((C + 127) / 128, static_cast<unsigned>((R + rows_per_block - 1) / rows_per_block));
-  col_amax_kernel<<<g1, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), amax_scratch, R, C, ldx, rows_per_block);
-  dim3 g2((C + 63) / 64, static_cast<unsigned>((R + 63) / 64));
+  dim3 g1((C + 127) / 128, static_cast<unsigned>((R + rows_per_block - 1) / rows_per_block), E);
+  col_amax_kernel<<<g1, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), amax_scratch, R, C, ldx, rows_per_block, pl);
+  dim3 g2((C + 63) / 64, static_cast<unsigned>((R + 63) / 64), E);
   quant_colwise_t_kernel<<<g2, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), amax_scratch, static_cast<uint8_t*>(qt),
-                                                 scale, R, C, ldx, ldq);
+                                                 scale, R, C, ldx, ldq, pl);
+}
+
+void quantize_segments_t_e4m3(const void* x, void* qt, float* scale, float* amax_scratch, const int* tile_group,
+                              const int* seg_offsets, const int* counts, int E, long long R, int C, long long ldx, long long ldq,
+                              cudaStream_t stream) {
+  if (C <= 0 || E <= 0) return;
+  cudaMemsetAsync(amax_scratch, 0, sizeof(float) * C * E, stream);
+  const ColTPlanes pl{0, 0, tile_group, seg_offsets, counts, E};
+  // R (the capacity) is a multiple of 128: one expert per 128-row block of pass 1; pass 2 writes the scales of all E
+  // experts from its first tile row, so it runs even when R is 0
+  if (R > 0) {
+    dim3 g1((C + 127) / 128, static_cast<unsigned>(R / 128));
+    col_amax_kernel<<<g1, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), amax_scratch, R, C, ldx, 128, pl);
+  }
+  dim3 g2((C + 63) / 64, static_cast<unsigned>(R > 0 ? R / 64 : 1));
+  quant_colwise_t_kernel<<<g2, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), amax_scratch, static_cast<uint8_t*>(qt),
+                                                 scale, R, C, ldx, ldq, pl);
 }
 
 void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long long ldx, cudaStream_t stream) {
@@ -207,6 +287,18 @@ void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream) {
     if (a.K % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr)
       throw std::runtime_error("d9d gemm_mxfp8: K must be a multiple of 128 and both scale-factor tensors are required");
     launch_fp8<128, fp8::MX>(a, stream);
+  } else if (a.mode == gemm::GROUPED_M) {
+    if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_M, gemm::EPI_BF16>(a, stream);
+    else if (a.epi == gemm::EPI_BF16_ACC) launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_M, gemm::EPI_BF16_ACC>(a, stream);
+    else throw std::runtime_error("d9d gemm_fp8: GROUPED_M supports bf16 store / accumulate only");
+  } else if (a.mode == gemm::GROUPED_K) {
+    switch (a.epi) {
+      case gemm::EPI_BF16: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_BF16>(a, stream); break;
+      case gemm::EPI_F32: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_F32>(a, stream); break;
+      case gemm::EPI_F32_ACC: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_F32_ACC>(a, stream); break;
+      case gemm::EPI_BF16_ACC: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_BF16_ACC>(a, stream); break;
+      default: throw std::runtime_error("d9d gemm_fp8: GROUPED_K supports fp32 / bf16 store / accumulate only");
+    }
   } else {
     // 128-wide tiles only: a 256-wide fp32 accumulator (128 registers per consumer thread) spills at the kernel's
     // 168-register budget

@@ -150,22 +150,25 @@ struct TileCoord {
   bool valid;
 };
 
-template <int MODE, int BLOCK_N, int TILE_M = BLOCK_M>
-__device__ __forceinline__ int num_tiles(const Params& p) {
+// The tile walk is shared with the fp8 kernel (gemm_fp8_sm90.cuh): BK is the depth of a k-block in elements, and the
+// parameter block P needs M, N, K, num_groups, tile_group and group_offsets; the DENSE-only fields (k_splits,
+// comm_m_rot) are read in DENSE instances only.
+template <int MODE, int BLOCK_N, int TILE_M = BLOCK_M, typename P = Params>
+__device__ __forceinline__ int num_tiles(const P& p) {
   const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int m_tiles = (p.M + TILE_M - 1) / TILE_M;
-  if (MODE == GROUPED_K) return p.num_groups * m_tiles * n_tiles;
-  if (MODE == DENSE) return m_tiles * n_tiles * p.k_splits;
+  if constexpr (MODE == GROUPED_K) return p.num_groups * m_tiles * n_tiles;
+  if constexpr (MODE == DENSE) return m_tiles * n_tiles * p.k_splits;
   return m_tiles * n_tiles;
 }
 
-template <int MODE, int BLOCK_N, int TILE_M = BLOCK_M>
-__device__ __forceinline__ TileCoord get_tile(const Params& p, int tile) {
+template <int MODE, int BLOCK_N, int TILE_M = BLOCK_M, int BK = BLOCK_K, typename P = Params>
+__device__ __forceinline__ TileCoord get_tile(const P& p, int tile) {
   TileCoord t;
   const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int m_tiles = (p.M + TILE_M - 1) / TILE_M;
   t.valid = true;
-  if (MODE == GROUPED_K) {
+  if constexpr (MODE == GROUPED_K) {
     const int per_group = m_tiles * n_tiles;
     t.group = tile / per_group;
     const int r = tile - t.group * per_group;
@@ -173,13 +176,15 @@ __device__ __forceinline__ TileCoord get_tile(const Params& p, int tile) {
     t.n_blk = r - t.m_blk * n_tiles;
     const int k0 = p.group_offsets[t.group], k1 = p.group_offsets[t.group + 1];
     t.k_begin = k0;
-    t.k_blocks = (k1 - k0 + BLOCK_K - 1) / BLOCK_K;
+    t.k_blocks = (k1 - k0 + BK - 1) / BK;
     return t;
   }
   int k_split = 0;
-  if (MODE == DENSE && p.k_splits > 1) {  // tile = split * (m_tiles * n_tiles) + mn: one K-slice per wave
-    k_split = tile / (m_tiles * n_tiles);
-    tile -= k_split * (m_tiles * n_tiles);
+  if constexpr (MODE == DENSE) {
+    if (p.k_splits > 1) {  // tile = split * (m_tiles * n_tiles) + mn: one K-slice per wave
+      k_split = tile / (m_tiles * n_tiles);
+      tile -= k_split * (m_tiles * n_tiles);
+    }
   }
   // L2-friendly rasterisation: walk GROUP_M m-blocks for each n-block before moving on.
   constexpr int GROUP_M = 8;
@@ -190,18 +195,22 @@ __device__ __forceinline__ TileCoord get_tile(const Params& p, int tile) {
   const int r = tile - gid * group_span;
   t.m_blk = first_m + (r % gm);
   t.n_blk = r / gm;
-  if (MODE == DENSE && p.comm_m_rot != 0) t.m_blk = (t.m_blk + p.comm_m_rot) % m_tiles;
+  if constexpr (MODE == DENSE) {
+    if (p.comm_m_rot != 0) t.m_blk = (t.m_blk + p.comm_m_rot) % m_tiles;
+  }
   t.k_begin = 0;
-  t.k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-  if (MODE == DENSE && p.k_splits > 1) {
-    const int per_split = (t.k_blocks + p.k_splits - 1) / p.k_splits;
-    const int first = k_split * per_split;
-    t.k_begin = first * BLOCK_K;
-    t.k_blocks = max(0, min(per_split, t.k_blocks - first));
-    t.valid = t.k_blocks > 0;  // an empty slice has nothing to add
+  t.k_blocks = (p.K + BK - 1) / BK;
+  if constexpr (MODE == DENSE) {
+    if (p.k_splits > 1) {
+      const int per_split = (t.k_blocks + p.k_splits - 1) / p.k_splits;
+      const int first = k_split * per_split;
+      t.k_begin = first * BK;
+      t.k_blocks = max(0, min(per_split, t.k_blocks - first));
+      t.valid = t.k_blocks > 0;  // an empty slice has nothing to add
+    }
   }
   t.group = 0;
-  if (MODE == GROUPED_M) {
+  if constexpr (MODE == GROUPED_M) {
     t.group = p.tile_group[t.m_blk];
     t.valid = t.group >= 0;
   }
