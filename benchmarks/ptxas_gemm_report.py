@@ -35,7 +35,7 @@ EPIS = {0: "BF16", 1: "F32", 2: "F32_ACC", 3: "BF16_ACC", 4: "CE_LSE", 5: "CE_DL
 COMMS = {0: "-", 1: "AG_A", 2: "RS_D", 3: "AG_KA", 4: "AG_KB", 5: "WAIT_A"}
 _GEMM = re.compile(r"gemm_kernelILi(\d+)ELi(\d+)ELb([01])ELb([01])ELi(\d+)ELi(\d+)ELi(\d+)EE")
 _FP8 = re.compile(r"gemm_fp8_kernelILi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)EE")
-SCALINGS = {0: "ROWCOL", 1: "MX"}
+SCALINGS = {0: "ROWCOL", 1: "MX", 2: "BLOCK"}
 _ATTN_FWD = re.compile(r"flash_attn_fwd_kernelILi(\d+)ELi(\d+)EE")
 _ATTN_BWD = re.compile(r"flash_attn_bwd_kernelILi(\d+)ELi(\d+)ELb([01])EE")
 

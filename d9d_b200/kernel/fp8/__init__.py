@@ -1,6 +1,6 @@
 """FP8 (e4m3) linear algebra on the Hopper tensor cores (wgmma).
 
-Two operand recipes, both with fp32 accumulation in registers and a bf16 result:
+Three operand recipes, all with fp32 accumulation in registers:
 
 * **row / column scaling**: one fp32 scale per row of each operand (per token / per output channel),
   applied to the accumulator in the GEMM epilogue.  Used by :class:`Fp8LinearFunction` for all three GEMMs of a linear
@@ -8,6 +8,12 @@ Two operand recipes, both with fp32 accumulation in registers and a bf16 result:
   dimension, which the transposing column-wise quantiser produces in one pass.
 * **MXFP8**: OCP micro-scaling - one power-of-two (UE8M0) scale per 32 consecutive
   K-elements; every K=32 wgmma produces a partial product that is added to the accumulator with its two scales.
+* **blockwise** (DeepSeek-V3): one fp32 scale per 1x128 group of an activation row and per 128x128 block of a weight,
+  both along the reduction dimension.  Every 128-deep k-block of the GEMM is summed by the tensor core into a fresh
+  accumulator and added to the fp32 accumulator with its row x column scale ("promotion"), so one outlier only sets the
+  scale of its own group and the accumulation is never one long reduced-precision chain.  Scales are stored
+  k-block-major, ``[ceil(K/128), rows]``.  Used by :class:`BlockwiseFp8LinearFunction`; the weight gradient is written
+  by the GEMM in the gradient dtype (fp32 or bf16).
 
 The reference framework has no fp8 path of its own (its published fp8 numbers come from torchao-style recipes layered on
 top); this module is the native equivalent.  Every function has a PyTorch emulation (same rounding, same scale rules) that
@@ -98,6 +104,51 @@ def _scaled_mm_reference(aq, sa, bq, sb) -> torch.Tensor:
     return ((aq.float() @ bq.float().t()) * sa[:, None] * sb[None, :]).to(torch.bfloat16)
 
 
+def _group_scales(amax: torch.Tensor) -> torch.Tensor:
+    return torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+
+
+def quantize_blockwise_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [M, K]`` -> ``(q [M, K] e4m3, s [ceil(K/128), M] fp32)`` with ``x[m, k] ~= q[m, k] * s[k // 128, m]``: one scale
+    per 1x128 group of every row (a partial last group covers its valid elements; an all-zero group gets scale 1)."""
+    M, K = x.shape
+    G = (K + 127) // 128
+    xg = torch.nn.functional.pad(x.float(), (0, G * 128 - K)).view(M, G, 128)
+    scale = _group_scales(xg.abs().amax(dim=-1))  # [M, G]
+    q = (xg / scale[..., None]).clamp(-E4M3_MAX, E4M3_MAX).to(FP8).view(M, G * 128)[:, :K]
+    return q.contiguous(), scale.t().contiguous()
+
+
+def quantize_blockwise_t_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [M, C]`` -> ``(qT [C, M], s [ceil(M/128), C])``: the transposed copy with one scale per 128 rows (tokens) of every
+    column (channel)."""
+    return quantize_blockwise_reference(x.t())
+
+
+def quantize_weight_blocks_reference(w: torch.Tensor, transpose: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
+    """``w [N, K]`` -> one scale per 128x128 block, repeated on each row of the copy the GEMM reads:
+    ``(q [N, K], s [ceil(K/128), N])``, or with ``transpose`` ``(qT [K, N], s [ceil(N/128), K])``.  ``qT`` is bitwise ``q^T``."""
+    N, K = w.shape
+    Nb, Kb = (N + 127) // 128, (K + 127) // 128
+    wb = torch.nn.functional.pad(w.float(), (0, Kb * 128 - K, 0, Nb * 128 - N)).view(Nb, 128, Kb, 128)
+    scale = _group_scales(wb.abs().amax(dim=(1, 3)))  # [Nb, Kb]
+    q = (wb / scale[:, None, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(FP8).view(Nb * 128, Kb * 128)[:N, :K]
+    if transpose:
+        return q.t().contiguous(), scale.repeat_interleave(128, dim=1)[:, :K].contiguous()
+    return q.contiguous(), scale.t().repeat_interleave(128, dim=1)[:, :N].contiguous()
+
+
+def blockwise_mm_reference(aq, sa, bq, sb, out_dtype: torch.dtype = torch.bfloat16, acc_dtype: torch.dtype = torch.float32):
+    """``sum_kb (aq[:, kb] @ bq[:, kb]^T) * sa[kb, :, None] * sb[kb, None, :]`` over the 128-deep k-blocks ``kb``."""
+    K = aq.shape[1]
+    acc = torch.zeros(aq.shape[0], bq.shape[0], dtype=acc_dtype, device=aq.device)
+    for kb in range((K + 127) // 128):
+        ks = slice(kb * 128, min(K, kb * 128 + 128))
+        part = aq[:, ks].to(acc_dtype) @ bq[:, ks].to(acc_dtype).t()
+        acc += part * sa[kb].to(acc_dtype)[:, None] * sb[kb].to(acc_dtype)[None, :]
+    return acc.to(out_dtype)
+
+
 # ---------------------------------------------------------------------------------------------------- public ops
 def quantize_rowwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     return native_ops().quantize_rowwise(x) if on_gpu(x) else quantize_rowwise_reference(x)
@@ -128,6 +179,31 @@ def mx_mm(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     aq, ea = quantize_mx_reference(a)
     bq, eb = quantize_mx_reference(b)
     return (dequantize_mx(aq, ea) @ dequantize_mx(bq, eb).t()).to(torch.bfloat16)
+
+
+def quantize_blockwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [M, K]`` -> ``(q [M, K], s [ceil(K/128), M])``: 1x128 groups along the reduction dimension."""
+    return native_ops().quantize_blockwise(x) if on_gpu(x) else quantize_blockwise_reference(x)
+
+
+def quantize_blockwise_t(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [M, C]`` -> ``(qT [C, M], s [ceil(M/128), C])``: 128-token groups of every channel, transposed copy."""
+    return native_ops().quantize_blockwise_t(x) if on_gpu(x) else quantize_blockwise_t_reference(x)
+
+
+def quantize_weight_blocks(w: torch.Tensor, transpose: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
+    """``w [N, K]`` -> 128x128-block scaled ``(q [N, K], s [ceil(K/128), N])`` or ``(qT [K, N], s [ceil(N/128), K])``."""
+    return native_ops().quantize_weight_blocks(w, transpose) if on_gpu(w) else quantize_weight_blocks_reference(w, transpose)
+
+
+def blockwise_mm(aq: torch.Tensor, sa: torch.Tensor, bq: torch.Tensor, sb: torch.Tensor, out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """``sum_kb (aq[:, kb] @ bq[:, kb]^T) * sa[kb, :, None] * sb[kb, None, :]`` -> ``out_dtype`` (bf16 or fp32), with the
+    per-(k-block, row) scales of :func:`quantize_blockwise`, :func:`quantize_blockwise_t` and :func:`quantize_weight_blocks`."""
+    if on_gpu(aq):
+        out = torch.empty(aq.shape[0], bq.shape[0], device=aq.device, dtype=out_dtype)
+        native_ops().gemm_fp8_blockwise(aq, sa, bq, sb, out)
+        return out
+    return blockwise_mm_reference(aq, sa, bq, sb, out_dtype)
 
 
 class Fp8LinearFunction(Function):
@@ -203,21 +279,68 @@ class MxFp8LinearFunction(Function):
         return dx, dw
 
 
+class BlockwiseFp8LinearFunction(Function):
+    """``y = x @ W^T`` with all three GEMMs in e4m3 with DeepSeek-V3's blockwise scaling and promoted accumulation.
+
+    forward  ``y  = Q_blk(x)  · Q_W(W)^T``           x: 1x128 groups along ``in``; W: 128x128 blocks
+    dgrad    ``dx = Q_blk(dy) · Q_W(W^T)^T``         dy: 1x128 groups along ``out``; the transposed copy of W's blocks
+    wgrad    ``dW = Q_blkT(dy) · Q_blkT(x)^T``       128-token groups of every channel, written in the gradient dtype
+
+    Nothing quantised is kept between forward and backward: the backward re-quantises ``x`` and ``W`` from the saved bf16
+    tensors, so the activation memory is that of the row-wise recipe.  Feature sizes must be multiples of 16; the token
+    count is free.
+    """
+
+    @staticmethod
+    def forward(ctx: Any, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+        x2 = x.reshape(-1, x.shape[-1])
+        if not x2.is_contiguous():
+            x2 = x2.contiguous()
+        xq, sx = quantize_blockwise(x2)
+        wq, sw = quantize_weight_blocks(weight)
+        ctx.save_for_backward(x2, weight)
+        ctx.x_shape = x.shape
+        return blockwise_mm(xq, sx, wq, sw).view(*x.shape[:-1], weight.shape[0])
+
+    @staticmethod
+    def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
+        x2, weight = ctx.saved_tensors
+        dy = grad_output.reshape(-1, grad_output.shape[-1])
+        if not dy.is_contiguous():
+            dy = dy.contiguous()
+        dx = dw = None
+        if ctx.needs_input_grad[0] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.inputs):
+            dyq, sdy = quantize_blockwise(dy)
+            wtq, swt = quantize_weight_blocks(weight, transpose=True)  # [in, out]
+            dx = blockwise_mm(dyq, sdy, wtq, swt).view(ctx.x_shape)
+        if ctx.needs_input_grad[1] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.weight):
+            dytq, sdyt = quantize_blockwise_t(dy)  # [out, tokens]
+            xtq, sxt = quantize_blockwise_t(x2)  # [in, tokens]
+            dw = blockwise_mm(dytq, sdyt, xtq, sxt, out_dtype=grad_dtype_of(weight))
+        return dx, dw
+
+
 def fp8_linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = None, recipe: str = "rowwise") -> torch.Tensor:
     """``x @ weight^T (+ bias)`` in fp8.  ``recipe="rowwise"``: dynamic per-row / per-column fp32 scales
     (:class:`Fp8LinearFunction`, feature sizes multiples of 16); ``recipe="mx"``: MXFP8 block scaling
-    (:class:`MxFp8LinearFunction`, feature sizes and token count multiples of 128)."""
-    if recipe not in ("rowwise", "mx"):
+    (:class:`MxFp8LinearFunction`, feature sizes and token count multiples of 128); ``recipe="blockwise"``: DeepSeek-V3's
+    1x128 / 128x128 scaling with promoted accumulation (:class:`BlockwiseFp8LinearFunction`, feature sizes multiples of
+    16, any token count)."""
+    if recipe not in _RECIPES:
         raise ValueError(f"unknown fp8 recipe {recipe!r}")
-    granule = 16 if recipe == "rowwise" else 128
+    granule = _GRANULE[recipe]
     tokens = x.numel() // max(x.shape[-1], 1)
     if x.shape[-1] % granule or weight.shape[0] % granule or (recipe == "mx" and tokens % granule):
         raise ValueError(f"fp8_linear[{recipe}]: sizes must be multiples of {granule} (got in={x.shape[-1]}, out={weight.shape[0]}, "
                          f"tokens={tokens})")
     if on_gpu(x) and (x.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16):
         raise RuntimeError("fp8_linear: bf16 activations and weights required on CUDA")
-    out = (Fp8LinearFunction if recipe == "rowwise" else MxFp8LinearFunction).apply(x, weight)
+    out = _RECIPES[recipe].apply(x, weight)
     return out if bias is None else out + bias
+
+
+_RECIPES = {"rowwise": Fp8LinearFunction, "mx": MxFp8LinearFunction, "blockwise": BlockwiseFp8LinearFunction}
+_GRANULE = {"rowwise": 16, "mx": 128, "blockwise": 16}  # feature sizes (and, for "mx", the token count) must be multiples
 
 
 class Fp8Linear(nn.Linear):
@@ -237,9 +360,9 @@ def convert_linears_to_fp8(module: nn.Module, predicate=lambda name, m: True, re
     number converted."""
     from d9d_b200.module.block.linear import Linear as NativeLinear
 
-    if recipe not in ("rowwise", "mx"):
+    if recipe not in _RECIPES:
         raise ValueError(f"unknown fp8 recipe {recipe!r}")
-    granule = 16 if recipe == "rowwise" else 128
+    granule = _GRANULE[recipe]
     n = 0
     for name, m in module.named_modules():
         if type(m) in (nn.Linear, NativeLinear) and m.in_features % granule == 0 and m.out_features % granule == 0 and predicate(name, m):
@@ -250,8 +373,10 @@ def convert_linears_to_fp8(module: nn.Module, predicate=lambda name, m: True, re
 
 
 __all__ = [
-    "Fp8Linear", "Fp8LinearFunction", "MxFp8LinearFunction", "convert_linears_to_fp8", "dequantize_mx", "fp8_linear", "mx_mm", "mx_scale_exponent",
+    "BlockwiseFp8LinearFunction", "Fp8Linear", "Fp8LinearFunction", "MxFp8LinearFunction", "blockwise_mm", "blockwise_mm_reference",
+    "convert_linears_to_fp8", "dequantize_mx", "fp8_linear", "mx_mm", "mx_scale_exponent",
+    "quantize_blockwise", "quantize_blockwise_reference", "quantize_blockwise_t", "quantize_blockwise_t_reference",
     "quantize_colwise_t", "quantize_colwise_t_batched_reference", "quantize_colwise_t_reference", "quantize_mx_reference",
-    "quantize_segments_t_reference", "quantize_rowwise", "quantize_rowwise_reference",
-    "scaled_mm", "unpack_mx_scales",
+    "quantize_segments_t_reference", "quantize_rowwise", "quantize_rowwise_reference", "quantize_weight_blocks",
+    "quantize_weight_blocks_reference", "scaled_mm", "unpack_mx_scales",
 ]

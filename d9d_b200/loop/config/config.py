@@ -51,7 +51,9 @@ class Fp8LinearConfig(BaseModel):
 
     include: str = r".*"
     exclude: str | None = r"lm_head|cls_head|embedding_head|router|\.gate$"
-    recipe: Literal["rowwise", "mx"] = "rowwise"  # "mx": MXFP8 block scaling (feature sizes and token count multiples of 128)
+    # "mx": MXFP8 block scaling (feature sizes and token count multiples of 128); "blockwise": DeepSeek-V3's 1x128 activation
+    # / 128x128 weight scaling with promoted accumulation (feature sizes multiples of 16)
+    recipe: Literal["rowwise", "mx", "blockwise"] = "rowwise"
 
 
 class ModelStageFactoryConfig(BaseModel):

@@ -485,6 +485,101 @@ void gemm_fp8_grouped_k(const Tensor& a, const Tensor& sa, const Tensor& b, cons
   d9d::gemm_fp8(g, cur_stream());
 }
 
+// ------------------------------------------------------------------ blockwise fp8 (DeepSeek-V3 recipe) ----------------
+// Scales are k-block-major: [ceil(K/128), rows] with a row pitch of round_up(rows, 128) (a view of a zero-padded
+// allocation), so the GEMM reads a tile's scales as one aligned 512-byte copy inside the tensor.
+static int64_t round_up128(int64_t v) { return (v + 127) / 128 * 128; }
+
+static Tensor blockwise_scales(const Tensor& like, int64_t groups, int64_t rows) {
+  return at::zeros({groups, round_up128(rows)}, like.options().dtype(at::kFloat)).narrow(1, 0, rows);
+}
+
+static void check_blockwise_input(const char* op, const Tensor& x) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.stride(1) == 1 && x.scalar_type() == at::kBFloat16, op, ": 2-D bf16 CUDA tensor with unit column stride required");
+  TORCH_CHECK(x.stride(0) % 8 == 0 && (reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0, op, ": rows must be 16-byte aligned");
+  TORCH_CHECK(x.size(0) < (int64_t(1) << 31) && x.size(1) < (int64_t(1) << 31), op, ": too large");
+}
+
+// x[M,K] bf16 (K a multiple of 16) -> (q[M,K] e4m3, s[ceil(K/128), M] fp32): one scale per 1 x 128 group of every row
+std::tuple<Tensor, Tensor> quantize_blockwise(const Tensor& x) {
+  check_blockwise_input("quantize_blockwise", x);
+  TORCH_CHECK(x.size(1) % 16 == 0, "quantize_blockwise: K must be a multiple of 16");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t M = x.size(0), K = x.size(1);
+  Tensor q = at::empty({M, K}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = blockwise_scales(x, (K + 127) / 128, M);
+  d9d::quantize_blockwise_e4m3(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), M, static_cast<int>(K), x.stride(0), K, s.stride(0),
+                               0, false, cur_stream());
+  return {q, s};
+}
+
+// x[M,C] bf16 (C a multiple of 16, any M) -> (qt[C,M] e4m3 with a 16-byte row pitch and zero pad columns,
+// s[ceil(M/128), C] fp32): one scale per 128 rows of every column, i.e. per 128-token group of a channel
+std::tuple<Tensor, Tensor> quantize_blockwise_t(const Tensor& x) {
+  check_blockwise_input("quantize_blockwise_t", x);
+  TORCH_CHECK(x.size(1) % 16 == 0, "quantize_blockwise_t: C must be a multiple of 16");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t M = x.size(0), C = x.size(1);
+  const int64_t pitch = (M + 15) / 16 * 16;
+  Tensor qt = at::empty({C, pitch}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = blockwise_scales(x, (M + 127) / 128, C);
+  d9d::quantize_blockwise_e4m3(x.data_ptr(), qt.data_ptr(), s.data_ptr<float>(), M, static_cast<int>(C), x.stride(0), pitch, s.stride(0),
+                               1, true, cur_stream());
+  return {qt.narrow(1, 0, M), s};
+}
+
+// w[N,K] bf16 (N, K multiples of 16) -> one scale per 128 x 128 block, repeated on each row of the copy the GEMM reads:
+//   transpose = false: (q[N,K], s[ceil(K/128), N]);  transpose = true: (qt[K,N], s[ceil(N/128), K])
+std::tuple<Tensor, Tensor> quantize_weight_blocks(const Tensor& w, bool transpose) {
+  check_blockwise_input("quantize_weight_blocks", w);
+  TORCH_CHECK(w.size(0) % 16 == 0 && w.size(1) % 16 == 0, "quantize_weight_blocks: both dims must be multiples of 16");
+  c10::cuda::CUDAGuard guard(w.device());
+  const int64_t N = w.size(0), K = w.size(1);
+  Tensor q = transpose ? at::empty({K, N}, w.options().dtype(at::kFloat8_e4m3fn)) : at::empty({N, K}, w.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = transpose ? blockwise_scales(w, (N + 127) / 128, K) : blockwise_scales(w, (K + 127) / 128, N);
+  d9d::quantize_blockwise_e4m3(w.data_ptr(), q.data_ptr(), s.data_ptr<float>(), N, static_cast<int>(K), w.stride(0), q.stride(0),
+                               s.stride(0), 2, transpose, cur_stream());
+  return {q, s};
+}
+
+static void check_blockwise_scales(const char* name, const Tensor& s, const Tensor& like, int64_t groups, int64_t rows) {
+  TORCH_CHECK(s.is_cuda() && s.device() == like.device(), "gemm_fp8_blockwise: ", name, " must be on the operands' device");
+  TORCH_CHECK(s.scalar_type() == at::kFloat && s.dim() == 2 && s.size(0) == groups && s.size(1) == rows && s.stride(1) == 1,
+              "gemm_fp8_blockwise: ", name, " must be fp32 [ceil(K/128), rows] with the K and rows of its operand");
+  TORCH_CHECK(s.stride(0) == round_up128(rows), "gemm_fp8_blockwise: ", name, " must have a row pitch of round_up(rows, 128)");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(s.data_ptr()) & 15) == 0, "gemm_fp8_blockwise: ", name, " must start on a 16-byte boundary");
+  const int64_t avail = static_cast<int64_t>(s.storage().nbytes()) - s.storage_offset() * 4;
+  TORCH_CHECK(avail >= groups * s.stride(0) * 4, "gemm_fp8_blockwise: ", name, "'s storage must hold its padded rows");
+}
+
+// d[M,N] (bf16 or fp32) = sum over 128-deep k-blocks kb of (a[:, kb] · b[:, kb]^T) * sa[kb, m] * sb[kb, n]
+void gemm_fp8_blockwise(const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, Tensor d) {
+  for (const Tensor* t : {&a, &b, static_cast<const Tensor*>(&d)})
+    TORCH_CHECK(t->is_cuda() && t->device() == a.device() && t->dim() == 2 && t->stride(1) == 1,
+                "gemm_fp8_blockwise: a, b and d must be 2-D CUDA tensors on one device with unit column stride");
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn, "gemm_fp8_blockwise: a and b must be float8_e4m3fn");
+  TORCH_CHECK(d.scalar_type() == at::kBFloat16 || d.scalar_type() == at::kFloat, "gemm_fp8_blockwise: d must be bf16 or fp32");
+  TORCH_CHECK(a.size(1) == b.size(1) && a.size(1) > 0, "gemm_fp8_blockwise: a and b must share a positive K");
+  TORCH_CHECK(d.size(0) == a.size(0) && d.size(1) == b.size(0), "gemm_fp8_blockwise: d must be [M, N]");
+  TORCH_CHECK(a.size(0) < (int64_t(1) << 31) && b.size(0) < (int64_t(1) << 31) && a.size(1) < (int64_t(1) << 31), "gemm_fp8_blockwise: too large");
+  CHECK_ALIGNED16(a); CHECK_ALIGNED16(b); CHECK_ALIGNED16(d);
+  TORCH_CHECK(a.stride(0) % 16 == 0 && b.stride(0) % 16 == 0, "gemm_fp8_blockwise: rows of a and b must be 16-byte aligned");
+  TORCH_CHECK(d.stride(0) * d.element_size() % 16 == 0 && d.size(1) * d.element_size() % 16 == 0,
+              "gemm_fp8_blockwise: rows of d must be a multiple of 16 bytes");
+  const int64_t kb = (a.size(1) + 127) / 128;
+  check_blockwise_scales("sa", sa, a, kb, a.size(0));
+  check_blockwise_scales("sb", sb, a, kb, b.size(0));
+  c10::cuda::CUDAGuard guard(a.device());
+  d9d::Fp8GemmArgs g;
+  g.blockwise = true;
+  g.epi = d.scalar_type() == at::kBFloat16 ? 0 : 1;
+  g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1)); g.N = static_cast<int>(b.size(0));
+  g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
+  g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(0);
+  g.scale_a = sa.data_ptr<float>(); g.scale_b = sb.data_ptr<float>();
+  d9d::gemm_fp8(g, cur_stream());
+}
+
 // ------------------------------------------------------------------ RMSNorm ---------------------
 std::tuple<Tensor, Tensor> rms_norm_fwd(const Tensor& x, const Tensor& w, double eps, bool zero_centered) {
   CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(w); CHECK_ALIGNED16(x); CHECK_ALIGNED16(w);
@@ -1149,6 +1244,10 @@ TORCH_LIBRARY(d9d_b200, m) {
   m.def("quantize_segments_t(Tensor x, Tensor tile_group, Tensor seg_offsets, Tensor counts) -> (Tensor, Tensor)");
   m.def("gemm_fp8_grouped_m(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d, Tensor tile_group, bool accumulate=False) -> ()");
   m.def("gemm_fp8_grouped_k(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d, Tensor group_offsets, bool accumulate) -> ()");
+  m.def("quantize_blockwise(Tensor x) -> (Tensor, Tensor)");
+  m.def("quantize_blockwise_t(Tensor x) -> (Tensor, Tensor)");
+  m.def("quantize_weight_blocks(Tensor w, bool transpose=False) -> (Tensor, Tensor)");
+  m.def("gemm_fp8_blockwise(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d) -> ()");
   m.def("rms_norm_fwd(Tensor x, Tensor w, float eps, bool zero_centered) -> (Tensor, Tensor)");
   m.def("rms_norm_bwd(Tensor dout, Tensor x, Tensor w, Tensor inv_rms, bool zero_centered) -> (Tensor, Tensor)");
   m.def("silu_mul_fwd(Tensor x, Tensor y) -> Tensor");
@@ -1210,6 +1309,10 @@ TORCH_LIBRARY_IMPL(d9d_b200, CUDA, m) {
   m.impl("quantize_segments_t", &quantize_segments_t);
   m.impl("gemm_fp8_grouped_m", &gemm_fp8_grouped_m);
   m.impl("gemm_fp8_grouped_k", &gemm_fp8_grouped_k);
+  m.impl("quantize_blockwise", &quantize_blockwise);
+  m.impl("quantize_blockwise_t", &quantize_blockwise_t);
+  m.impl("quantize_weight_blocks", &quantize_weight_blocks);
+  m.impl("gemm_fp8_blockwise", &gemm_fp8_blockwise);
   m.impl("rms_norm_fwd", &rms_norm_fwd);
   m.impl("rms_norm_bwd", &rms_norm_bwd);
   m.impl("silu_mul_fwd", &silu_mul_fwd);

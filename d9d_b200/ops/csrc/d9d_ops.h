@@ -93,6 +93,8 @@ struct Fp8GemmArgs {
   float scale_scalar = 1.f;
   const uint8_t* sfa = nullptr;       // [ceil(M/128), K/128, 512]
   const uint8_t* sfb = nullptr;       // [2*ceil(N/256), K/128, 512]
+  bool blockwise = false;             // true: scale_a / scale_b are [ceil(K/128), round_up(M / N, 128)] per (k-block, row)
+                                      // scales (DENSE, epi bf16 or fp32 store)
 };
 void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream);
 void quantize_rowwise_e4m3(const void* x, void* q, float* scale, long long M, int K, long long ldx, cudaStream_t stream);
@@ -108,6 +110,12 @@ void quantize_segments_t_e4m3(const void* x, void* qt, float* scale, float* amax
                               cudaStream_t stream);
 // sf must be zero-initialised by the caller when M is not a multiple of 256 (pad blocks)
 void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long long ldx, cudaStream_t stream);
+// x[R, C] bf16 -> e4m3 with one fp32 scale (amax / 448, 1 for all-zero groups) per group: group 0 = 1 x 128 row groups
+// (q[R, C], s[ceil(C/128), lds]), 1 = 128 x 1 column groups (transposed qT[C, R] with pitch ldq >= R, zero pad columns,
+// s[ceil(R/128), lds]), 2 = 128 x 128 blocks (plain: s[ceil(C/128), lds] per row, transposed: s[ceil(R/128), lds] per
+// column of qT's rows).  lds is the scale row pitch, a multiple of 128 at least the scaled dimension.
+void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, int C, long long ldx, long long ldq, long long lds,
+                             int group, bool transpose, cudaStream_t stream);
 
 // ------------------------------------------------------------------ normalisation ----------------
 // dtype codes: 0 = bf16, 1 = fp32, 2 = fp16

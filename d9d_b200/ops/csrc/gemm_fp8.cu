@@ -4,8 +4,11 @@
 //   quantize_segments_t  x[cap,C] bf16 -> qT[C,cap] e4m3, scale[E,C]   (transposed copy, scale per column of every expert's
 //                                                                      rows; pad rows come out as zeros)
 //   quantize_mx          x[M,K] bf16 -> q[M,K] e4m3, UE8M0 scale blocks  (one scale per 32 K-elements, 128-row x 4-group blocks)
-//   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on wgmma e4m3 (MX: per-32-K scales applied in registers), and the
-//                          grouped expert GEMMs (GROUPED_M / GROUPED_K, see gemm_fp8_sm90.cuh)
+//   quantize_blockwise   x[R,C] bf16 -> e4m3 with fp32 scales per 1x128 row group, 128x1 column group (transposed copy) or
+//                        128x128 block (either copy), stored k-block-major for the BLOCKWISE GEMM
+//   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on wgmma e4m3 (MX: per-32-K scales applied in registers), the
+//                          grouped expert GEMMs (GROUPED_M / GROUPED_K) and the BLOCKWISE GEMM (bf16 / fp32 D), see
+//                          gemm_fp8_sm90.cuh
 #include <cuda_fp8.h>
 
 #include "gemm_fp8_sm90.cuh"
@@ -184,6 +187,137 @@ __global__ void quant_mx_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __
   sf[blk * 512 + (r % 32) * 16 + (r / 32) * 4 + (g % 4)] = static_cast<uint8_t>(e + 127);
 }
 
+// ---- blockwise: one CTA per 128 x 128 tile of x, single pass ------------------------------------------------------
+// Every scale group (1 x 128 row group, 128 x 1 column group, 128 x 128 block) lies inside one tile, so the tile's amax
+// needs no second pass, atomics or scratch.  Thread (tx, ty) of 256 holds rows 8 ty .. 8 ty + 7 and columns
+// 8 tx .. 8 tx + 7 of the tile; elements past R / C are read as zero (a partial group's scale covers its valid elements).
+//   not transposed: q[r, c] row pitch ldq bytes; s[c / 128][r] (ROW: the row group's scale, BLOCK: the block's)
+//   transposed:     q[c, r] row pitch ldq bytes, columns r in [R, ldq) written as zeros; s[r / 128][c] (COL / BLOCK)
+enum BlockGroup : int { GROUP_ROW = 0, GROUP_COL = 1, GROUP_BLOCK = 2 };
+
+template <int GROUP, bool TRANSPOSE>
+__global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
+                                                              float* __restrict__ s, long long R, int C, long long ldx, long long ldq,
+                                                              long long lds) {
+  static_assert(GROUP == GROUP_BLOCK || (GROUP == GROUP_ROW) != TRANSPOSE, "row groups: plain copy; column groups: transposed");
+  __shared__ float red[8][128];                          // per-warp partial amax (COL: per column, BLOCK: one value)
+  __shared__ uint32_t tq[TRANSPOSE ? 128 : 1][33];       // transposed tile: 128 columns x 128 row bytes (+1 word pad)
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r0 = static_cast<long long>(blockIdx.y) * 128;
+  const int c0 = blockIdx.x * 128;
+  const int cc = c0 + 8 * tx;
+  float v[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const long long r = r0 + 8 * ty + i;
+    if (r < R && cc < C) {
+      load8_bf16(x + r * ldx + cc, v[i]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[i][j] = 0.f;
+    }
+  }
+  // scales: the ROW group of each of this thread's rows, the COL group of each of its columns, or the BLOCK's
+  float inv_r[8], inv_c[8];
+  if constexpr (GROUP == GROUP_ROW) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      float a = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a = fmaxf(a, fabsf(v[i][j]));
+#pragma unroll
+      for (int o = 1; o < 16; o <<= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));  // the 16 threads of the row
+      const float sc = a > 0.f ? a / E4M3_MAX : 1.f;
+      inv_r[i] = 1.f / sc;
+      const long long r = r0 + 8 * ty + i;
+      if (tx == 0 && r < R) s[static_cast<long long>(blockIdx.x) * lds + r] = sc;
+    }
+  } else if constexpr (GROUP == GROUP_COL) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float a = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) a = fmaxf(a, fabsf(v[i][j]));
+      a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, 16));  // the warp's two row slices
+      if (lane < 16) red[warp][8 * tx + j] = a;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float a = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) a = fmaxf(a, red[w][8 * tx + j]);
+      const float sc = a > 0.f ? a / E4M3_MAX : 1.f;
+      inv_c[j] = 1.f / sc;
+      if (ty == 0 && cc + j < C) s[static_cast<long long>(blockIdx.y) * lds + cc + j] = sc;
+    }
+  } else {
+    float a = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a = fmaxf(a, fabsf(v[i][j]));
+    a = warp_max(a);
+    if (lane == 0) red[warp][0] = a;
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < 8; ++w) a = fmaxf(a, red[w][0]);
+    const float sc = a > 0.f ? a / E4M3_MAX : 1.f;
+    inv_r[0] = 1.f / sc;
+    // one scale per row (plain copy) or per column (transposed copy) of the block: 128 values, 256 threads
+    if (threadIdx.x < 128) {
+      if constexpr (TRANSPOSE) {
+        if (c0 + static_cast<int>(threadIdx.x) < C) s[static_cast<long long>(blockIdx.y) * lds + c0 + threadIdx.x] = sc;
+      } else {
+        if (r0 + threadIdx.x < R) s[static_cast<long long>(blockIdx.x) * lds + r0 + threadIdx.x] = sc;
+      }
+    }
+  }
+  auto inv_of = [&](int i, int j) {
+    if constexpr (GROUP == GROUP_ROW) return inv_r[i];
+    else if constexpr (GROUP == GROUP_COL) return inv_c[j];
+    else return inv_r[0];
+  };
+  if constexpr (!TRANSPOSE) {
+    if (cc >= C) return;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const long long r = r0 + 8 * ty + i;
+      if (r >= R) break;
+      float w[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) w[j] = v[i][j] * inv_of(i, j);
+      *reinterpret_cast<uint2*>(q + r * ldq + cc) = quant8(w, 1.f);
+    }
+  } else {
+    // column 8 tx + j of the tile becomes row 8 tx + j of the transposed tile; this thread's 8 rows are its bytes 8 ty ..
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      uint32_t lo = 0, hi = 0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        lo |= static_cast<uint32_t>(__nv_cvt_float_to_fp8(v[i][j] * inv_of(i, j), __NV_SATFINITE, __NV_E4M3)) << (8 * i);
+        hi |= static_cast<uint32_t>(__nv_cvt_float_to_fp8(v[i + 4][j] * inv_of(i + 4, j), __NV_SATFINITE, __NV_E4M3)) << (8 * i);
+      }
+      tq[8 * tx + j][2 * ty] = lo;
+      tq[8 * tx + j][2 * ty + 1] = hi;
+    }
+    __syncthreads();
+    // 16 bytes per thread: 8 threads per output row of 128 bytes, 32 rows per pass; pad columns up to ldq get the zeros
+    // of the rows past R
+#pragma unroll
+    for (int pass = 0; pass < 4; ++pass) {
+      const int row = pass * 32 + (threadIdx.x >> 3), seg = threadIdx.x & 7;
+      const long long col = r0 + 16 * seg;
+      if (c0 + row < C && col < ldq) {
+        const uint4 w = make_uint4(tq[row][4 * seg], tq[row][4 * seg + 1], tq[row][4 * seg + 2], tq[row][4 * seg + 3]);
+        *reinterpret_cast<uint4*>(q + static_cast<long long>(c0 + row) * ldq + col) = w;
+      }
+    }
+  }
+}
+
 // 2-D map, or 3-D ([d2, d1, d0], box depth 1) when d2 > 0
 CUtensorMap make_tmap_u8(const void* base, uint64_t d0, uint64_t d1, uint64_t stride1_bytes, uint32_t box0, uint32_t box1,
                          uint64_t d2 = 0, uint64_t stride2_bytes = 0) {
@@ -281,9 +415,33 @@ void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long
                                                                              static_cast<uint8_t*>(q), static_cast<uint8_t*>(sf), M, K, ldx);
 }
 
+void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, int C, long long ldx, long long ldq, long long lds,
+                             int group, bool transpose, cudaStream_t stream) {
+  if (R <= 0 || C <= 0) return;
+  if (C % 8 != 0) throw std::runtime_error("d9d quantize_blockwise: C must be a multiple of 8");
+  const dim3 grid(static_cast<unsigned>((C + 127) / 128), static_cast<unsigned>((R + 127) / 128));
+  const auto* xb = static_cast<const __nv_bfloat16*>(x);
+  auto* qb = static_cast<uint8_t*>(q);
+  if (group == GROUP_ROW && !transpose)
+    quant_blockwise_kernel<GROUP_ROW, false><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, ldx, ldq, lds);
+  else if (group == GROUP_COL && transpose)
+    quant_blockwise_kernel<GROUP_COL, true><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, ldx, ldq, lds);
+  else if (group == GROUP_BLOCK && !transpose)
+    quant_blockwise_kernel<GROUP_BLOCK, false><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, ldx, ldq, lds);
+  else if (group == GROUP_BLOCK && transpose)
+    quant_blockwise_kernel<GROUP_BLOCK, true><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, ldx, ldq, lds);
+  else
+    throw std::runtime_error("d9d quantize_blockwise: row groups give a plain copy, column groups a transposed one");
+}
+
 void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0) return;
-  if (a.block_scaled) {
+  if (a.blockwise) {
+    if (a.scale_a == nullptr || a.scale_b == nullptr) throw std::runtime_error("d9d gemm_fp8_blockwise: both scale tensors are required");
+    if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_BF16>(a, stream);
+    else if (a.epi == gemm::EPI_F32) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_F32>(a, stream);
+    else throw std::runtime_error("d9d gemm_fp8_blockwise: bf16 or fp32 store only");
+  } else if (a.block_scaled) {
     if (a.K % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr)
       throw std::runtime_error("d9d gemm_mxfp8: K must be a multiple of 128 and both scale-factor tensors are required");
     launch_fp8<128, fp8::MX>(a, stream);
