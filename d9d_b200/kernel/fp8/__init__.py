@@ -1,13 +1,14 @@
 """FP8 (e4m3) linear algebra on the Hopper tensor cores (wgmma).
 
-Three operand recipes, all with fp32 accumulation in registers:
+Three operand recipes.  The tensor core sums an MMA chain in a reduced-precision accumulator (not fp32), so how long the
+chains are sets the accuracy of a long reduction:
 
-* **row / column scaling**: one fp32 scale per row of each operand (per token / per output channel),
-  applied to the accumulator in the GEMM epilogue.  Used by :class:`Fp8LinearFunction` for all three GEMMs of a linear
-  layer (forward, input gradient, weight gradient); the two backward GEMMs need K-major operands along the *other*
-  dimension, which the transposing column-wise quantiser produces in one pass.
+* **row / column scaling**: one fp32 scale per row of each operand (per token / per output channel), applied to the
+  accumulator in the GEMM epilogue; the whole of K is one chain (no promotion).  Used by :class:`Fp8LinearFunction`
+  for all three GEMMs of a linear layer (forward, input gradient, weight gradient); the two backward GEMMs need K-major
+  operands along the *other* dimension, which the transposing column-wise quantiser produces in one pass.
 * **MXFP8**: OCP micro-scaling - one power-of-two (UE8M0) scale per 32 consecutive
-  K-elements; every K=32 wgmma produces a partial product that is added to the accumulator with its two scales.
+  K-elements; every K=32 wgmma produces a partial product that is added to an fp32 accumulator with its two scales.
 * **blockwise** (DeepSeek-V3): one fp32 scale per 1x128 group of an activation row and per 128x128 block of a weight,
   both along the reduction dimension.  Every 128-deep k-block of the GEMM is summed by the tensor core into a fresh
   accumulator and added to the fp32 accumulator with its row x column scale ("promotion"), so one outlier only sets the
@@ -39,8 +40,7 @@ FP8 = torch.float8_e4m3fn
 # ---------------------------------------------------------------------------------------------------- emulation
 def quantize_rowwise_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     xf = x.float()
-    amax = xf.abs().amax(dim=1)
-    scale = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+    scale = _group_scales(xf.abs().amax(dim=1))
     q = (xf / scale[:, None]).clamp(-E4M3_MAX, E4M3_MAX).to(FP8)
     return q, scale
 
@@ -105,7 +105,9 @@ def _scaled_mm_reference(aq, sa, bq, sb) -> torch.Tensor:
 
 
 def _group_scales(amax: torch.Tensor) -> torch.Tensor:
-    return torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+    """``amax / 448``, at least 2**-126 (the smallest normal fp32, so that the kernels' reciprocal stays finite under
+    flush-to-zero), and 1 for an all-zero group."""
+    return torch.where(amax > 0, (amax / E4M3_MAX).clamp_min(2.0**-126), torch.ones_like(amax))
 
 
 def quantize_blockwise_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:

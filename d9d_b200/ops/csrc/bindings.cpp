@@ -408,7 +408,7 @@ void gemm_mxfp8(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tenso
   TORCH_CHECK(g.K % 128 == 0, "gemm_mxfp8: K must be a multiple of 128");
   const int64_t kb = g.K / 128;
   TORCH_CHECK(sfa.scalar_type() == at::kByte && sfa.numel() >= (static_cast<int64_t>(g.M) + 127) / 128 * kb * 512, "gemm_mxfp8: sfa too small");
-  TORCH_CHECK(sfb.scalar_type() == at::kByte && sfb.numel() >= (static_cast<int64_t>(g.N) + 255) / 256 * 2 * kb * 512, "gemm_mxfp8: sfb too small");
+  TORCH_CHECK(sfb.scalar_type() == at::kByte && sfb.numel() >= (static_cast<int64_t>(g.N) + 127) / 128 * kb * 512, "gemm_mxfp8: sfb too small");
   g.block_scaled = true;
   g.sfa = sfa.data_ptr<uint8_t>(); g.sfb = sfb.data_ptr<uint8_t>();
   d9d::gemm_fp8(g, cur_stream());

@@ -92,7 +92,7 @@ struct Fp8GemmArgs {
   const float* scale_b = nullptr;     // [N] or nullptr; grouped: [E, N]
   float scale_scalar = 1.f;
   const uint8_t* sfa = nullptr;       // [ceil(M/128), K/128, 512]
-  const uint8_t* sfb = nullptr;       // [2*ceil(N/256), K/128, 512]
+  const uint8_t* sfb = nullptr;       // [ceil(N/128), K/128, 512]
   bool blockwise = false;             // true: scale_a / scale_b are [ceil(K/128), round_up(M / N, 128)] per (k-block, row)
                                       // scales (DENSE, epi bf16 or fp32 store)
 };

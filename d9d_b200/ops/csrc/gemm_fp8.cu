@@ -19,6 +19,11 @@ namespace {
 
 constexpr float E4M3_MAX = 448.f;
 
+// Scale of a group with the given amax: amax / 448, at least FLT_MIN (2^-126), and 1 for an all-zero group.  The library
+// builds with fast math, where amax / 448 below FLT_MIN flushes to zero and 1 / 0 is inf: every code of the group would
+// become NaN or +-448.  With the floor, the reciprocal is at most 2^126 and every code stays finite.
+__device__ __forceinline__ float e4m3_scale(float amax) { return amax > 0.f ? fmaxf(amax / E4M3_MAX, 0x1p-126f) : 1.f; }
+
 __device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
   return static_cast<uint16_t>(__nv_cvt_float2_to_fp8x2(make_float2(lo, hi), __NV_SATFINITE, __NV_E4M3));
 }
@@ -51,7 +56,7 @@ __global__ void quant_rowwise_kernel(const __nv_bfloat16* __restrict__ x, uint8_
     for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(v[i]));
   }
   amax = warp_max(amax);
-  const float s = amax > 0.f ? amax / E4M3_MAX : 1.f;
+  const float s = e4m3_scale(amax);
   const float inv = 1.f / s;
   if (lane == 0) scale[row] = s;
   uint8_t* qr = q + row * K;
@@ -124,8 +129,7 @@ __global__ void quant_colwise_t_kernel(const __nv_bfloat16* __restrict__ x, cons
     qt += g * pl.q_plane;
   }
   auto put_scale = [&](int e) {
-    const float a = amax[static_cast<long long>(e) * C + c];
-    scale[static_cast<long long>(e) * C + c] = a > 0.f ? a / E4M3_MAX : 1.f;
+    scale[static_cast<long long>(e) * C + c] = e4m3_scale(amax[static_cast<long long>(e) * C + c]);
   };
   if (blockIdx.y == 0 && c < C) {
     if (segments) {
@@ -136,8 +140,7 @@ __global__ void quant_colwise_t_kernel(const __nv_bfloat16* __restrict__ x, cons
   }
   float inv = 0.f;
   if (c < C && g >= 0) {
-    const float a = amax[static_cast<long long>(g) * C + c];
-    inv = 1.f / (a > 0.f ? a / E4M3_MAX : 1.f);
+    inv = 1.f / e4m3_scale(amax[static_cast<long long>(g) * C + c]);
   }
   for (int i = ty; i < 64; i += 4) {
     const long long r = r0 + i;
@@ -228,7 +231,7 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
       for (int j = 0; j < 8; ++j) a = fmaxf(a, fabsf(v[i][j]));
 #pragma unroll
       for (int o = 1; o < 16; o <<= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));  // the 16 threads of the row
-      const float sc = a > 0.f ? a / E4M3_MAX : 1.f;
+      const float sc = e4m3_scale(a);
       inv_r[i] = 1.f / sc;
       const long long r = r0 + 8 * ty + i;
       if (tx == 0 && r < R) s[static_cast<long long>(blockIdx.x) * lds + r] = sc;
@@ -248,7 +251,7 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
       float a = 0.f;
 #pragma unroll
       for (int w = 0; w < 8; ++w) a = fmaxf(a, red[w][8 * tx + j]);
-      const float sc = a > 0.f ? a / E4M3_MAX : 1.f;
+      const float sc = e4m3_scale(a);
       inv_c[j] = 1.f / sc;
       if (ty == 0 && cc + j < C) s[static_cast<long long>(blockIdx.y) * lds + cc + j] = sc;
     }
@@ -263,7 +266,7 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
     __syncthreads();
 #pragma unroll
     for (int w = 0; w < 8; ++w) a = fmaxf(a, red[w][0]);
-    const float sc = a > 0.f ? a / E4M3_MAX : 1.f;
+    const float sc = e4m3_scale(a);
     inv_r[0] = 1.f / sc;
     // one scale per row (plain copy) or per column (transposed copy) of the block: 128 values, 256 threads
     if (threadIdx.x < 128) {

@@ -1,6 +1,9 @@
 // d9d_b200 — persistent warp-specialised wgmma GEMM for 8-bit floating point operands (sm_90a).
 //
-//   D[M,N] (bf16) = scale( A[M,K] · B[N,K]^T )       A, B: e4m3, K-major; fp32 accumulation in registers.
+//   D[M,N] (bf16) = scale( A[M,K] · B[N,K]^T )       A, B: e4m3, K-major.
+// The tensor core sums each MMA chain in a reduced-precision accumulator (the tests model it with a unit roundoff of
+// 2^-13); fp32 registers hold only what the kernel adds outside a chain.  ROWCOL / MX DENSE: one chain over all of K (ROWCOL) or per
+// 32-deep MMA (MX); BLOCKWISE and the grouped modes: one chain per 128-deep k-block (promoted accumulation).
 //
 // Two scaling recipes share the mainloop:
 //   ROWCOL  D = acc * scale_a[row] * scale_b[col]  (per-token / per-output-channel or per-tensor scales, applied in the
@@ -15,6 +18,10 @@
 //           fp32 accumulator with its row x column scale (promoted accumulation); bf16 or fp32 output.
 // Same structure as the bf16 kernel (gemm_sm90.cuh): warpgroup 0 = TMA producer, warpgroups 1-2 = wgmma + epilogue over
 // 64 rows each (registers -> swizzled smem -> TMA store); a stage holds 128 bytes of K (= 128 fp8 elements = 4 MMAs).
+//
+// Every epilogue applies the row and the column scale one at a time, (acc * sa) * sb, never acc * (sa * sb): the library
+// builds with fast math (flush to zero), and the product of two small scales flushes to 0 below 2^-126 even when the result
+// is a normal number.  With sb <= 1 (quantiser scales are amax / 448) an intermediate flushes only when the result does.
 //
 // Three problem shapes (gemm::Mode, with the bf16 kernel's tile walk, gemm::get_tile), all K-major:
 //   DENSE      D[M,N] bf16
@@ -208,7 +215,7 @@ __device__ __forceinline__ void grouped_tiles(const CUtensorMap& tmap_a, const C
           for (int e = 0; e < 2; ++e) {
             const int col = col0 + 8 * j + cq + e;
             const float cs = col < p.N ? scale_b[col] : 0.f;
-            acc[4 * j + 2 * h + e] *= row_scale * cs;
+            acc[4 * j + 2 * h + e] = acc[4 * j + 2 * h + e] * row_scale * cs;  // one scale at a time: see the header
           }
         }
       }
@@ -365,10 +372,10 @@ __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const
         if (lane == 0) mbar_arrive(&empty_bar[stage]);
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 8; ++j) {
-          acc[4 * j] = fmaf(part[4 * j], sa0 * sbj[j].x, acc[4 * j]);
-          acc[4 * j + 1] = fmaf(part[4 * j + 1], sa0 * sbj[j].y, acc[4 * j + 1]);
-          acc[4 * j + 2] = fmaf(part[4 * j + 2], sa1 * sbj[j].x, acc[4 * j + 2]);
-          acc[4 * j + 3] = fmaf(part[4 * j + 3], sa1 * sbj[j].y, acc[4 * j + 3]);
+          acc[4 * j] = fmaf(part[4 * j] * sa0, sbj[j].x, acc[4 * j]);
+          acc[4 * j + 1] = fmaf(part[4 * j + 1] * sa0, sbj[j].y, acc[4 * j + 1]);
+          acc[4 * j + 2] = fmaf(part[4 * j + 2] * sa1, sbj[j].x, acc[4 * j + 2]);
+          acc[4 * j + 3] = fmaf(part[4 * j + 3] * sa1, sbj[j].y, acc[4 * j + 3]);
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
@@ -541,8 +548,8 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
                 for (int e = 0; e < 2; ++e) {
                   const int n = 8 * j + cq + e;
                   const float sb = ue8m0(sfb[(n / 128) * SF_BLOCK_BYTES + (n % 32) * 16 + ((n % 128) / 32) * 4 + k]);
-                  acc[4 * j + e] = fmaf(part[4 * j + e], sa[0] * sb, acc[4 * j + e]);
-                  acc[4 * j + 2 + e] = fmaf(part[4 * j + 2 + e], sa[1] * sb, acc[4 * j + 2 + e]);
+                  acc[4 * j + e] = fmaf(part[4 * j + e] * sa[0], sb, acc[4 * j + e]);
+                  acc[4 * j + 2 + e] = fmaf(part[4 * j + 2 + e] * sa[1], sb, acc[4 * j + 2 + e]);
                 }
               }
             }
@@ -571,15 +578,14 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = rbase + (lane >> 2) + 8 * h;
-            float row_scale = p.scale_scalar;
-            if (p.scale_a != nullptr && row < p.M) row_scale *= p.scale_a[row];
+            const float row_scale = (p.scale_a != nullptr && row < p.M) ? p.scale_a[row] : 1.f;
 #pragma unroll
             for (int j = 0; j < BLOCK_N / 8; ++j) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const int col = col0 + 8 * j + cq + e;
                 const float cs = (p.scale_b != nullptr && col < p.N) ? p.scale_b[col] : 1.f;
-                acc[4 * j + 2 * h + e] *= row_scale * cs;
+                acc[4 * j + 2 * h + e] = acc[4 * j + 2 * h + e] * row_scale * cs * p.scale_scalar;
               }
             }
           }

@@ -1,5 +1,5 @@
-"""FP8 wgmma kernels (e4m3 with epilogue scales, MXFP8 block scales) and their quantisers against fp32
-PyTorch references of the same operations."""
+"""FP8 wgmma kernels (e4m3 with epilogue scales, MXFP8 block scales) and their quantisers against their PyTorch
+emulations, norm-wise.  The per-element checks against fp64 models are in ``test_fp8_kernels_gpu.py``."""
 
 import pytest
 import torch
@@ -28,7 +28,8 @@ def test_quantize_rowwise(ops, M, K):
     q, s = ops.quantize_rowwise(x)
     qr, sr = fp8.quantize_rowwise_reference(x)
     assert torch.allclose(s, sr, rtol=1e-6, atol=0)
-    # the kernel multiplies by 1/s: at most one e4m3 step away from the division-based reference, and only rarely
+    # the kernel multiplies by a fast-math 1/s: at most one e4m3 step away from the division-based reference, and only
+    # rarely (the exact admissible-code check is in test_fp8_kernels_gpu.py)
     assert (q.float() != qr.float()).float().mean().item() < 0.02
     assert _rel(q.float() * s[:, None], x) < 0.04
 
@@ -69,7 +70,8 @@ def test_gemm_fp8_rowcol(ops, M, N, K, scales):
     else:
         ops.gemm_fp8(aq, bq, None, None, 0.5, d)
         ref = (aq.float() @ bq.float().t()) * 0.5
-    assert _rel(d, ref) < 5e-3  # the products of e4m3 values are exact in fp32: only the bf16 output rounding remains
+    # one reduced-precision tensor-core chain over K (about 2^-13 per addition, unpromoted) and the bf16 output rounding
+    assert _rel(d, ref) < 5e-3
     if scales == "both":
         assert _rel(d, a.float() @ b.float().t()) < 0.06  # end-to-end quantisation error of the recipe
 

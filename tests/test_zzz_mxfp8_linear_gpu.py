@@ -1,5 +1,5 @@
 """MXFP8 recipe of ``Fp8Linear`` (forward, dgrad and wgrad quantised along their own reduction dimensions) on the GPU against
-its CPU emulation.  Collected last on purpose: the composition was written after the round's GPU budget was spent."""
+its CPU emulation and against fp64."""
 
 import pytest
 import torch
@@ -13,8 +13,7 @@ def _rel(a, b):
     a, b = a.float(), b.float()
     return ((a - b).norm() / (b.norm() + 1e-12)).item()
 
-@pytest.mark.xfail(strict=False, reason="composition of GPU-verified ops (quantize_mx, gemm_mxfp8) written after the round's GPU budget "
-                                        "was spent: first executed by the round-end run")
+
 def test_mxfp8_linear_function_matches_emulation():
     torch.manual_seed(0)
     x = torch.randn(4, 256, 512, device="cuda").bfloat16().requires_grad_()  # 1024 tokens
@@ -28,4 +27,9 @@ def test_mxfp8_linear_function_matches_emulation():
     assert _rel(y.cpu(), yc) < 2e-2
     assert _rel(x.grad.cpu(), xc.grad) < 2e-2
     assert _rel(w.grad.cpu(), wc.grad) < 2e-2
-    assert _rel(y, x.detach().float() @ w.detach().float().t()) < 0.06
+    xd, wd = x.detach().double().requires_grad_(), w.detach().double().requires_grad_()
+    yd = xd @ wd.t()
+    yd.backward(g.double())
+    errs = (_rel(y, yd), _rel(x.grad, xd.grad), _rel(w.grad, wd.grad))
+    print(f"mxfp8 linear: rel err y / dx / dW = {errs[0]:.2e} / {errs[1]:.2e} / {errs[2]:.2e}")
+    assert max(errs) < 0.06
