@@ -4,16 +4,17 @@ Three operand recipes.  The tensor core sums an MMA chain in a reduced-precision
 chains are sets the accuracy of a long reduction:
 
 * **row / column scaling**: one fp32 scale per row of each operand (per token / per output channel), applied to the
-  accumulator in the GEMM epilogue; the whole of K is one chain (no promotion).  Used by :class:`Fp8LinearFunction`
-  for all three GEMMs of a linear layer (forward, input gradient, weight gradient); the two backward GEMMs need K-major
-  operands along the *other* dimension, which the transposing column-wise quantiser produces in one pass.
+  accumulator in the GEMM epilogue; the whole of K is one chain (no promotion).  The default recipe of
+  :class:`Fp8LinearFunction` for all three GEMMs of a linear layer (forward, input gradient, weight gradient); the two
+  backward GEMMs need K-major operands along the *other* dimension, which the transposing column-wise quantiser produces
+  in one pass.
 * **MXFP8**: OCP micro-scaling - one power-of-two (UE8M0) scale per 32 consecutive
   K-elements; every K=32 wgmma produces a partial product that is added to an fp32 accumulator with its two scales.
 * **blockwise** (DeepSeek-V3): one fp32 scale per 1x128 group of an activation row and per 128x128 block of a weight,
   both along the reduction dimension.  Every 128-deep k-block of the GEMM is summed by the tensor core into a fresh
   accumulator and added to the fp32 accumulator with its row x column scale ("promotion"), so one outlier only sets the
   scale of its own group and the accumulation is never one long reduced-precision chain.  Scales are stored
-  k-block-major, ``[ceil(K/128), rows]``.  Used by :class:`BlockwiseFp8LinearFunction`; the weight gradient is written
+  k-block-major, ``[ceil(K/128), rows]``.  In the linear layer (``recipe="blockwise"``) the weight gradient is written
   by the GEMM in the gradient dtype (fp32 or bf16).
 
 The reference framework has no fp8 path of its own (its published fp8 numbers come from torchao-style recipes layered on
@@ -23,7 +24,7 @@ runs on CPU and is the numerical oracle of the GPU tests.
 
 from __future__ import annotations
 
-from typing import Any
+from typing import Any, Callable, NamedTuple
 
 import torch
 from torch import nn
@@ -208,24 +209,103 @@ def blockwise_mm(aq: torch.Tensor, sa: torch.Tensor, bq: torch.Tensor, sb: torch
     return blockwise_mm_reference(aq, sa, bq, sb, out_dtype)
 
 
+class _Recipe(NamedTuple):
+    """One fp8 recipe of the dense linear layer: its size rule and its three GEMMs."""
+
+    granule: int  # the feature sizes must be multiples of it
+    tokens_too: bool  # ... and so must the token count
+    forward: Callable[[torch.Tensor, torch.Tensor], torch.Tensor]  # (x2, w) -> y2
+    dgrad: Callable[[torch.Tensor, torch.Tensor], torch.Tensor]  # (dy, w) -> dx2
+    wgrad: Callable[[torch.Tensor, torch.Tensor, torch.dtype], torch.Tensor]  # (dy, x2, grad_dtype) -> dW
+
+
+# row / column scaling:
+#   forward  y  = Q_row(x)  · Q_row(W)^T        scales: token x output channel
+#   dgrad    dx = Q_row(dy) · Q_colT(W)^T       Q_colT(W) = W^T stored [in, out], scale per input channel
+#   wgrad    dW = Q_colT(dy) · Q_colT(x)^T      both transposed copies come from the transposing quantiser
+def _rowwise_forward(x2, w):
+    xq, sx = quantize_rowwise(x2)
+    wq, sw = quantize_rowwise(w)
+    return scaled_mm(xq, sx, wq, sw)
+
+
+def _rowwise_dgrad(dy, w):
+    dyq, sdy = quantize_rowwise(dy)
+    wtq, swt = quantize_colwise_t(w)  # [in, out]
+    return scaled_mm(dyq, sdy, wtq, swt)
+
+
+def _rowwise_wgrad(dy, x2, grad_dtype):
+    dytq, sdyt = quantize_colwise_t(dy)  # [out, tokens]
+    xtq, sxt = quantize_colwise_t(x2)  # [in, tokens]
+    return scaled_mm(dytq, sdyt, xtq, sxt).to(grad_dtype)
+
+
+# MXFP8 (e4m3 elements, one power-of-two scale per 32 elements of the reduction dimension, applied to the K=32 partial
+# products of the GEMM).  Every GEMM quantises both operands along its own reduction dimension, so the backward GEMMs work
+# on transposed copies:
+#   forward  y  = MX(x)[M,K]    · MX(W)[N,K]^T          reduction over in
+#   dgrad    dx = MX(dy)[M,N]   · MX(W^T)[K,N]^T        reduction over out
+#   wgrad    dW = MX(dy^T)[N,M] · MX(x^T)[K,M]^T        reduction over tokens
+# in, out and the token count must be multiples of 128 (one scale-factor block of the tensor core).
+def _mx_dgrad(dy, w):
+    return mx_mm(dy, w.t().contiguous())
+
+
+def _mx_wgrad(dy, x2, grad_dtype):
+    return mx_mm(dy.t().contiguous(), x2.t().contiguous()).to(grad_dtype)
+
+
+# DeepSeek-V3's blockwise scaling with promoted accumulation:
+#   forward  y  = Q_blk(x)  · Q_W(W)^T           x: 1x128 groups along in; W: 128x128 blocks
+#   dgrad    dx = Q_blk(dy) · Q_W(W^T)^T         dy: 1x128 groups along out; the transposed copy of W's blocks
+#   wgrad    dW = Q_blkT(dy) · Q_blkT(x)^T       128-token groups of every channel, written in the gradient dtype
+# Feature sizes must be multiples of 16; the token count is free.
+def _blockwise_forward(x2, w):
+    xq, sx = quantize_blockwise(x2)
+    wq, sw = quantize_weight_blocks(w)
+    return blockwise_mm(xq, sx, wq, sw)
+
+
+def _blockwise_dgrad(dy, w):
+    dyq, sdy = quantize_blockwise(dy)
+    wtq, swt = quantize_weight_blocks(w, transpose=True)  # [in, out]
+    return blockwise_mm(dyq, sdy, wtq, swt)
+
+
+def _blockwise_wgrad(dy, x2, grad_dtype):
+    dytq, sdyt = quantize_blockwise_t(dy)  # [out, tokens]
+    xtq, sxt = quantize_blockwise_t(x2)  # [in, tokens]
+    return blockwise_mm(dytq, sdyt, xtq, sxt, out_dtype=grad_dtype)
+
+
+_LINEAR_RECIPES = {
+    "rowwise": _Recipe(16, False, _rowwise_forward, _rowwise_dgrad, _rowwise_wgrad),
+    "mx": _Recipe(128, True, mx_mm, _mx_dgrad, _mx_wgrad),
+    "blockwise": _Recipe(16, False, _blockwise_forward, _blockwise_dgrad, _blockwise_wgrad),
+}
+
+
+def _linear_recipe(recipe: str) -> _Recipe:
+    if recipe not in _LINEAR_RECIPES:
+        raise ValueError(f"unknown fp8 recipe {recipe!r}")
+    return _LINEAR_RECIPES[recipe]
+
+
 class Fp8LinearFunction(Function):
-    """``y = x @ W^T`` with all three GEMMs in e4m3 (dynamic row / column scaling, bf16 in / out).
-
-    forward  ``y  = Q_row(x)  · Q_row(W)^T``        scales: token x output channel
-    dgrad    ``dx = Q_row(dy) · Q_colT(W)^T``       ``Q_colT(W)`` = ``W^T`` stored [in, out], scale per input channel
-    wgrad    ``dW = Q_colT(dy) · Q_colT(x)^T``      both transposed copies come from the transposing quantiser
-    """
+    """``y = x @ W^T`` with all three GEMMs (forward, input gradient, weight gradient) in e4m3, bf16 in / out, under
+    ``recipe`` (default ``"rowwise"``).  Nothing quantised is kept between forward and backward: the backward quantises
+    again from the saved bf16 ``x`` and ``W``."""
 
     @staticmethod
-    def forward(ctx: Any, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    def forward(ctx: Any, x: torch.Tensor, weight: torch.Tensor, recipe: str = "rowwise") -> torch.Tensor:
         x2 = x.reshape(-1, x.shape[-1])
         if not x2.is_contiguous():
             x2 = x2.contiguous()
-        xq, sx = quantize_rowwise(x2)
-        wq, sw = quantize_rowwise(weight)
+        ctx.recipe = _linear_recipe(recipe)
         ctx.save_for_backward(x2, weight)
         ctx.x_shape = x.shape
-        return scaled_mm(xq, sx, wq, sw).view(*x.shape[:-1], weight.shape[0])
+        return ctx.recipe.forward(x2, weight).view(*x.shape[:-1], weight.shape[0])
 
     @staticmethod
     def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
@@ -235,114 +315,27 @@ class Fp8LinearFunction(Function):
             dy = dy.contiguous()
         dx = dw = None
         if ctx.needs_input_grad[0] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.inputs):
-            dyq, sdy = quantize_rowwise(dy)
-            wtq, swt = quantize_colwise_t(weight)  # [in, out]
-            dx = scaled_mm(dyq, sdy, wtq, swt).view(ctx.x_shape)
+            dx = ctx.recipe.dgrad(dy, weight).view(ctx.x_shape)
         if ctx.needs_input_grad[1] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.weight):
-            dytq, sdyt = quantize_colwise_t(dy)  # [out, tokens]
-            xtq, sxt = quantize_colwise_t(x2)  # [in, tokens]
-            dw = scaled_mm(dytq, sdyt, xtq, sxt).to(grad_dtype_of(weight))
-        return dx, dw
-
-
-class MxFp8LinearFunction(Function):
-    """``y = x @ W^T`` with all three GEMMs in **MXFP8** (e4m3 elements, one power-of-two scale per 32 elements of the
-    reduction dimension, applied to the K=32 partial products of the GEMM).
-
-    Every GEMM quantises both operands along *its own* reduction dimension, so the backward GEMMs work on transposed copies:
-
-    forward  ``y  = MX(x)[M,K]    · MX(W)[N,K]^T``          reduction over ``in``
-    dgrad    ``dx = MX(dy)[M,N]   · MX(W^T)[K,N]^T``        reduction over ``out``
-    wgrad    ``dW = MX(dy^T)[N,M] · MX(x^T)[K,M]^T``        reduction over tokens
-
-    ``in``, ``out`` and the token count must be multiples of 128 (one scale-factor block of the tensor core).
-    """
-
-    @staticmethod
-    def forward(ctx: Any, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
-        ctx.save_for_backward(x2, weight)
-        ctx.x_shape = x.shape
-        return mx_mm(x2, weight).view(*x.shape[:-1], weight.shape[0])
-
-    @staticmethod
-    def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
-        x2, weight = ctx.saved_tensors
-        dy = grad_output.reshape(-1, grad_output.shape[-1])
-        if not dy.is_contiguous():
-            dy = dy.contiguous()
-        dx = dw = None
-        if ctx.needs_input_grad[0] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.inputs):
-            dx = mx_mm(dy, weight.t().contiguous()).view(ctx.x_shape)
-        if ctx.needs_input_grad[1] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.weight):
-            dw = mx_mm(dy.t().contiguous(), x2.t().contiguous()).to(grad_dtype_of(weight))
-        return dx, dw
-
-
-class BlockwiseFp8LinearFunction(Function):
-    """``y = x @ W^T`` with all three GEMMs in e4m3 with DeepSeek-V3's blockwise scaling and promoted accumulation.
-
-    forward  ``y  = Q_blk(x)  · Q_W(W)^T``           x: 1x128 groups along ``in``; W: 128x128 blocks
-    dgrad    ``dx = Q_blk(dy) · Q_W(W^T)^T``         dy: 1x128 groups along ``out``; the transposed copy of W's blocks
-    wgrad    ``dW = Q_blkT(dy) · Q_blkT(x)^T``       128-token groups of every channel, written in the gradient dtype
-
-    Nothing quantised is kept between forward and backward: the backward re-quantises ``x`` and ``W`` from the saved bf16
-    tensors, so the activation memory is that of the row-wise recipe.  Feature sizes must be multiples of 16; the token
-    count is free.
-    """
-
-    @staticmethod
-    def forward(ctx: Any, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
-        xq, sx = quantize_blockwise(x2)
-        wq, sw = quantize_weight_blocks(weight)
-        ctx.save_for_backward(x2, weight)
-        ctx.x_shape = x.shape
-        return blockwise_mm(xq, sx, wq, sw).view(*x.shape[:-1], weight.shape[0])
-
-    @staticmethod
-    def backward(ctx: Any, grad_output: torch.Tensor):  # type: ignore[override]
-        x2, weight = ctx.saved_tensors
-        dy = grad_output.reshape(-1, grad_output.shape[-1])
-        if not dy.is_contiguous():
-            dy = dy.contiguous()
-        dx = dw = None
-        if ctx.needs_input_grad[0] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.inputs):
-            dyq, sdy = quantize_blockwise(dy)
-            wtq, swt = quantize_weight_blocks(weight, transpose=True)  # [in, out]
-            dx = blockwise_mm(dyq, sdy, wtq, swt).view(ctx.x_shape)
-        if ctx.needs_input_grad[1] and GLOBAL_GRAD_CONTEXT.check_direction(GradDirection.weight):
-            dytq, sdyt = quantize_blockwise_t(dy)  # [out, tokens]
-            xtq, sxt = quantize_blockwise_t(x2)  # [in, tokens]
-            dw = blockwise_mm(dytq, sdyt, xtq, sxt, out_dtype=grad_dtype_of(weight))
-        return dx, dw
+            dw = ctx.recipe.wgrad(dy, x2, grad_dtype_of(weight))
+        return dx, dw, None
 
 
 def fp8_linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = None, recipe: str = "rowwise") -> torch.Tensor:
-    """``x @ weight^T (+ bias)`` in fp8.  ``recipe="rowwise"``: dynamic per-row / per-column fp32 scales
-    (:class:`Fp8LinearFunction`, feature sizes multiples of 16); ``recipe="mx"``: MXFP8 block scaling
-    (:class:`MxFp8LinearFunction`, feature sizes and token count multiples of 128); ``recipe="blockwise"``: DeepSeek-V3's
-    1x128 / 128x128 scaling with promoted accumulation (:class:`BlockwiseFp8LinearFunction`, feature sizes multiples of
-    16, any token count)."""
-    if recipe not in _RECIPES:
-        raise ValueError(f"unknown fp8 recipe {recipe!r}")
-    granule = _GRANULE[recipe]
+    """``x @ weight^T (+ bias)`` in fp8 (:class:`Fp8LinearFunction`).  ``recipe="rowwise"``: dynamic per-row / per-column
+    fp32 scales (feature sizes multiples of 16); ``recipe="mx"``: MXFP8 block scaling (feature sizes and token count
+    multiples of 128); ``recipe="blockwise"``: DeepSeek-V3's 1x128 / 128x128 scaling with promoted accumulation (feature
+    sizes multiples of 16, any token count)."""
+    r = _linear_recipe(recipe)
+    granule = r.granule
     tokens = x.numel() // max(x.shape[-1], 1)
-    if x.shape[-1] % granule or weight.shape[0] % granule or (recipe == "mx" and tokens % granule):
+    if x.shape[-1] % granule or weight.shape[0] % granule or (r.tokens_too and tokens % granule):
         raise ValueError(f"fp8_linear[{recipe}]: sizes must be multiples of {granule} (got in={x.shape[-1]}, out={weight.shape[0]}, "
                          f"tokens={tokens})")
     if on_gpu(x) and (x.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16):
         raise RuntimeError("fp8_linear: bf16 activations and weights required on CUDA")
-    out = _RECIPES[recipe].apply(x, weight)
+    out = Fp8LinearFunction.apply(x, weight, recipe)
     return out if bias is None else out + bias
-
-
-_RECIPES = {"rowwise": Fp8LinearFunction, "mx": MxFp8LinearFunction, "blockwise": BlockwiseFp8LinearFunction}
-_GRANULE = {"rowwise": 16, "mx": 128, "blockwise": 16}  # feature sizes (and, for "mx", the token count) must be multiples
 
 
 class Fp8Linear(nn.Linear):
@@ -362,9 +355,7 @@ def convert_linears_to_fp8(module: nn.Module, predicate=lambda name, m: True, re
     number converted."""
     from d9d_b200.module.block.linear import Linear as NativeLinear
 
-    if recipe not in _RECIPES:
-        raise ValueError(f"unknown fp8 recipe {recipe!r}")
-    granule = _GRANULE[recipe]
+    granule = _linear_recipe(recipe).granule
     n = 0
     for name, m in module.named_modules():
         if type(m) in (nn.Linear, NativeLinear) and m.in_features % granule == 0 and m.out_features % granule == 0 and predicate(name, m):
@@ -375,7 +366,7 @@ def convert_linears_to_fp8(module: nn.Module, predicate=lambda name, m: True, re
 
 
 __all__ = [
-    "BlockwiseFp8LinearFunction", "Fp8Linear", "Fp8LinearFunction", "MxFp8LinearFunction", "blockwise_mm", "blockwise_mm_reference",
+    "Fp8Linear", "Fp8LinearFunction", "blockwise_mm", "blockwise_mm_reference",
     "convert_linears_to_fp8", "dequantize_mx", "fp8_linear", "mx_mm", "mx_scale_exponent",
     "quantize_blockwise", "quantize_blockwise_reference", "quantize_blockwise_t", "quantize_blockwise_t_reference",
     "quantize_colwise_t", "quantize_colwise_t_batched_reference", "quantize_colwise_t_reference", "quantize_mx_reference",

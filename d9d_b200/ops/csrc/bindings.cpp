@@ -11,16 +11,18 @@
 
 #include "d9d_ops.h"
 
+using namespace d9d::gemm;  // the GEMM launch codes: Mode, Epi, Comm
+
 namespace {
 
 using at::Tensor;
 
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
-inline int dtype_code(const Tensor& t) {
-  if (t.scalar_type() == at::kBFloat16) return 0;
-  if (t.scalar_type() == at::kFloat) return 1;
-  if (t.scalar_type() == at::kHalf) return 2;
+inline d9d::DType dtype_code(const Tensor& t) {
+  if (t.scalar_type() == at::kBFloat16) return d9d::DTYPE_BF16;
+  if (t.scalar_type() == at::kFloat) return d9d::DTYPE_F32;
+  if (t.scalar_type() == at::kHalf) return d9d::DTYPE_F16;
   TORCH_CHECK(false, "d9d_b200: unsupported dtype ", t.scalar_type());
 }
 
@@ -31,10 +33,10 @@ inline int dtype_code(const Tensor& t) {
   TORCH_CHECK(reinterpret_cast<uintptr_t>((t).data_ptr()) % 16 == 0, #t " must start on a 16-byte boundary")
 
 // ------------------------------------------------------------------ GEMM ------------------------
-int epi_for(const Tensor& d, bool accumulate) {
-  if (d.scalar_type() == at::kBFloat16) return accumulate ? 3 : 0;
+Epi epi_for(const Tensor& d, bool accumulate) {
+  if (d.scalar_type() == at::kBFloat16) return accumulate ? EPI_BF16_ACC : EPI_BF16;
   TORCH_CHECK(d.scalar_type() == at::kFloat, "gemm output must be bf16 or fp32");
-  return accumulate ? 2 : 1;
+  return accumulate ? EPI_F32_ACC : EPI_F32;
 }
 
 // block_n: output tile width (0 = the heuristic's choice). Single-CTA dense and grouped kernels are built for 128, 192 and
@@ -55,7 +57,7 @@ void gemm(const Tensor& a, const Tensor& b, Tensor d, bool a_mn, bool b_mn, bool
   TORCH_CHECK(a.stride(1) == 1 && b.stride(1) == 1 && d.stride(1) == 1, "gemm: innermost stride must be 1");
   c10::cuda::CUDAGuard guard(a.device());
   d9d::GemmArgs g;
-  g.mode = 0;
+  g.mode = DENSE;
   g.a_mn = a_mn; g.b_mn = b_mn;
   g.M = static_cast<int>(a_mn ? a.size(1) : a.size(0));
   g.K = static_cast<int>(a_mn ? a.size(0) : a.size(1));
@@ -70,7 +72,7 @@ void gemm(const Tensor& a, const Tensor& b, Tensor d, bool a_mn, bool b_mn, bool
   const bool pair = ctas == 2 || (ctas == 0 && d9d::gemm_pair_mode() == 1 && d9d::gemm_pair_eligible(g));
   check_block_n(block_n, !pair, pair ? "gemm (CTA pair)" : "gemm");
   TORCH_CHECK(k_splits >= 0, "gemm: k_splits must be >= 0");
-  TORCH_CHECK(k_splits <= 1 || g.epi == 2, "gemm: k_splits needs an fp32 output with accumulate=True");
+  TORCH_CHECK(k_splits <= 1 || g.epi == EPI_F32_ACC, "gemm: k_splits needs an fp32 output with accumulate=True");
   g.block_n = static_cast<int>(block_n);
   g.k_splits = static_cast<int>(k_splits);
   d9d::gemm_dense(g, cur_stream());
@@ -86,7 +88,7 @@ void gemm_grouped_m(const Tensor& a, const Tensor& b, Tensor d, const Tensor& ti
   TORCH_CHECK(tile_group.scalar_type() == at::kInt && a.size(0) % 128 == 0 && tile_group.numel() == a.size(0) / 128);
   c10::cuda::CUDAGuard guard(a.device());
   d9d::GemmArgs g;
-  g.mode = 1; g.epi = accumulate ? 3 : 0; g.a_mn = false; g.b_mn = b_mn;
+  g.mode = GROUPED_M; g.epi = accumulate ? EPI_BF16_ACC : EPI_BF16; g.a_mn = false; g.b_mn = b_mn;
   g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1));
   g.N = static_cast<int>(b_mn ? b.size(2) : b.size(1));
   TORCH_CHECK((b_mn ? b.size(1) : b.size(2)) == g.K, "gemm_grouped_m: K mismatch");
@@ -108,7 +110,7 @@ void gemm_grouped_k(const Tensor& a, const Tensor& b, Tensor d, const Tensor& gr
   TORCH_CHECK(group_offsets.scalar_type() == at::kInt && a.size(0) == b.size(0));
   c10::cuda::CUDAGuard guard(a.device());
   d9d::GemmArgs g;
-  g.mode = 2; g.a_mn = true; g.b_mn = true;
+  g.mode = GROUPED_K; g.a_mn = true; g.b_mn = true;
   g.M = static_cast<int>(a.size(1)); g.N = static_cast<int>(b.size(1)); g.K = 0;
   g.k_total = a.size(0);
   g.num_groups = static_cast<int>(d.size(0));
@@ -137,7 +139,7 @@ std::tuple<Tensor, Tensor, Tensor> ce_forward_ex(const Tensor& h, const Tensor& 
   Tensor part_max = at::empty({n_tiles, T}, fopt), part_sum = at::empty({n_tiles, T}, fopt);
   Tensor tgt_logit = at::zeros({T}, fopt), lse = at::empty({T}, fopt), nll = at::empty({T}, fopt);
   d9d::GemmArgs g;
-  g.mode = 0; g.epi = 4;
+  g.mode = DENSE; g.epi = EPI_CE_LSE;
   g.M = T; g.N = V; g.K = K;
   g.A = h.data_ptr(); g.B = w.data_ptr(); g.lda = K; g.ldb = K; g.ldd = V;
   g.ce_target = reinterpret_cast<const long long*>(target.data_ptr<int64_t>());
@@ -195,7 +197,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> ce_forward_reg(const Tensor& h, const
   Tensor tgt_logit = at::zeros({T}, fopt), lse = at::empty({T}, fopt), nll = at::empty({T}, fopt);
   Tensor zsum = at::empty({T}, fopt);
   d9d::GemmArgs g;
-  g.mode = 0; g.epi = 6;
+  g.mode = DENSE; g.epi = EPI_CE_LSE_SUM;
   g.M = T; g.N = V; g.K = K;
   g.A = h.data_ptr(); g.B = w.data_ptr(); g.lda = K; g.ldb = K; g.ldd = V;
   g.ce_target = reinterpret_cast<const long long*>(target.data_ptr<int64_t>());
@@ -232,7 +234,7 @@ void ce_dlogits(const Tensor& h, const Tensor& w, const Tensor& target, const Te
   const int T = static_cast<int>(h.size(0)), K = static_cast<int>(h.size(1)), V = static_cast<int>(w.size(0));
   TORCH_CHECK(out.size(0) == T && out.size(1) == V);
   d9d::GemmArgs g;
-  g.mode = 0; g.epi = 5;
+  g.mode = DENSE; g.epi = EPI_CE_DLOGITS;
   g.M = T; g.N = V; g.K = K;
   g.A = h.data_ptr(); g.B = w.data_ptr(); g.D = out.data_ptr(); g.lda = K; g.ldb = K; g.ldd = out.stride(0);
   g.ce_target = reinterpret_cast<const long long*>(target.data_ptr<int64_t>());
@@ -270,7 +272,7 @@ void ce_dlogits_reg(const Tensor& h, const Tensor& w, const Tensor& target, cons
   c10::cuda::CUDAGuard guard(h.device());
   const int T = static_cast<int>(h.size(0)), K = static_cast<int>(h.size(1)), V = static_cast<int>(w.size(0));
   d9d::GemmArgs g;
-  g.mode = 0; g.epi = 7;
+  g.mode = DENSE; g.epi = EPI_CE_DLOGITS_REG;
   g.M = T; g.N = V; g.K = K;
   g.A = h.data_ptr(); g.B = w.data_ptr(); g.D = out.data_ptr(); g.lda = K; g.ldb = K; g.ldd = out.stride(0);
   g.ce_target = reinterpret_cast<const long long*>(target.data_ptr<int64_t>());
@@ -409,7 +411,7 @@ void gemm_mxfp8(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tenso
   const int64_t kb = g.K / 128;
   TORCH_CHECK(sfa.scalar_type() == at::kByte && sfa.numel() >= (static_cast<int64_t>(g.M) + 127) / 128 * kb * 512, "gemm_mxfp8: sfa too small");
   TORCH_CHECK(sfb.scalar_type() == at::kByte && sfb.numel() >= (static_cast<int64_t>(g.N) + 127) / 128 * kb * 512, "gemm_mxfp8: sfb too small");
-  g.block_scaled = true;
+  g.scaling = d9d::fp8::MX;
   g.sfa = sfa.data_ptr<uint8_t>(); g.sfb = sfb.data_ptr<uint8_t>();
   d9d::gemm_fp8(g, cur_stream());
 }
@@ -446,7 +448,7 @@ void gemm_fp8_grouped_m(const Tensor& a, const Tensor& sa, const Tensor& b, cons
   TORCH_CHECK(d.size(1) % 8 == 0, "gemm_fp8_grouped_m: N must be a multiple of 8 (16-byte output rows)");
   c10::cuda::CUDAGuard guard(a.device());
   d9d::Fp8GemmArgs g;
-  g.mode = 1; g.epi = accumulate ? 3 : 0;
+  g.mode = GROUPED_M; g.epi = accumulate ? EPI_BF16_ACC : EPI_BF16;
   g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1)); g.N = static_cast<int>(b.size(1));
   g.num_groups = static_cast<int>(b.size(0));
   g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
@@ -474,7 +476,7 @@ void gemm_fp8_grouped_k(const Tensor& a, const Tensor& sa, const Tensor& b, cons
   TORCH_CHECK(sb.numel() == d.size(0) * d.size(2), "gemm_fp8_grouped_k: sb must be [E * N]");
   c10::cuda::CUDAGuard guard(a.device());
   d9d::Fp8GemmArgs g;
-  g.mode = 2; g.epi = epi_for(d, accumulate);
+  g.mode = GROUPED_K; g.epi = epi_for(d, accumulate);
   g.M = static_cast<int>(a.size(0)); g.N = static_cast<int>(b.size(0)); g.K = 0;
   g.k_total = a.size(1);
   g.num_groups = static_cast<int>(d.size(0));
@@ -509,7 +511,7 @@ std::tuple<Tensor, Tensor> quantize_blockwise(const Tensor& x) {
   Tensor q = at::empty({M, K}, x.options().dtype(at::kFloat8_e4m3fn));
   Tensor s = blockwise_scales(x, (K + 127) / 128, M);
   d9d::quantize_blockwise_e4m3(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), M, static_cast<int>(K), x.stride(0), K, s.stride(0),
-                               0, false, cur_stream());
+                               d9d::GROUP_ROW, false, cur_stream());
   return {q, s};
 }
 
@@ -524,7 +526,7 @@ std::tuple<Tensor, Tensor> quantize_blockwise_t(const Tensor& x) {
   Tensor qt = at::empty({C, pitch}, x.options().dtype(at::kFloat8_e4m3fn));
   Tensor s = blockwise_scales(x, (M + 127) / 128, C);
   d9d::quantize_blockwise_e4m3(x.data_ptr(), qt.data_ptr(), s.data_ptr<float>(), M, static_cast<int>(C), x.stride(0), pitch, s.stride(0),
-                               1, true, cur_stream());
+                               d9d::GROUP_COL, true, cur_stream());
   return {qt.narrow(1, 0, M), s};
 }
 
@@ -538,7 +540,7 @@ std::tuple<Tensor, Tensor> quantize_weight_blocks(const Tensor& w, bool transpos
   Tensor q = transpose ? at::empty({K, N}, w.options().dtype(at::kFloat8_e4m3fn)) : at::empty({N, K}, w.options().dtype(at::kFloat8_e4m3fn));
   Tensor s = transpose ? blockwise_scales(w, (N + 127) / 128, K) : blockwise_scales(w, (K + 127) / 128, N);
   d9d::quantize_blockwise_e4m3(w.data_ptr(), q.data_ptr(), s.data_ptr<float>(), N, static_cast<int>(K), w.stride(0), q.stride(0),
-                               s.stride(0), 2, transpose, cur_stream());
+                               s.stride(0), d9d::GROUP_BLOCK, transpose, cur_stream());
   return {q, s};
 }
 
@@ -571,8 +573,8 @@ void gemm_fp8_blockwise(const Tensor& a, const Tensor& sa, const Tensor& b, cons
   check_blockwise_scales("sb", sb, a, kb, b.size(0));
   c10::cuda::CUDAGuard guard(a.device());
   d9d::Fp8GemmArgs g;
-  g.blockwise = true;
-  g.epi = d.scalar_type() == at::kBFloat16 ? 0 : 1;
+  g.scaling = d9d::fp8::BLOCKWISE;
+  g.epi = d.scalar_type() == at::kBFloat16 ? EPI_BF16 : EPI_F32;
   g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1)); g.N = static_cast<int>(b.size(0));
   g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
   g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(0);
@@ -1076,13 +1078,13 @@ void gemm_ag_a(at::IntArrayRef a_peer_ptrs, int64_t rows_local, int64_t lda, int
   c10::cuda::CUDAGuard guard(d.device());
   auto ptrs = to_ptrs(a_peer_ptrs);
   d9d::GemmArgs g;
-  g.mode = 0; g.a_mn = false; g.b_mn = b_mn; g.epi = 0;
+  g.mode = DENSE; g.a_mn = false; g.b_mn = b_mn; g.epi = EPI_BF16;
   g.M = static_cast<int>(d.size(0)); g.N = static_cast<int>(d.size(1));
   g.K = static_cast<int>(b_mn ? b.size(0) : b.size(1));
   TORCH_CHECK((b_mn ? b.size(1) : b.size(0)) == g.N, "gemm_ag_a: N mismatch");
   TORCH_CHECK(rows_local * static_cast<int64_t>(ptrs.size()) == g.M, "gemm_ag_a: shards do not add up to M");
   g.B = b.data_ptr(); g.D = d.data_ptr(); g.ldb = b.stride(0); g.ldd = d.stride(0);
-  g.comm = 1; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
+  g.comm = COMM_AG_A; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_peer_ptrs = ptrs.data(); g.comm_rows_local = rows_local; g.comm_ld = lda;
   check_block_n(block_n, false, "gemm_ag_a");
   g.block_n = static_cast<int>(block_n);
@@ -1099,13 +1101,13 @@ void gemm_wait_a(const Tensor& a, const Tensor& flags, int64_t rank, int64_t blo
   TORCH_CHECK(flags.is_cuda() && flags.scalar_type() == at::kInt && flags.is_contiguous());
   c10::cuda::CUDAGuard guard(d.device());
   d9d::GemmArgs g;
-  g.mode = 0; g.a_mn = false; g.b_mn = b_mn; g.epi = 0;
+  g.mode = DENSE; g.a_mn = false; g.b_mn = b_mn; g.epi = EPI_BF16;
   g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1));
   g.N = static_cast<int>(b_mn ? b.size(1) : b.size(0));
   TORCH_CHECK((b_mn ? b.size(0) : b.size(1)) == g.K && d.size(0) == g.M && d.size(1) == g.N, "gemm_wait_a: shape mismatch");
   g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
   g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(0);
-  g.comm = 5; g.comm_world = static_cast<int>(flags.numel()); g.comm_block_rows = static_cast<int>(block_rows);
+  g.comm = COMM_WAIT_A; g.comm_world = static_cast<int>(flags.numel()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_rank = static_cast<int>(rank); g.comm_flags = flags.data_ptr<int>();
   g.comm_spare_sms = static_cast<int>(spare_sms);
   check_block_n(block_n, false, "gemm_wait_a");
@@ -1121,13 +1123,13 @@ void gemm_rs_d(const Tensor& a, const Tensor& b, at::IntArrayRef d_peer_ptrs, in
   c10::cuda::CUDAGuard guard(a.device());
   auto ptrs = to_ptrs(d_peer_ptrs);
   d9d::GemmArgs g;
-  g.mode = 0; g.a_mn = false; g.b_mn = b_mn; g.epi = 3;
+  g.mode = DENSE; g.a_mn = false; g.b_mn = b_mn; g.epi = EPI_BF16_ACC;
   g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1));
   g.N = static_cast<int>(b_mn ? b.size(1) : b.size(0));
   TORCH_CHECK((b_mn ? b.size(0) : b.size(1)) == g.K, "gemm_rs_d: K mismatch");
   TORCH_CHECK(rows_local * static_cast<int64_t>(ptrs.size()) == g.M, "gemm_rs_d: shards do not add up to M");
   g.A = a.data_ptr(); g.B = b.data_ptr(); g.lda = a.stride(0); g.ldb = b.stride(0);
-  g.comm = 2; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
+  g.comm = COMM_RS_D; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_peer_ptrs = ptrs.data(); g.comm_rows_local = rows_local; g.comm_ld = ldd;
   check_block_n(block_n, false, "gemm_rs_d");
   g.block_n = static_cast<int>(block_n);
@@ -1142,7 +1144,7 @@ void gemm_ag_k(const Tensor& local, at::IntArrayRef peer_ptrs, bool peer_is_a, i
   c10::cuda::CUDAGuard guard(d.device());
   auto ptrs = to_ptrs(peer_ptrs);
   d9d::GemmArgs g;
-  g.mode = 0; g.a_mn = true; g.b_mn = true;
+  g.mode = DENSE; g.a_mn = true; g.b_mn = true;
   g.M = static_cast<int>(d.size(0)); g.N = static_cast<int>(d.size(1)); g.K = static_cast<int>(local.size(0));
   TORCH_CHECK(rows_local * static_cast<int64_t>(ptrs.size()) == g.K, "gemm_ag_k: shards do not add up to the token dim");
   TORCH_CHECK(local.size(1) == (peer_is_a ? g.N : g.M), "gemm_ag_k: local operand width mismatch");
@@ -1150,11 +1152,11 @@ void gemm_ag_k(const Tensor& local, at::IntArrayRef peer_ptrs, bool peer_is_a, i
   else { g.A = local.data_ptr(); g.lda = local.stride(0); }
   g.D = d.data_ptr(); g.ldd = d.stride(0);
   g.epi = epi_for(d, accumulate);
-  g.comm = peer_is_a ? 3 : 4; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
+  g.comm = peer_is_a ? COMM_AG_KA : COMM_AG_KB; g.comm_world = static_cast<int>(ptrs.size()); g.comm_block_rows = static_cast<int>(block_rows);
   g.comm_peer_ptrs = ptrs.data(); g.comm_rows_local = rows_local; g.comm_ld = peer_ld;
   check_block_n(block_n, false, "gemm_ag_k");
   TORCH_CHECK(k_splits >= 0, "gemm_ag_k: k_splits must be >= 0");
-  TORCH_CHECK(k_splits <= 1 || g.epi == 2, "gemm_ag_k: k_splits needs an fp32 output with accumulate=True");
+  TORCH_CHECK(k_splits <= 1 || g.epi == EPI_F32_ACC, "gemm_ag_k: k_splits needs an fp32 output with accumulate=True");
   g.block_n = static_cast<int>(block_n);
   g.k_splits = static_cast<int>(k_splits);
   d9d::gemm_comm(g, cur_stream());

@@ -8,9 +8,45 @@
 namespace d9d {
 
 // ------------------------------------------------------------------ GEMM (wgmma) -----------------
+// Launch codes of the GEMMs, named here once for the bindings and the launchers.  The kernels take them as int template
+// parameters, so their values are part of the kernels' symbol names.
+namespace gemm {
+
+enum Mode : int { DENSE = 0, GROUPED_M = 1, GROUPED_K = 2 };
+enum Epi : int {
+  EPI_BF16 = 0,       // D(bf16) = acc
+  EPI_F32 = 1,        // D(f32) = acc
+  EPI_F32_ACC = 2,    // D(f32) += acc
+  EPI_BF16_ACC = 3,   // D(bf16) += acc   TMA path: rn(D + rn_bf16(acc)), the add done in bf16 in L2;
+                      //                  direct-store path: rn(D + acc) with the add in fp32
+  EPI_CE_LSE = 4,     // fused linear-CE forward: per (row, n_tile) running max / sum-exp / target logit
+  EPI_CE_DLOGITS = 5, // fused linear-CE backward: D(bf16) = g[row] * (exp(acc - lse[row]) - [col == target[row]])
+  // regularised linear-CE (label smoothing eps, z-loss zeta over V classes in all):
+  EPI_CE_LSE_SUM = 6,    // EPI_CE_LSE + per (row, n_tile) sum of the tile's logits
+  EPI_CE_DLOGITS_REG = 7 // D(bf16) = g[row] * ((1 + 2 zeta lse[row]) p - (1 - eps) [col == target[row]] - eps / V)
+};
+
+// Tensor-parallel communication fused into the GEMM (operands / outputs living in NVLink peer memory):
+//   COMM_AG_A   A's rows (the M dim) are sharded over the peers: every m-tile is TMA-loaded straight from the owner's
+//               shard                                   => all-gather -> GEMM without a gathered copy of A
+//   COMM_RS_D   every output tile is TMA reduce-added into the shard of the peer that owns those rows
+//                                                        => GEMM -> reduce-scatter without a partial-sum buffer
+//   COMM_AG_KA / COMM_AG_KB   A / B (MN-major) is sharded along the *reduction* dim (wgrad of a sequence-parallel
+//               layer): every k-block is loaded from the owner's shard
+// Row index -> (owner, local row):  blk = idx / comm_block_rows; owner = blk % comm_world;
+//                                   local = (blk / comm_world) * comm_block_rows + idx % comm_block_rows
+// (covers both "tokens sharded as one contiguous block per rank" and "[batch, seq/W] per rank, batch-major").
+//   COMM_WAIT_A A is a *local* gathered buffer that is being filled shard by shard (peer copies running concurrently on
+//               the copy engines / another stream); the producer waits on the owner's arrival flag before the first
+//               load of an m-tile and tiles are visited starting with the local shard  => all-gather overlapped with
+//               the GEMM tile by tile while every remote byte crosses NVLink exactly once
+enum Comm : int { COMM_NONE = 0, COMM_AG_A = 1, COMM_RS_D = 2, COMM_AG_KA = 3, COMM_AG_KB = 4, COMM_WAIT_A = 5 };
+
+}  // namespace gemm
+
 struct GemmArgs {
-  int mode = 0;        // gemm::Mode
-  int epi = 0;         // gemm::Epi
+  gemm::Mode mode = gemm::DENSE;
+  gemm::Epi epi = gemm::EPI_BF16;
   bool a_mn = false;   // A stored [K, M] (M contiguous) instead of [M, K]
   bool b_mn = false;   // B stored [K, N] (N contiguous) instead of [N, K]
   const void* A = nullptr;
@@ -28,7 +64,7 @@ struct GemmArgs {
   int ctas = 0;                        // 1: one CTA per tile, 2: CTA pairs (cta_group::2, 256-row tiles), 0: process-wide policy
   int k_splits = 0;                    // dense fp32-accumulate epilogue only: 0 => heuristic, 1 => off
   // fused tensor-parallel communication (gemm::Comm); the sharded operand / output is described by its peers
-  int comm = 0;
+  gemm::Comm comm = gemm::COMM_NONE;
   int comm_world = 1;
   int comm_block_rows = 0;                     // rows per (rank, block) of the sharded dim
   const void* const* comm_peer_ptrs = nullptr; // host array [comm_world]: base pointer of every peer's shard
@@ -74,9 +110,17 @@ void ce_finalize_zsum(const float* part_max, const float* part_sum, const float*
                       float* zsum, cudaStream_t stream);
 
 // ------------------------------------------------------------------ fp8 GEMM (wgmma e4m3, MX block scales) -----
+namespace fp8 {
+enum Scaling : int { ROWCOL = 0, MX = 1, BLOCKWISE = 2 };
+}  // namespace fp8
+
 struct Fp8GemmArgs {
-  int mode = 0;              // gemm::Mode: DENSE, GROUPED_M (MoE forward / dgrad), GROUPED_K (MoE wgrad)
-  int epi = 0;               // gemm::Epi: bf16 store (dense); GROUPED_M: + bf16 accumulate; GROUPED_K: fp32 / bf16 store / accumulate
+  gemm::Mode mode = gemm::DENSE;  // DENSE, GROUPED_M (MoE forward / dgrad), GROUPED_K (MoE wgrad)
+  gemm::Epi epi = gemm::EPI_BF16; // bf16 store (dense); GROUPED_M: + bf16 accumulate; GROUPED_K: fp32 / bf16 store / accumulate;
+                                  // BLOCKWISE: bf16 or fp32 store
+  // ROWCOL: row / column scales in the epilogue; MX: UE8M0 scale per 32 K-elements (DENSE); BLOCKWISE: scale_a / scale_b
+  // are [ceil(K/128), round_up(M / N, 128)] per (k-block, row) scales (DENSE)
+  fp8::Scaling scaling = fp8::ROWCOL;
   const void* A = nullptr;   // [M, K] e4m3, K contiguous (row pitch lda bytes); GROUPED_K: [M, k_total]
   const void* B = nullptr;   // [N, K] e4m3; GROUPED_M: [E, N, K] (expert pitch b_group_stride bytes); GROUPED_K: [N, k_total]
   void* D = nullptr;         // [M, N] bf16; GROUPED_K: [E, M, N] (expert pitch d_group_stride elements)
@@ -87,14 +131,11 @@ struct Fp8GemmArgs {
   long long k_total = 0;               // GROUPED_K: rows of the grouped reduction dim
   const int* tile_group = nullptr;     // GROUPED_M: [M/128] expert per m-tile or -1
   const int* group_offsets = nullptr;  // GROUPED_K: [E+1] row offsets, multiples of 128
-  bool block_scaled = false;          // true: MXFP8 (UE8M0 scale per 32 K-elements), false: row / column scales in the epilogue
   const float* scale_a = nullptr;     // [M] or nullptr; GROUPED_K: [E, M]
   const float* scale_b = nullptr;     // [N] or nullptr; grouped: [E, N]
   float scale_scalar = 1.f;
   const uint8_t* sfa = nullptr;       // [ceil(M/128), K/128, 512]
   const uint8_t* sfb = nullptr;       // [ceil(N/128), K/128, 512]
-  bool blockwise = false;             // true: scale_a / scale_b are [ceil(K/128), round_up(M / N, 128)] per (k-block, row)
-                                      // scales (DENSE, epi bf16 or fp32 store)
 };
 void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream);
 void quantize_rowwise_e4m3(const void* x, void* q, float* scale, long long M, int K, long long ldx, cudaStream_t stream);
@@ -110,25 +151,27 @@ void quantize_segments_t_e4m3(const void* x, void* qt, float* scale, float* amax
                               cudaStream_t stream);
 // sf must be zero-initialised by the caller when M is not a multiple of 256 (pad blocks)
 void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long long ldx, cudaStream_t stream);
-// x[R, C] bf16 -> e4m3 with one fp32 scale (amax / 448, 1 for all-zero groups) per group: group 0 = 1 x 128 row groups
-// (q[R, C], s[ceil(C/128), lds]), 1 = 128 x 1 column groups (transposed qT[C, R] with pitch ldq >= R, zero pad columns,
-// s[ceil(R/128), lds]), 2 = 128 x 128 blocks (plain: s[ceil(C/128), lds] per row, transposed: s[ceil(R/128), lds] per
-// column of qT's rows).  lds is the scale row pitch, a multiple of 128 at least the scaled dimension.
+// x[R, C] bf16 -> e4m3 with one fp32 scale (amax / 448, 1 for all-zero groups) per group: GROUP_ROW = 1 x 128 row groups
+// (q[R, C], s[ceil(C/128), lds]), GROUP_COL = 128 x 1 column groups (transposed qT[C, R] with pitch ldq >= R, zero pad
+// columns, s[ceil(R/128), lds]), GROUP_BLOCK = 128 x 128 blocks (plain: s[ceil(C/128), lds] per row, transposed:
+// s[ceil(R/128), lds] per column of qT's rows).  lds is the scale row pitch, a multiple of 128 at least the scaled dimension.
+enum BlockGroup : int { GROUP_ROW = 0, GROUP_COL = 1, GROUP_BLOCK = 2 };
 void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, int C, long long ldx, long long ldq, long long lds,
-                             int group, bool transpose, cudaStream_t stream);
+                             BlockGroup group, bool transpose, cudaStream_t stream);
 
 // ------------------------------------------------------------------ normalisation ----------------
-// dtype codes: 0 = bf16, 1 = fp32, 2 = fp16
+// element type of the normalisation, activation and grad-utility launchers
+enum DType : int { DTYPE_BF16 = 0, DTYPE_F32 = 1, DTYPE_F16 = 2 };
 void rms_norm_fwd(const void* x, const void* w, void* out, float* inv_rms, long long M, int N, float eps,
-                  bool zero_centered, int dtype, cudaStream_t stream);
+                  bool zero_centered, DType dtype, cudaStream_t stream);
 // dw_partial: [rms_norm_bwd_num_partials(), N] fp32 scratch; dw: [N] in dtype
 int rms_norm_bwd_num_partials();
 void rms_norm_bwd(const void* dout, const void* x, const void* w, const float* inv_rms, void* dx, void* dw,
-                  float* dw_partial, long long M, int N, bool zero_centered, int dtype, cudaStream_t stream);
+                  float* dw_partial, long long M, int N, bool zero_centered, DType dtype, cudaStream_t stream);
 
 // ------------------------------------------------------------------ activations ------------------
-void silu_mul_fwd(const void* x, const void* y, void* out, long long n, int dtype, cudaStream_t stream);
-void silu_mul_bwd(const void* dout, const void* x, const void* y, void* dx, void* dy, long long n, int dtype,
+void silu_mul_fwd(const void* x, const void* y, void* out, long long n, DType dtype, cudaStream_t stream);
+void silu_mul_bwd(const void* dout, const void* x, const void* y, void* dx, void* dy, long long n, DType dtype,
                   cudaStream_t stream);
 // MoE variant: out[r, :] = silu(x) * y * probs[r];  bwd also yields dprobs[r]
 void silu_mul_probs_fwd(const void* x, const void* y, const float* probs, void* out, long long rows, int cols,
@@ -183,10 +226,10 @@ void moe_permute_bwd(const void* dxp, const float* dpp, const int* row_map, void
                      int k, int H, cudaStream_t stream);
 
 // ------------------------------------------------------------------ grad utilities ---------------
-// out[0] += sum(x^2) over a flat fp32/bf16 buffer (dtype code as above)
-void sumsq_accumulate(const void* x, long long n, int dtype, float* out, cudaStream_t stream);
+// out[0] += sum(x^2) over a flat fp32/bf16 buffer
+void sumsq_accumulate(const void* x, long long n, DType dtype, float* out, cudaStream_t stream);
 // x *= *scale (device scalar)
-void scale_inplace(void* x, long long n, int dtype, const float* scale, cudaStream_t stream);
+void scale_inplace(void* x, long long n, DType dtype, const float* scale, cudaStream_t stream);
 
 // ------------------------------------------------------------------ flash attention (forward / backward) --
 // q / dq [total_q, Hq, Dqk], out / dout [total_q, Hq, Dv], k / dk [total_k, Hk, Dqk], v / dv [total_k, Hk, Dv] bf16

@@ -568,19 +568,19 @@ void rms_bwd_block_launch(const void* dout, const void* x, const void* w, const 
 int rms_norm_bwd_num_partials() { return num_sms() * 8; }
 
 void rms_norm_fwd(const void* x, const void* w, void* out, float* inv_rms, long long M, int N, float eps,
-                  bool zero_centered, int dtype, cudaStream_t stream) {
+                  bool zero_centered, DType dtype, cudaStream_t stream) {
   if (M == 0) return;
   if (N % 8 != 0) throw std::runtime_error("d9d rms_norm: N must be a multiple of 8");
-  if (dtype == 0) D9D_RMS_FWD_DISPATCH(__nv_bfloat16, x, w, out, inv_rms, M, N, eps, zero_centered, stream);
-  else if (dtype == 1) D9D_RMS_FWD_DISPATCH(float, x, w, out, inv_rms, M, N, eps, zero_centered, stream);
+  if (dtype == DTYPE_BF16) D9D_RMS_FWD_DISPATCH(__nv_bfloat16, x, w, out, inv_rms, M, N, eps, zero_centered, stream);
+  else if (dtype == DTYPE_F32) D9D_RMS_FWD_DISPATCH(float, x, w, out, inv_rms, M, N, eps, zero_centered, stream);
   else D9D_RMS_FWD_DISPATCH(__half, x, w, out, inv_rms, M, N, eps, zero_centered, stream);
 }
 
 void rms_norm_bwd(const void* dout, const void* x, const void* w, const float* inv_rms, void* dx, void* dw,
-                  float* dw_partial, long long M, int N, bool zero_centered, int dtype, cudaStream_t stream) {
+                  float* dw_partial, long long M, int N, bool zero_centered, DType dtype, cudaStream_t stream) {
   if (N % 8 != 0) throw std::runtime_error("d9d rms_norm: N must be a multiple of 8");
-  if (dtype == 0) D9D_RMS_BWD_DISPATCH(__nv_bfloat16, dout, x, w, inv_rms, dx, dw, dw_partial, M, N, zero_centered, stream);
-  else if (dtype == 1) D9D_RMS_BWD_DISPATCH(float, dout, x, w, inv_rms, dx, dw, dw_partial, M, N, zero_centered, stream);
+  if (dtype == DTYPE_BF16) D9D_RMS_BWD_DISPATCH(__nv_bfloat16, dout, x, w, inv_rms, dx, dw, dw_partial, M, N, zero_centered, stream);
+  else if (dtype == DTYPE_F32) D9D_RMS_BWD_DISPATCH(float, dout, x, w, inv_rms, dx, dw, dw_partial, M, N, zero_centered, stream);
   else D9D_RMS_BWD_DISPATCH(__half, dout, x, w, inv_rms, dx, dw, dw_partial, M, N, zero_centered, stream);
 }
 
@@ -716,20 +716,20 @@ __global__ void __launch_bounds__(256) silu_mul_probs_bwd_kernel(
 
 }  // namespace
 
-void silu_mul_fwd(const void* x, const void* y, void* out, long long n, int dtype, cudaStream_t s) {
+void silu_mul_fwd(const void* x, const void* y, void* out, long long n, DType dtype, cudaStream_t s) {
   if (n == 0) return;
   const int grid = ew_grid(n >> 3);
-  if (dtype == 0) silu_mul_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)y, (__nv_bfloat16*)out, n);
-  else if (dtype == 1) silu_mul_fwd_kernel<float><<<grid, 256, 0, s>>>((const float*)x, (const float*)y, (float*)out, n);
+  if (dtype == DTYPE_BF16) silu_mul_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)y, (__nv_bfloat16*)out, n);
+  else if (dtype == DTYPE_F32) silu_mul_fwd_kernel<float><<<grid, 256, 0, s>>>((const float*)x, (const float*)y, (float*)out, n);
   else silu_mul_fwd_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, (const __half*)y, (__half*)out, n);
 }
 
-void silu_mul_bwd(const void* dout, const void* x, const void* y, void* dx, void* dy, long long n, int dtype,
+void silu_mul_bwd(const void* dout, const void* x, const void* y, void* dx, void* dy, long long n, DType dtype,
                   cudaStream_t s) {
   if (n == 0) return;
   const int grid = ew_grid(n >> 3);
-  if (dtype == 0) silu_mul_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)x, (const __nv_bfloat16*)y, (__nv_bfloat16*)dx, (__nv_bfloat16*)dy, n);
-  else if (dtype == 1) silu_mul_bwd_kernel<float><<<grid, 256, 0, s>>>((const float*)dout, (const float*)x, (const float*)y, (float*)dx, (float*)dy, n);
+  if (dtype == DTYPE_BF16) silu_mul_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)x, (const __nv_bfloat16*)y, (__nv_bfloat16*)dx, (__nv_bfloat16*)dy, n);
+  else if (dtype == DTYPE_F32) silu_mul_bwd_kernel<float><<<grid, 256, 0, s>>>((const float*)dout, (const float*)x, (const float*)y, (float*)dx, (float*)dy, n);
   else silu_mul_bwd_kernel<__half><<<grid, 256, 0, s>>>((const __half*)dout, (const __half*)x, (const __half*)y, (__half*)dx, (__half*)dy, n);
 }
 
@@ -1049,22 +1049,22 @@ __global__ void __launch_bounds__(256) scale_kernel(T* __restrict__ x, long long
 
 }  // namespace
 
-void sumsq_accumulate(const void* x, long long n, int dtype, float* out, cudaStream_t s) {
+void sumsq_accumulate(const void* x, long long n, DType dtype, float* out, cudaStream_t s) {
   if (n == 0) return;
   long long blocks = ((n >> 3) + 255) / 256;
   const long long cap = static_cast<long long>(num_sms()) * 4;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  if (dtype == 0) sumsq_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, s>>>((const __nv_bfloat16*)x, n, out);
-  else if (dtype == 1) sumsq_kernel<float><<<(int)blocks, 256, 0, s>>>((const float*)x, n, out);
+  if (dtype == DTYPE_BF16) sumsq_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, s>>>((const __nv_bfloat16*)x, n, out);
+  else if (dtype == DTYPE_F32) sumsq_kernel<float><<<(int)blocks, 256, 0, s>>>((const float*)x, n, out);
   else sumsq_kernel<__half><<<(int)blocks, 256, 0, s>>>((const __half*)x, n, out);
 }
 
-void scale_inplace(void* x, long long n, int dtype, const float* scale, cudaStream_t s) {
+void scale_inplace(void* x, long long n, DType dtype, const float* scale, cudaStream_t s) {
   if (n == 0) return;
   const int grid = ew_grid(n >> 3);
-  if (dtype == 0) scale_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((__nv_bfloat16*)x, n, scale);
-  else if (dtype == 1) scale_kernel<float><<<grid, 256, 0, s>>>((float*)x, n, scale);
+  if (dtype == DTYPE_BF16) scale_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((__nv_bfloat16*)x, n, scale);
+  else if (dtype == DTYPE_F32) scale_kernel<float><<<grid, 256, 0, s>>>((float*)x, n, scale);
   else scale_kernel<__half><<<grid, 256, 0, s>>>((__half*)x, n, scale);
 }
 

@@ -26,7 +26,7 @@ int gemm_set_pair_mode(int mode) {
 int gemm_pair_mode() { return pair_mode_ref(); }
 
 // CTA pairs pay off once there are enough 256-row tiles to fill the 66 SM pairs; tiny problems keep the single-CTA kernels
-bool gemm_pair_eligible(const GemmArgs& a) { return a.M >= 512 && a.N >= 128 && a.comm == 0; }
+bool gemm_pair_eligible(const GemmArgs& a) { return a.M >= 512 && a.N >= 128 && a.comm == COMM_NONE; }
 
 void gemm_dense(const GemmArgs& a, cudaStream_t stream) {
   // MN-major A with K-major B has store epilogues only, whichever kernel (single CTA or pair) the shape would pick

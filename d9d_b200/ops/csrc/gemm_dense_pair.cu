@@ -7,7 +7,7 @@ using namespace gemm;
 
 void gemm_dense_pair(const GemmArgs& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0) return;
-  if (a.comm != 0) throw std::runtime_error("d9d gemm: CTA-pair kernels do not implement fused communication");
+  if (a.comm != COMM_NONE) throw std::runtime_error("d9d gemm: CTA-pair kernels do not implement fused communication");
   // 256-wide tiles unless the problem is narrow or the narrower tile wastes fewer columns of the last n-tile
   int bn = a.block_n ? a.block_n : 256;
   if (a.block_n == 0) {

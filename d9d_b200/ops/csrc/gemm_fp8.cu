@@ -196,7 +196,7 @@ __global__ void quant_mx_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __
 // 8 tx .. 8 tx + 7 of the tile; elements past R / C are read as zero (a partial group's scale covers its valid elements).
 //   not transposed: q[r, c] row pitch ldq bytes; s[c / 128][r] (ROW: the row group's scale, BLOCK: the block's)
 //   transposed:     q[c, r] row pitch ldq bytes, columns r in [R, ldq) written as zeros; s[r / 128][c] (COL / BLOCK)
-enum BlockGroup : int { GROUP_ROW = 0, GROUP_COL = 1, GROUP_BLOCK = 2 };
+// GROUP is a BlockGroup (d9d_ops.h).
 
 template <int GROUP, bool TRANSPOSE>
 __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
@@ -419,7 +419,7 @@ void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long
 }
 
 void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, int C, long long ldx, long long ldq, long long lds,
-                             int group, bool transpose, cudaStream_t stream) {
+                             BlockGroup group, bool transpose, cudaStream_t stream) {
   if (R <= 0 || C <= 0) return;
   if (C % 8 != 0) throw std::runtime_error("d9d quantize_blockwise: C must be a multiple of 8");
   const dim3 grid(static_cast<unsigned>((C + 127) / 128), static_cast<unsigned>((R + 127) / 128));
@@ -439,31 +439,41 @@ void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, 
 
 void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0) return;
-  if (a.blockwise) {
-    if (a.scale_a == nullptr || a.scale_b == nullptr) throw std::runtime_error("d9d gemm_fp8_blockwise: both scale tensors are required");
-    if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_BF16>(a, stream);
-    else if (a.epi == gemm::EPI_F32) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_F32>(a, stream);
-    else throw std::runtime_error("d9d gemm_fp8_blockwise: bf16 or fp32 store only");
-  } else if (a.block_scaled) {
-    if (a.K % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr)
-      throw std::runtime_error("d9d gemm_mxfp8: K must be a multiple of 128 and both scale-factor tensors are required");
-    launch_fp8<128, fp8::MX>(a, stream);
-  } else if (a.mode == gemm::GROUPED_M) {
-    if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_M, gemm::EPI_BF16>(a, stream);
-    else if (a.epi == gemm::EPI_BF16_ACC) launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_M, gemm::EPI_BF16_ACC>(a, stream);
-    else throw std::runtime_error("d9d gemm_fp8: GROUPED_M supports bf16 store / accumulate only");
-  } else if (a.mode == gemm::GROUPED_K) {
-    switch (a.epi) {
-      case gemm::EPI_BF16: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_BF16>(a, stream); break;
-      case gemm::EPI_F32: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_F32>(a, stream); break;
-      case gemm::EPI_F32_ACC: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_F32_ACC>(a, stream); break;
-      case gemm::EPI_BF16_ACC: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_BF16_ACC>(a, stream); break;
-      default: throw std::runtime_error("d9d gemm_fp8: GROUPED_K supports fp32 / bf16 store / accumulate only");
-    }
-  } else {
-    // 128-wide tiles only: a 256-wide fp32 accumulator (128 registers per consumer thread) spills at the kernel's
-    // 168-register budget
-    launch_fp8<128, fp8::ROWCOL>(a, stream);
+  switch (a.scaling) {
+    case fp8::BLOCKWISE:
+      if (a.scale_a == nullptr || a.scale_b == nullptr) throw std::runtime_error("d9d gemm_fp8_blockwise: both scale tensors are required");
+      if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_BF16>(a, stream);
+      else if (a.epi == gemm::EPI_F32) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_F32>(a, stream);
+      else throw std::runtime_error("d9d gemm_fp8_blockwise: bf16 or fp32 store only");
+      break;
+    case fp8::MX:
+      if (a.K % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr)
+        throw std::runtime_error("d9d gemm_mxfp8: K must be a multiple of 128 and both scale-factor tensors are required");
+      launch_fp8<128, fp8::MX>(a, stream);
+      break;
+    case fp8::ROWCOL:
+      switch (a.mode) {
+        case gemm::GROUPED_M:
+          if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_M, gemm::EPI_BF16>(a, stream);
+          else if (a.epi == gemm::EPI_BF16_ACC) launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_M, gemm::EPI_BF16_ACC>(a, stream);
+          else throw std::runtime_error("d9d gemm_fp8: GROUPED_M supports bf16 store / accumulate only");
+          break;
+        case gemm::GROUPED_K:
+          switch (a.epi) {
+            case gemm::EPI_BF16: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_BF16>(a, stream); break;
+            case gemm::EPI_F32: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_F32>(a, stream); break;
+            case gemm::EPI_F32_ACC: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_F32_ACC>(a, stream); break;
+            case gemm::EPI_BF16_ACC: launch_fp8<128, fp8::ROWCOL, gemm::GROUPED_K, gemm::EPI_BF16_ACC>(a, stream); break;
+            default: throw std::runtime_error("d9d gemm_fp8: GROUPED_K supports fp32 / bf16 store / accumulate only");
+          }
+          break;
+        case gemm::DENSE:
+          // 128-wide tiles only: a 256-wide fp32 accumulator (128 registers per consumer thread) spills at the kernel's
+          // 168-register budget
+          launch_fp8<128, fp8::ROWCOL>(a, stream);
+          break;
+      }
+      break;
   }
 }
 

@@ -39,6 +39,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "d9d_ops.h"  // fp8::Scaling
 #include "gemm_sm90.cuh"
 
 namespace d9d {
@@ -52,8 +53,6 @@ constexpr int NUM_CONSUMERS = 2;
 constexpr int NUM_EPI_WARPS = 4 * NUM_CONSUMERS;
 constexpr int EPI_BOX_ROWS = 16;
 constexpr int SF_BLOCK_BYTES = 512;  // 128 rows x 4 K-groups of 32 elements
-
-enum Scaling : int { ROWCOL = 0, MX = 1, BLOCKWISE = 2 };
 
 struct Params {
   int M, N, K;           // GROUPED_M: M = padded row capacity.  GROUPED_K: M, N = per-expert output dims, K unused

@@ -23,6 +23,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "d9d_ops.h"  // gemm::Mode, gemm::Epi, gemm::Comm
 
 namespace d9d {
 namespace gemm {
@@ -42,35 +43,6 @@ constexpr int EPI_BOX_ROWS = 16;  // output staging box: one warp's 16 accumulat
 constexpr int CONSUMER_REGS = 232;
 constexpr int PRODUCER_REGS = 40;
 
-enum Mode : int { DENSE = 0, GROUPED_M = 1, GROUPED_K = 2 };
-enum Epi : int {
-  EPI_BF16 = 0,       // D(bf16) = acc
-  EPI_F32 = 1,        // D(f32) = acc
-  EPI_F32_ACC = 2,    // D(f32) += acc
-  EPI_BF16_ACC = 3,   // D(bf16) += acc   TMA path: rn(D + rn_bf16(acc)), the add done in bf16 in L2;
-                      //                  direct-store path: rn(D + acc) with the add in fp32
-  EPI_CE_LSE = 4,     // fused linear-CE forward: per (row, n_tile) running max / sum-exp / target logit
-  EPI_CE_DLOGITS = 5, // fused linear-CE backward: D(bf16) = g[row] * (exp(acc - lse[row]) - [col == target[row]])
-  // regularised linear-CE (label smoothing eps, z-loss zeta over V classes in all):
-  EPI_CE_LSE_SUM = 6,    // EPI_CE_LSE + per (row, n_tile) sum of the tile's logits
-  EPI_CE_DLOGITS_REG = 7 // D(bf16) = g[row] * ((1 + 2 zeta lse[row]) p - (1 - eps) [col == target[row]] - eps / V)
-};
-
-// Tensor-parallel communication fused into the GEMM (operands / outputs living in NVLink peer memory):
-//   COMM_AG_A   A's rows (the M dim) are sharded over the peers: every m-tile is TMA-loaded straight from the owner's
-//               shard                                   => all-gather -> GEMM without a gathered copy of A
-//   COMM_RS_D   every output tile is TMA reduce-added into the shard of the peer that owns those rows
-//                                                        => GEMM -> reduce-scatter without a partial-sum buffer
-//   COMM_AG_KA / COMM_AG_KB   A / B (MN-major) is sharded along the *reduction* dim (wgrad of a sequence-parallel
-//               layer): every k-block is loaded from the owner's shard
-// Row index -> (owner, local row):  blk = idx / comm_block_rows; owner = blk % comm_world;
-//                                   local = (blk / comm_world) * comm_block_rows + idx % comm_block_rows
-// (covers both "tokens sharded as one contiguous block per rank" and "[batch, seq/W] per rank, batch-major").
-//   COMM_WAIT_A A is a *local* gathered buffer that is being filled shard by shard (peer copies running concurrently on
-//               the copy engines / another stream); the producer waits on the owner's arrival flag before the first
-//               load of an m-tile and tiles are visited starting with the local shard  => all-gather overlapped with
-//               the GEMM tile by tile while every remote byte crosses NVLink exactly once
-enum Comm : int { COMM_NONE = 0, COMM_AG_A = 1, COMM_RS_D = 2, COMM_AG_KA = 3, COMM_AG_KB = 4, COMM_WAIT_A = 5 };
 constexpr int MAX_PEERS = 8;
 struct PeerMaps { CUtensorMap m[MAX_PEERS]; };
 struct NoPeerMaps {};

@@ -1,5 +1,6 @@
 """The blockwise fp8 recipe on CPU: scale rules of the quantiser emulations, the outlier property that motivates it,
-the emulated linear layer's autograd (joint and split backward) and a Trainer run with ``Fp8LinearConfig(recipe="blockwise")``."""
+the emulated linear layer's autograd (joint backward, and the split backward of all three recipes) and a Trainer run with
+``Fp8LinearConfig(recipe="blockwise")``."""
 
 import pytest
 import torch
@@ -112,15 +113,14 @@ def test_blockwise_linear_autograd_close_to_fp32():
     assert _rel(w1.grad, w2.grad) < 0.06
 
 
-def test_split_backward_equals_the_joint_backward():
+def _assert_split_backward_equals_the_joint_backward(recipe, x, w):
     from d9d_b200.core.autograd import GLOBAL_GRAD_CONTEXT, GradDirection
 
-    x, w = _layer_inputs(6)
-    g = torch.randn(3, 50, 144)
+    g = torch.randn(*x.shape[:-1], w.shape[0])
     x1, w1 = x.clone().requires_grad_(), w.clone().requires_grad_()
-    fp8.fp8_linear(x1, w1, recipe="blockwise").float().backward(g)
+    fp8.fp8_linear(x1, w1, recipe=recipe).float().backward(g)
     x2, w2 = x.clone().requires_grad_(), w.clone().requires_grad_()
-    y = fp8.fp8_linear(x2, w2, recipe="blockwise").float()
+    y = fp8.fp8_linear(x2, w2, recipe=recipe).float()
     with GLOBAL_GRAD_CONTEXT.with_directions(GradDirection.inputs):
         y.backward(g, retain_graph=True)
     assert w2.grad is None and torch.equal(x2.grad, x1.grad)
@@ -128,6 +128,21 @@ def test_split_backward_equals_the_joint_backward():
     with GLOBAL_GRAD_CONTEXT.with_directions(GradDirection.weight):
         y.backward(g)
     assert x2.grad is None and torch.equal(w2.grad, w1.grad)
+
+
+def test_split_backward_equals_the_joint_backward():
+    _assert_split_backward_equals_the_joint_backward("blockwise", *_layer_inputs(6))
+
+
+@pytest.mark.parametrize("recipe", ["rowwise", "mx"])
+def test_split_backward_of_the_other_recipes_equals_the_joint_backward(recipe):
+    """The fp8 linear layer runs every recipe through one autograd function: the same split backward for each."""
+    if recipe == "mx":  # token and feature counts multiples of 128
+        torch.manual_seed(6)
+        x, w = torch.randn(2, 128, 256), torch.randn(128, 256) * 0.05
+    else:
+        x, w = _layer_inputs(6)
+    _assert_split_backward_equals_the_joint_backward(recipe, x, w)
 
 
 def test_blockwise_sizes_and_conversion():
