@@ -1,8 +1,9 @@
-"""The MoE expert block (``grouped_swiglu``) in bf16 against fp8 (e4m3 grouped GEMMs with per-expert scales), forward and
-forward + backward, at the flagship shape (T = 16 384 tokens, k = 8, E = 128, hidden 768, expert FFN 576) and at the
+"""The MoE expert block (``grouped_swiglu``) in bf16 against fp8 under the row-wise recipe (e4m3 grouped GEMMs with per-expert
+scales; the ``fp8`` keys) and under DeepSeek-V3's blockwise recipe (1x128 / 128x128 scales promoted per k-block; the
+``blockwise`` keys), forward and forward + backward, at the flagship shape (T = 16 384 tokens, k = 8, E = 128, hidden 768, expert FFN 576) and at the
 Qwen3-30B-A3B expert shape of ``bench.py`` (hidden 2048, expert FFN 768, same T / k / E).
 
-Timing: CUDA events around ``--iters`` calls; the bf16 and fp8 arms alternate window by window (``--repeats`` windows
+Timing: CUDA events around ``--iters`` calls; the three arms alternate window by window (``--repeats`` windows
 each) so that drifting clocks hit both alike; the median window is reported.  A separate ``torch.profiler`` run then splits
 one forward + backward of each arm into GEMMs, quantisers and the rest, with achieved TFLOP/s of the GEMMs (FLOPs
 counted from the routed tokens: 2 x tokens x in x out per GEMM, no padding).
@@ -41,24 +42,28 @@ def setup(T, k, E, H, F):
     return xp, pp.detach(), w, layout, dy
 
 
-def step(inputs, fp8, backward):
+# arm -> grouped_swiglu arguments; the keys name the arms in the JSON
+ARMS = {"bf16": {}, "fp8": {"fp8": True}, "blockwise": {"fp8": True, "recipe": "blockwise"}}
+
+
+def step(inputs, arm, backward):
     xp, pp, w, layout, dy = inputs
     if not backward:
         with torch.no_grad():
-            grouped_swiglu(xp, pp, *w, layout, fp8=fp8)
+            grouped_swiglu(xp, pp, *w, layout, **ARMS[arm])
         return
-    y = grouped_swiglu(xp, pp, *w, layout, fp8=fp8)
+    y = grouped_swiglu(xp, pp, *w, layout, **ARMS[arm])
     y.backward(dy)
     xp.grad = None
     for t in w:
         t.grad = None
 
 
-def window_ms(inputs, fp8, backward, iters):
+def window_ms(inputs, arm, backward, iters):
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     start.record()
     for _ in range(iters):
-        step(inputs, fp8, backward)
+        step(inputs, arm, backward)
     end.record()
     end.synchronize()
     return start.elapsed_time(end) / iters
@@ -72,14 +77,14 @@ def classify(name: str) -> str:
     return "other"
 
 
-def profile(inputs, fp8, routed, H, F):
+def profile(inputs, arm, routed, H, F):
     from torch.profiler import ProfilerActivity
     from torch.profiler import profile as tprofile
 
-    step(inputs, fp8, True)
+    step(inputs, arm, True)
     torch.cuda.synchronize()
     with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
-        step(inputs, fp8, True)
+        step(inputs, arm, True)
         torch.cuda.synchronize()
     us = {"gemm": 0.0, "quantise": 0.0, "other": 0.0}
     for ev in prof.key_averages():
@@ -106,19 +111,19 @@ def main() -> None:
         inputs = setup(T, k, E, H, F)
         row = {"name": name, "T": T, "k": k, "E": E, "hidden": H, "ffn": F}
         for backward in (False, True):
-            for fp8 in (False, True):
-                window_ms(inputs, fp8, backward, 2)  # warm-up
-            times = {False: [], True: []}
+            for arm in ARMS:
+                window_ms(inputs, arm, backward, 2)  # warm-up
+            times = {arm: [] for arm in ARMS}
             for _ in range(args.repeats):
-                for fp8 in (False, True):
-                    times[fp8].append(window_ms(inputs, fp8, backward, args.iters))
+                for arm in ARMS:
+                    times[arm].append(window_ms(inputs, arm, backward, args.iters))
             tag = "fwd_bwd" if backward else "fwd"
-            row[f"{tag}_bf16_ms"] = statistics.median(times[False])
-            row[f"{tag}_fp8_ms"] = statistics.median(times[True])
-            row[f"{tag}_bf16_spread_ms"] = max(times[False]) - min(times[False])
-            row[f"{tag}_fp8_spread_ms"] = max(times[True]) - min(times[True])
-        row["profile_bf16"] = profile(inputs, False, T * k, H, F)
-        row["profile_fp8"] = profile(inputs, True, T * k, H, F)
+            for arm in ARMS:
+                row[f"{tag}_{arm}_ms"] = statistics.median(times[arm])
+            for arm in ARMS:
+                row[f"{tag}_{arm}_spread_ms"] = max(times[arm]) - min(times[arm])
+        for arm in ARMS:
+            row[f"profile_{arm}"] = profile(inputs, arm, T * k, H, F)
         print(json.dumps(row))
         result["shapes"].append(row)
         del inputs

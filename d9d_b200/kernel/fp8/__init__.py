@@ -141,6 +141,34 @@ def quantize_weight_blocks_reference(w: torch.Tensor, transpose: bool = False) -
     return q.contiguous(), scale.t().repeat_interleave(128, dim=1)[:, :N].contiguous()
 
 
+def quantize_expert_weight_blocks_reference(w: torch.Tensor, transpose: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """``w [E, in, out]`` -> :func:`quantize_weight_blocks_reference` of every ``w[e]``: with ``transpose`` (the grouped
+    forward) ``(qT [E, out, in], s [E, ceil(in/128), out])``, else (the input gradient) ``(q [E, in, out], s [E, ceil(out/128), in])``."""
+    parts = [quantize_weight_blocks_reference(we, transpose) for we in w]
+    return torch.stack([q for q, _ in parts]), torch.stack([s for _, s in parts])
+
+
+def _segment_rows(x: torch.Tensor, starts, counts) -> torch.Tensor:
+    """``x`` with every row outside the experts' ranges ``[starts[e], starts[e] + counts[e])`` set to zero."""
+    keep = torch.zeros(x.shape[0], dtype=torch.bool, device=x.device)
+    for s0, n in zip(starts, counts):
+        keep[int(s0) : int(s0) + int(n)] = True
+    return torch.where(keep[:, None], x, torch.zeros((), dtype=x.dtype, device=x.device))
+
+
+def quantize_blockwise_segments_reference(x: torch.Tensor, starts, counts) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [cap, C]`` in the MoE layout -> ``(q [cap, C], s [ceil(C/128), cap])``: 1x128 row groups of the experts' rows;
+    every other row quantises to zero codes with scale 1."""
+    return quantize_blockwise_reference(_segment_rows(x, starts, counts))
+
+
+def quantize_blockwise_segments_t_reference(x: torch.Tensor, starts, counts) -> tuple[torch.Tensor, torch.Tensor]:
+    """``x [cap, C]`` in the MoE layout (segments start on 128-row boundaries) -> ``(qT [C, cap], s [cap/128, C])``: one scale
+    per 128-token group of every channel, the groups of expert ``e`` starting at its first row and ending at its last;
+    every row outside the experts' ranges quantises to zero (scale 1 for a group without rows)."""
+    return quantize_blockwise_t_reference(_segment_rows(x, starts, counts))
+
+
 def blockwise_mm_reference(aq, sa, bq, sb, out_dtype: torch.dtype = torch.bfloat16, acc_dtype: torch.dtype = torch.float32):
     """``sum_kb (aq[:, kb] @ bq[:, kb]^T) * sa[kb, :, None] * sb[kb, None, :]`` over the 128-deep k-blocks ``kb``."""
     K = aq.shape[1]
@@ -368,7 +396,9 @@ def convert_linears_to_fp8(module: nn.Module, predicate=lambda name, m: True, re
 __all__ = [
     "Fp8Linear", "Fp8LinearFunction", "blockwise_mm", "blockwise_mm_reference",
     "convert_linears_to_fp8", "dequantize_mx", "fp8_linear", "mx_mm", "mx_scale_exponent",
-    "quantize_blockwise", "quantize_blockwise_reference", "quantize_blockwise_t", "quantize_blockwise_t_reference",
+    "quantize_blockwise", "quantize_blockwise_reference", "quantize_blockwise_segments_reference",
+    "quantize_blockwise_segments_t_reference", "quantize_blockwise_t", "quantize_blockwise_t_reference",
+    "quantize_expert_weight_blocks_reference",
     "quantize_colwise_t", "quantize_colwise_t_batched_reference", "quantize_colwise_t_reference", "quantize_mx_reference",
     "quantize_segments_t_reference", "quantize_rowwise", "quantize_rowwise_reference", "quantize_weight_blocks",
     "quantize_weight_blocks_reference", "scaled_mm", "unpack_mx_scales",

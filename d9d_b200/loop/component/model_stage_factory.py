@@ -111,10 +111,11 @@ class ModelStageFactory:
             raise NotImplementedError("model_stage_factory.fp8_experts is not combined with tensor parallelism")
         from d9d_b200.module.block.moe import GroupedSwiGLU
 
+        recipe = self._config_model.fp8_experts_recipe
         blocks = [m for m in model.modules() if isinstance(m, GroupedSwiGLU)]
         for block in blocks:
-            block.enable_fp8()  # refuses LoRA-wrapped projections and sizes that are not multiples of 16
-        self._ctx.logger.info(f"fp8: {len(blocks)} expert blocks of this stage run in e4m3")
+            block.enable_fp8(recipe)  # refuses LoRA-wrapped projections and sizes that are not multiples of 16
+        self._ctx.logger.info(f"fp8: {len(blocks)} expert blocks of this stage run in e4m3 ({recipe})")
 
     def build_pipeline_and_modules(self) -> tuple[PipelineScheduleInfo, TrackedModules]:
         if self._config_model.checkpoint_only_trainable_parameters:

@@ -60,9 +60,12 @@ class ModelStageFactoryConfig(BaseModel):
     source_checkpoint: Path | None
     checkpoint_only_trainable_parameters: bool
     fp8_linear: Fp8LinearConfig | None = None
-    # run every MoE expert block (GroupedSwiGLU) of the stage in fp8: e4m3 grouped GEMMs with per-expert row / column
-    # scales for the forward, input gradient and weight gradient; the weights stay bf16 masters
+    # run every MoE expert block (GroupedSwiGLU) of the stage in fp8: e4m3 grouped GEMMs for the forward, input gradient
+    # and weight gradient; the weights stay bf16 masters
     fp8_experts: bool = False
+    # the fp8 experts' scaling: "rowwise" (per-expert row / column scales) or "blockwise" (DeepSeek-V3's 1x128 activation /
+    # 128x128 weight scales, promoted per 128-deep k-block); read only when fp8_experts is on
+    fp8_experts_recipe: Literal["rowwise", "blockwise"] = "rowwise"
 
 
 class GradientClippingConfig(BaseModel):

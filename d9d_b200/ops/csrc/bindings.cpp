@@ -582,6 +582,152 @@ void gemm_fp8_blockwise(const Tensor& a, const Tensor& sa, const Tensor& b, cons
   d9d::gemm_fp8(g, cur_stream());
 }
 
+// ------------------------------------------------------------------ blockwise fp8 MoE experts ---------------------------
+// w[E, in, out] bf16 (in, out multiples of 16) -> one scale per 128 x 128 block of every w[e], in the copy a grouped GEMM reads:
+//   transpose = true (forward):  (qt[E, out, in], s[E, ceil(in/128), out])
+//   transpose = false (dgrad):   (q[E, in, out],  s[E, ceil(out/128), in])
+// s is a view with a row pitch of round_up(rows, 128) (zero pad)
+std::tuple<Tensor, Tensor> quantize_expert_weight_blocks(const Tensor& w, bool transpose) {
+  TORCH_CHECK(w.is_cuda() && w.dim() == 3 && w.is_contiguous() && w.scalar_type() == at::kBFloat16,
+              "quantize_expert_weight_blocks: contiguous 3-D bf16 CUDA tensor [E, in, out] required");
+  TORCH_CHECK(w.size(0) > 0 && w.size(1) % 16 == 0 && w.size(2) % 16 == 0, "quantize_expert_weight_blocks: in and out must be multiples of 16");
+  TORCH_CHECK(w.size(0) < (int64_t(1) << 16) && w.size(1) < (int64_t(1) << 31) && w.size(2) < (int64_t(1) << 31),
+              "quantize_expert_weight_blocks: too large");
+  CHECK_ALIGNED16(w);
+  c10::cuda::CUDAGuard guard(w.device());
+  const int64_t E = w.size(0), R = w.size(1), C = w.size(2);
+  const int64_t groups = transpose ? (R + 127) / 128 : (C + 127) / 128, rows = transpose ? C : R;
+  Tensor q = transpose ? at::empty({E, C, R}, w.options().dtype(at::kFloat8_e4m3fn)) : at::empty({E, R, C}, w.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = at::zeros({E, groups, round_up128(rows)}, w.options().dtype(at::kFloat)).narrow(2, 0, rows);
+  d9d::quantize_expert_blocks_e4m3(w.data_ptr(), q.data_ptr(), s.data_ptr<float>(), static_cast<int>(E), R, static_cast<int>(C),
+                                   s.stride(1), transpose, cur_stream());
+  return {q, s};
+}
+
+static void check_tiles_input(const char* op, const Tensor& x, const Tensor& tile_group) {
+  check_blockwise_input(op, x);
+  TORCH_CHECK(x.size(1) % 16 == 0, op, ": C must be a multiple of 16");
+  TORCH_CHECK(tile_group.is_cuda() && tile_group.device() == x.device() && tile_group.is_contiguous() && tile_group.scalar_type() == at::kInt,
+              op, ": tile_group must be a contiguous int32 tensor on x's device");
+  TORCH_CHECK(x.size(0) % 128 == 0 && tile_group.numel() == x.size(0) / 128, op,
+              ": rows must be a multiple of 128 with one tile_group entry per 128 rows");
+}
+
+// x[cap, C] bf16 in the MoE layout -> (q[cap, C] e4m3, s[ceil(C/128), cap] fp32): one scale per 1 x 128 group of every row
+// of the 128-row tiles in use; tiles whose tile_group is -1 are skipped (their codes and scales are never read)
+std::tuple<Tensor, Tensor> quantize_blockwise_tiles(const Tensor& x, const Tensor& tile_group) {
+  check_tiles_input("quantize_blockwise_tiles", x, tile_group);
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t R = x.size(0), C = x.size(1);
+  Tensor q = at::empty({R, C}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = at::empty({(C + 127) / 128, R}, x.options().dtype(at::kFloat));
+  d9d::quantize_blockwise_tiles_e4m3(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), tile_group.data_ptr<int>(), nullptr, nullptr, R,
+                                     static_cast<int>(C), x.stride(0), C, s.stride(0), false, cur_stream());
+  return {q, s};
+}
+
+// x[cap, C] bf16 in the MoE layout -> (qt[C, cap] e4m3, s[cap/128, C] fp32): one scale per 128-token group of every channel;
+// an expert's groups start at its segment and end at its last row (later rows of its tiles are zeros in qt); tiles whose
+// tile_group is -1 are skipped
+std::tuple<Tensor, Tensor> quantize_blockwise_t_tiles(const Tensor& x, const Tensor& tile_group, const Tensor& seg_offsets,
+                                                      const Tensor& counts) {
+  check_tiles_input("quantize_blockwise_t_tiles", x, tile_group);
+  for (const Tensor* t : {&seg_offsets, &counts})
+    TORCH_CHECK(t->is_cuda() && t->device() == x.device() && t->is_contiguous() && t->scalar_type() == at::kInt,
+                "quantize_blockwise_t_tiles: seg_offsets and counts must be contiguous int32 tensors on x's device");
+  TORCH_CHECK(counts.numel() > 0 && seg_offsets.numel() == counts.numel() + 1, "quantize_blockwise_t_tiles: seg_offsets must be [E + 1], counts [E]");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t R = x.size(0), C = x.size(1);
+  Tensor qt = at::empty({C, R}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = blockwise_scales(x, R / 128, C);
+  d9d::quantize_blockwise_tiles_e4m3(x.data_ptr(), qt.data_ptr(), s.data_ptr<float>(), tile_group.data_ptr<int>(), seg_offsets.data_ptr<int>(),
+                                     counts.data_ptr<int>(), R, static_cast<int>(C), x.stride(0), R, s.stride(0), true, cur_stream());
+  return {qt, s};
+}
+
+// Operand checks of the blockwise grouped GEMMs: e4m3 K-major operands with 16-byte rows, int32 table, one device
+static void check_blockwise_grouped(const char* op, const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, const Tensor& d,
+                                    const Tensor& table) {
+  for (const Tensor* t : {&a, &sa, &b, &sb, &d, &table})
+    TORCH_CHECK(t->is_cuda() && t->device() == a.device(), op, ": all operands must be CUDA tensors on one device");
+  for (const Tensor* t : {&a, &b, &d, &table}) TORCH_CHECK(t->is_contiguous(), op, ": a, b, d and the expert table must be contiguous");
+  CHECK_ALIGNED16(a); CHECK_ALIGNED16(b); CHECK_ALIGNED16(d);
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn, op, ": a and b must be float8_e4m3fn");
+  TORCH_CHECK(sa.scalar_type() == at::kFloat && sb.scalar_type() == at::kFloat, op, ": scales must be fp32");
+  TORCH_CHECK(table.scalar_type() == at::kInt, op, ": the expert table must be int32");
+  TORCH_CHECK(a.dim() == 2 && a.size(1) % 16 == 0 && a.size(1) > 0, op, ": a must be 2-D with rows of a positive multiple of 16 bytes");
+  TORCH_CHECK(a.size(0) < (int64_t(1) << 31) && a.size(1) < (int64_t(1) << 31), op, ": a is too large");
+}
+
+// s: [..., groups, rows] fp32 view with unit column stride, a row pitch of round_up(rows, 128), planes groups * pitch apart
+static void check_grouped_scales(const char* op, const char* name, const Tensor& s, std::vector<int64_t> shape) {
+  const int64_t rows = shape.back(), pitch = round_up128(rows);
+  TORCH_CHECK(s.sizes().vec() == shape, op, ": ", name, " has the wrong shape for its operand");
+  TORCH_CHECK(s.stride(-1) == 1 && s.stride(-2) == pitch && (s.dim() == 2 || s.stride(0) == shape[1] * pitch), op, ": ", name,
+              " must be k-block-major with a row pitch of round_up(rows, 128)");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(s.data_ptr()) & 15) == 0, op, ": ", name, " must start on a 16-byte boundary");
+  int64_t planes = 1;
+  for (size_t i = 0; i + 1 < shape.size(); ++i) planes *= shape[i];
+  const int64_t avail = static_cast<int64_t>(s.storage().nbytes()) - s.storage_offset() * 4;
+  TORCH_CHECK(avail >= planes * pitch * 4, op, ": ", name, "'s storage must hold its padded rows");
+}
+
+// d[R, N] (+)= sum_kb (a[R, kb] · b[e(r), :, kb]^T) * sa[kb, r] * sb[e(r), kb, n]: the MoE forward / input gradient under the
+// blockwise recipe.  a: expert-sorted rows (R a multiple of 128), b: [E, N, K], tile_group: [R/128] (-1: never read or written)
+void gemm_fp8_blockwise_grouped_m(const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, Tensor d, const Tensor& tile_group,
+                                  bool accumulate) {
+  const char* op = "gemm_fp8_blockwise_grouped_m";
+  check_blockwise_grouped(op, a, sa, b, sb, d, tile_group);
+  TORCH_CHECK(b.dim() == 3 && b.size(2) == a.size(1), op, ": b must be [E, N, K] with the K of a");
+  TORCH_CHECK(b.size(0) > 0 && b.size(1) > 0 && b.size(1) < (int64_t(1) << 31), op, ": b must have experts and N > 0");
+  TORCH_CHECK(a.size(0) % 128 == 0 && tile_group.numel() == a.size(0) / 128, op, ": rows must be a multiple of 128 with one tile_group entry per 128 rows");
+  TORCH_CHECK(d.dim() == 2 && d.size(0) == a.size(0) && d.size(1) == b.size(1) && d.scalar_type() == at::kBFloat16, op, ": d must be bf16 [R, N]");
+  TORCH_CHECK(d.size(1) % 8 == 0, op, ": N must be a multiple of 8 (16-byte output rows)");
+  const int64_t kb = (a.size(1) + 127) / 128;
+  check_grouped_scales(op, "sa", sa, {kb, a.size(0)});
+  check_grouped_scales(op, "sb", sb, {b.size(0), kb, b.size(1)});
+  c10::cuda::CUDAGuard guard(a.device());
+  d9d::Fp8GemmArgs g;
+  g.scaling = d9d::fp8::BLOCKWISE;
+  g.mode = GROUPED_M; g.epi = accumulate ? EPI_BF16_ACC : EPI_BF16;
+  g.M = static_cast<int>(a.size(0)); g.K = static_cast<int>(a.size(1)); g.N = static_cast<int>(b.size(1));
+  g.num_groups = static_cast<int>(b.size(0));
+  g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
+  g.lda = a.stride(0); g.ldb = b.stride(1); g.b_group_stride = b.stride(0); g.ldd = d.stride(0);
+  g.scale_a = sa.data_ptr<float>(); g.scale_b = sb.data_ptr<float>();
+  g.tile_group = tile_group.data_ptr<int>();
+  d9d::gemm_fp8(g, cur_stream());
+}
+
+// d[e] (+)= sum over expert e's 128-token groups kb of (a[:, kb] · b[:, kb]^T) * sa[kb, m] * sb[kb, n]: the MoE weight gradient
+// under the blockwise recipe.  a: [M, R], b: [N, R] from quantize_blockwise_t_tiles, d: [E, M, N] fp32 or bf16 (an expert without
+// rows: zeros when storing, untouched when accumulating)
+void gemm_fp8_blockwise_grouped_k(const Tensor& a, const Tensor& sa, const Tensor& b, const Tensor& sb, Tensor d, const Tensor& group_offsets,
+                                  bool accumulate) {
+  const char* op = "gemm_fp8_blockwise_grouped_k";
+  check_blockwise_grouped(op, a, sa, b, sb, d, group_offsets);
+  TORCH_CHECK(b.dim() == 2 && b.size(1) == a.size(1) && b.size(0) > 0 && b.size(0) < (int64_t(1) << 31), op, ": b must be [N, R] with the R of a");
+  TORCH_CHECK(a.size(1) % 128 == 0, op, ": R must be a multiple of 128 (the expert segments' alignment)");
+  TORCH_CHECK(d.dim() == 3 && d.size(0) > 0 && d.size(1) == a.size(0) && d.size(2) == b.size(0), op, ": d must be [E, M, N]");
+  TORCH_CHECK(d.scalar_type() == at::kFloat || d.scalar_type() == at::kBFloat16, op, ": d must be fp32 or bf16");
+  TORCH_CHECK(d.size(2) * d.element_size() % 16 == 0, op, ": rows of d must be a multiple of 16 bytes");
+  TORCH_CHECK(group_offsets.numel() == d.size(0) + 1, op, ": group_offsets must be [E + 1]");
+  check_grouped_scales(op, "sa", sa, {a.size(1) / 128, a.size(0)});
+  check_grouped_scales(op, "sb", sb, {a.size(1) / 128, b.size(0)});
+  c10::cuda::CUDAGuard guard(a.device());
+  d9d::Fp8GemmArgs g;
+  g.scaling = d9d::fp8::BLOCKWISE;
+  g.mode = GROUPED_K; g.epi = epi_for(d, accumulate);
+  g.M = static_cast<int>(a.size(0)); g.N = static_cast<int>(b.size(0)); g.K = 0;
+  g.k_total = a.size(1);
+  g.num_groups = static_cast<int>(d.size(0));
+  g.A = a.data_ptr(); g.B = b.data_ptr(); g.D = d.data_ptr();
+  g.lda = a.stride(0); g.ldb = b.stride(0); g.ldd = d.stride(1); g.d_group_stride = d.stride(0);
+  g.scale_a = sa.data_ptr<float>(); g.scale_b = sb.data_ptr<float>();
+  g.group_offsets = group_offsets.data_ptr<int>();
+  d9d::gemm_fp8(g, cur_stream());
+}
+
 // ------------------------------------------------------------------ RMSNorm ---------------------
 std::tuple<Tensor, Tensor> rms_norm_fwd(const Tensor& x, const Tensor& w, double eps, bool zero_centered) {
   CHECK_CUDA_CONTIG(x); CHECK_CUDA_CONTIG(w); CHECK_ALIGNED16(x); CHECK_ALIGNED16(w);
@@ -1250,6 +1396,11 @@ TORCH_LIBRARY(d9d_b200, m) {
   m.def("quantize_blockwise_t(Tensor x) -> (Tensor, Tensor)");
   m.def("quantize_weight_blocks(Tensor w, bool transpose=False) -> (Tensor, Tensor)");
   m.def("gemm_fp8_blockwise(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d) -> ()");
+  m.def("quantize_expert_weight_blocks(Tensor w, bool transpose) -> (Tensor, Tensor)");
+  m.def("quantize_blockwise_tiles(Tensor x, Tensor tile_group) -> (Tensor, Tensor)");
+  m.def("quantize_blockwise_t_tiles(Tensor x, Tensor tile_group, Tensor seg_offsets, Tensor counts) -> (Tensor, Tensor)");
+  m.def("gemm_fp8_blockwise_grouped_m(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d, Tensor tile_group, bool accumulate=False) -> ()");
+  m.def("gemm_fp8_blockwise_grouped_k(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor(a!) d, Tensor group_offsets, bool accumulate) -> ()");
   m.def("rms_norm_fwd(Tensor x, Tensor w, float eps, bool zero_centered) -> (Tensor, Tensor)");
   m.def("rms_norm_bwd(Tensor dout, Tensor x, Tensor w, Tensor inv_rms, bool zero_centered) -> (Tensor, Tensor)");
   m.def("silu_mul_fwd(Tensor x, Tensor y) -> Tensor");
@@ -1315,6 +1466,11 @@ TORCH_LIBRARY_IMPL(d9d_b200, CUDA, m) {
   m.impl("quantize_blockwise_t", &quantize_blockwise_t);
   m.impl("quantize_weight_blocks", &quantize_weight_blocks);
   m.impl("gemm_fp8_blockwise", &gemm_fp8_blockwise);
+  m.impl("quantize_expert_weight_blocks", &quantize_expert_weight_blocks);
+  m.impl("quantize_blockwise_tiles", &quantize_blockwise_tiles);
+  m.impl("quantize_blockwise_t_tiles", &quantize_blockwise_t_tiles);
+  m.impl("gemm_fp8_blockwise_grouped_m", &gemm_fp8_blockwise_grouped_m);
+  m.impl("gemm_fp8_blockwise_grouped_k", &gemm_fp8_blockwise_grouped_k);
   m.impl("rms_norm_fwd", &rms_norm_fwd);
   m.impl("rms_norm_bwd", &rms_norm_bwd);
   m.impl("silu_mul_fwd", &silu_mul_fwd);

@@ -119,7 +119,8 @@ struct Fp8GemmArgs {
   gemm::Epi epi = gemm::EPI_BF16; // bf16 store (dense); GROUPED_M: + bf16 accumulate; GROUPED_K: fp32 / bf16 store / accumulate;
                                   // BLOCKWISE: bf16 or fp32 store
   // ROWCOL: row / column scales in the epilogue; MX: UE8M0 scale per 32 K-elements (DENSE); BLOCKWISE: scale_a / scale_b
-  // are [ceil(K/128), round_up(M / N, 128)] per (k-block, row) scales (DENSE)
+  // are [ceil(K/128), round_up(M / N, 128)] per (k-block, row) scales (DENSE; GROUPED_M: scale_b [E, ceil(K/128),
+  // round_up(N, 128)]; GROUPED_K: both [k_total/128, round_up(M / N, 128)], one k-block per 128-token group)
   fp8::Scaling scaling = fp8::ROWCOL;
   const void* A = nullptr;   // [M, K] e4m3, K contiguous (row pitch lda bytes); GROUPED_K: [M, k_total]
   const void* B = nullptr;   // [N, K] e4m3; GROUPED_M: [E, N, K] (expert pitch b_group_stride bytes); GROUPED_K: [N, k_total]
@@ -158,6 +159,16 @@ void quantize_mx_e4m3(const void* x, void* q, void* sf, long long M, int K, long
 enum BlockGroup : int { GROUP_ROW = 0, GROUP_COL = 1, GROUP_BLOCK = 2 };
 void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, int C, long long ldx, long long ldq, long long lds,
                              BlockGroup group, bool transpose, cudaStream_t stream);
+// The 128 x 128 blocks of every expert's weight w[e, R, C] (contiguous): plain q[e, R, C] with s[e, ceil(C/128), lds] per row,
+// or transposed qt[e, C, R] with s[e, ceil(R/128), lds] per column; lds as above.
+void quantize_expert_blocks_e4m3(const void* w, void* q, float* scale, int E, long long R, int C, long long lds, bool transpose,
+                                 cudaStream_t stream);
+// x[R, C] in the MoE layout (R a multiple of 128): 128-row tiles with tile_group -1 are skipped.  Plain: GROUP_ROW codes
+// q[R, C] (row pitch ldq) and s[ceil(C/128), lds]; transposed: GROUP_COL codes qt[C, R] (pitch ldq >= R) and s[R/128, lds],
+// the token groups of expert g ending at row seg_offsets[g] + counts[g] (later rows of its tiles are zeros).
+void quantize_blockwise_tiles_e4m3(const void* x, void* q, float* scale, const int* tile_group, const int* seg_offsets,
+                                   const int* counts, long long R, int C, long long ldx, long long ldq, long long lds, bool transpose,
+                                   cudaStream_t stream);
 
 // ------------------------------------------------------------------ normalisation ----------------
 // element type of the normalisation, activation and grad-utility launchers

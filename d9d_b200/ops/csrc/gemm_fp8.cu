@@ -6,6 +6,8 @@
 //   quantize_mx          x[M,K] bf16 -> q[M,K] e4m3, UE8M0 scale blocks  (one scale per 32 K-elements, 128-row x 4-group blocks)
 //   quantize_blockwise   x[R,C] bf16 -> e4m3 with fp32 scales per 1x128 row group, 128x1 column group (transposed copy) or
 //                        128x128 block (either copy), stored k-block-major for the BLOCKWISE GEMM
+//   quantize_expert_blocks / quantize_blockwise_tiles  the same blockwise groups for the MoE experts: every expert's weight
+//                        blocks (batched over E), and the MoE layout's row / 128-token groups, skipping unused 128-row tiles
 //   gemm_fp8 / gemm_mxfp8  D[M,N] bf16 = scaled A·B^T on wgmma e4m3 (MX: per-32-K scales applied in registers), the
 //                          grouped expert GEMMs (GROUPED_M / GROUPED_K) and the BLOCKWISE GEMM (bf16 / fp32 D), see
 //                          gemm_fp8_sm90.cuh
@@ -198,17 +200,18 @@ __global__ void quant_mx_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __
 //   transposed:     q[c, r] row pitch ldq bytes, columns r in [R, ldq) written as zeros; s[r / 128][c] (COL / BLOCK)
 // GROUP is a BlockGroup (d9d_ops.h).
 
+// quant_blockwise_tile: the tile (row_tile, col_tile) of x, the work of one CTA of 256 threads.
 template <int GROUP, bool TRANSPOSE>
-__global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
-                                                              float* __restrict__ s, long long R, int C, long long ldx, long long ldq,
-                                                              long long lds) {
+__device__ __forceinline__ void quant_blockwise_tile(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q, float* __restrict__ s,
+                                                     long long R, int C, long long ldx, long long ldq, long long lds,
+                                                     unsigned row_tile, unsigned col_tile) {
   static_assert(GROUP == GROUP_BLOCK || (GROUP == GROUP_ROW) != TRANSPOSE, "row groups: plain copy; column groups: transposed");
   __shared__ float red[8][128];                          // per-warp partial amax (COL: per column, BLOCK: one value)
   __shared__ uint32_t tq[TRANSPOSE ? 128 : 1][33];       // transposed tile: 128 columns x 128 row bytes (+1 word pad)
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long r0 = static_cast<long long>(blockIdx.y) * 128;
-  const int c0 = blockIdx.x * 128;
+  const long long r0 = static_cast<long long>(row_tile) * 128;
+  const int c0 = col_tile * 128;
   const int cc = c0 + 8 * tx;
   float v[8][8];
 #pragma unroll
@@ -234,7 +237,7 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
       const float sc = e4m3_scale(a);
       inv_r[i] = 1.f / sc;
       const long long r = r0 + 8 * ty + i;
-      if (tx == 0 && r < R) s[static_cast<long long>(blockIdx.x) * lds + r] = sc;
+      if (tx == 0 && r < R) s[static_cast<long long>(col_tile) * lds + r] = sc;
     }
   } else if constexpr (GROUP == GROUP_COL) {
 #pragma unroll
@@ -253,7 +256,7 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
       for (int w = 0; w < 8; ++w) a = fmaxf(a, red[w][8 * tx + j]);
       const float sc = e4m3_scale(a);
       inv_c[j] = 1.f / sc;
-      if (ty == 0 && cc + j < C) s[static_cast<long long>(blockIdx.y) * lds + cc + j] = sc;
+      if (ty == 0 && cc + j < C) s[static_cast<long long>(row_tile) * lds + cc + j] = sc;
     }
   } else {
     float a = 0.f;
@@ -271,9 +274,9 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
     // one scale per row (plain copy) or per column (transposed copy) of the block: 128 values, 256 threads
     if (threadIdx.x < 128) {
       if constexpr (TRANSPOSE) {
-        if (c0 + static_cast<int>(threadIdx.x) < C) s[static_cast<long long>(blockIdx.y) * lds + c0 + threadIdx.x] = sc;
+        if (c0 + static_cast<int>(threadIdx.x) < C) s[static_cast<long long>(row_tile) * lds + c0 + threadIdx.x] = sc;
       } else {
-        if (r0 + threadIdx.x < R) s[static_cast<long long>(blockIdx.x) * lds + r0 + threadIdx.x] = sc;
+        if (r0 + threadIdx.x < R) s[static_cast<long long>(col_tile) * lds + r0 + threadIdx.x] = sc;
       }
     }
   }
@@ -319,6 +322,37 @@ __global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat1
       }
     }
   }
+}
+
+template <int GROUP, bool TRANSPOSE>
+__global__ void __launch_bounds__(256) quant_blockwise_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
+                                                              float* __restrict__ s, long long R, int C, long long ldx, long long ldq,
+                                                              long long lds) {
+  quant_blockwise_tile<GROUP, TRANSPOSE>(x, q, s, R, C, ldx, ldq, lds, blockIdx.y, blockIdx.x);
+}
+
+// The 128x128 blocks of every expert's weight w[e] (blockIdx.z = e): planes of x and q R * C elements apart, of s
+// s_plane floats apart.
+template <bool TRANSPOSE>
+__global__ void __launch_bounds__(256) quant_expert_blocks_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
+                                                                  float* __restrict__ s, long long R, int C, long long ldq,
+                                                                  long long lds, long long s_plane) {
+  const long long e = blockIdx.z;
+  quant_blockwise_tile<GROUP_BLOCK, TRANSPOSE>(x + e * R * C, q + e * R * C, s + e * s_plane, R, C, C, ldq, lds, blockIdx.y, blockIdx.x);
+}
+
+// The MoE layout x[cap, C] (cap a multiple of 128) in 128-row tiles: a tile whose tile_group entry is -1 is skipped (its
+// codes and scales are left as they were).  Row groups (plain copy) quantise every row of a tile in use; the transposed
+// 128-token groups end at the expert's last row, rows past it come out as zeros.
+template <int GROUP, bool TRANSPOSE>
+__global__ void __launch_bounds__(256) quant_blockwise_tiles_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
+                                                                    float* __restrict__ s, long long R, int C, long long ldx,
+                                                                    long long ldq, long long lds, const int* __restrict__ tile_group,
+                                                                    const int* __restrict__ seg_offsets, const int* __restrict__ counts) {
+  const int g = tile_group[blockIdx.y];
+  if (g < 0) return;
+  const long long r_end = TRANSPOSE ? static_cast<long long>(seg_offsets[g]) + counts[g] : R;
+  quant_blockwise_tile<GROUP, TRANSPOSE>(x, q, s, r_end, C, ldx, ldq, lds, blockIdx.y, blockIdx.x);
 }
 
 // 2-D map, or 3-D ([d2, d1, d0], box depth 1) when d2 > 0
@@ -437,14 +471,62 @@ void quantize_blockwise_e4m3(const void* x, void* q, float* scale, long long R, 
     throw std::runtime_error("d9d quantize_blockwise: row groups give a plain copy, column groups a transposed one");
 }
 
+void quantize_expert_blocks_e4m3(const void* w, void* q, float* scale, int E, long long R, int C, long long lds, bool transpose,
+                                 cudaStream_t stream) {
+  if (E <= 0 || R <= 0 || C <= 0) return;
+  if (C % 8 != 0 || (transpose && R % 16 != 0)) throw std::runtime_error("d9d quantize_expert_blocks: C must be a multiple of 8 (R of 16)");
+  const dim3 grid(static_cast<unsigned>((C + 127) / 128), static_cast<unsigned>((R + 127) / 128), static_cast<unsigned>(E));
+  const auto* xb = static_cast<const __nv_bfloat16*>(w);
+  auto* qb = static_cast<uint8_t*>(q);
+  if (transpose) {
+    const long long s_plane = (R + 127) / 128 * lds;
+    quant_expert_blocks_kernel<true><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, R, lds, s_plane);
+  } else {
+    const long long s_plane = (C + 127) / 128 * lds;
+    quant_expert_blocks_kernel<false><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, C, lds, s_plane);
+  }
+}
+
+void quantize_blockwise_tiles_e4m3(const void* x, void* q, float* scale, const int* tile_group, const int* seg_offsets,
+                                   const int* counts, long long R, int C, long long ldx, long long ldq, long long lds, bool transpose,
+                                   cudaStream_t stream) {
+  if (R <= 0 || C <= 0) return;
+  if (R % 128 != 0 || C % 8 != 0) throw std::runtime_error("d9d quantize_blockwise_tiles: R must be a multiple of 128 and C of 8");
+  const dim3 grid(static_cast<unsigned>((C + 127) / 128), static_cast<unsigned>(R / 128));
+  const auto* xb = static_cast<const __nv_bfloat16*>(x);
+  auto* qb = static_cast<uint8_t*>(q);
+  if (transpose)
+    quant_blockwise_tiles_kernel<GROUP_COL, true><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, ldx, ldq, lds, tile_group, seg_offsets, counts);
+  else
+    quant_blockwise_tiles_kernel<GROUP_ROW, false><<<grid, 256, 0, stream>>>(xb, qb, scale, R, C, ldx, ldq, lds, tile_group, seg_offsets, counts);
+}
+
 void gemm_fp8(const Fp8GemmArgs& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0) return;
   switch (a.scaling) {
     case fp8::BLOCKWISE:
       if (a.scale_a == nullptr || a.scale_b == nullptr) throw std::runtime_error("d9d gemm_fp8_blockwise: both scale tensors are required");
-      if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_BF16>(a, stream);
-      else if (a.epi == gemm::EPI_F32) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_F32>(a, stream);
-      else throw std::runtime_error("d9d gemm_fp8_blockwise: bf16 or fp32 store only");
+      switch (a.mode) {
+        case gemm::DENSE:
+          if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_BF16>(a, stream);
+          else if (a.epi == gemm::EPI_F32) launch_fp8<128, fp8::BLOCKWISE, gemm::DENSE, gemm::EPI_F32>(a, stream);
+          else throw std::runtime_error("d9d gemm_fp8_blockwise: bf16 or fp32 store only");
+          break;
+        case gemm::GROUPED_M:
+          if (a.epi == gemm::EPI_BF16) launch_fp8<128, fp8::BLOCKWISE, gemm::GROUPED_M, gemm::EPI_BF16>(a, stream);
+          else if (a.epi == gemm::EPI_BF16_ACC) launch_fp8<128, fp8::BLOCKWISE, gemm::GROUPED_M, gemm::EPI_BF16_ACC>(a, stream);
+          else throw std::runtime_error("d9d gemm_fp8_blockwise: GROUPED_M supports bf16 store / accumulate only");
+          break;
+        case gemm::GROUPED_K:
+          switch (a.epi) {
+            case gemm::EPI_BF16: launch_fp8<128, fp8::BLOCKWISE, gemm::GROUPED_K, gemm::EPI_BF16>(a, stream); break;
+            case gemm::EPI_F32: launch_fp8<128, fp8::BLOCKWISE, gemm::GROUPED_K, gemm::EPI_F32>(a, stream); break;
+            case gemm::EPI_F32_ACC: launch_fp8<128, fp8::BLOCKWISE, gemm::GROUPED_K, gemm::EPI_F32_ACC>(a, stream); break;
+            case gemm::EPI_BF16_ACC: launch_fp8<128, fp8::BLOCKWISE, gemm::GROUPED_K, gemm::EPI_BF16_ACC>(a, stream); break;
+            default: throw std::runtime_error("d9d gemm_fp8_blockwise: GROUPED_K supports fp32 / bf16 store / accumulate only");
+          }
+          break;
+      }
       break;
     case fp8::MX:
       if (a.K % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr)

@@ -33,7 +33,8 @@
 // The grouped modes promote the accumulation: every 128-deep k-block is summed by the tensor core into a fresh
 // accumulator, which is then added to the fp32 register accumulator.  Hopper's e4m3 wgmma keeps a reduced-precision
 // accumulator inside one MMA chain, and an expert's weight gradient reduces over thousands of tokens.
-// The grouped modes live in grouped_tiles() and BLOCKWISE in blockwise_tiles(); the ROWCOL / MX DENSE instances keep
+// The ROWCOL grouped modes live in grouped_tiles() and BLOCKWISE (DENSE and grouped) in blockwise_tiles(), whose DENSE
+// producer keeps its own loop; the ROWCOL / MX DENSE instances keep
 // their own body, unchanged, so that they compile to exactly the instructions they compiled to before the other modes
 // existed (even an unused local in a shared body changed their schedule).
 #pragma once
@@ -261,18 +262,43 @@ __device__ __forceinline__ void grouped_tiles(const CUtensorMap& tmap_a, const C
   }
 }
 
-// One CTA's work in the BLOCKWISE scaling (DENSE tile walk, BLOCK_N = 128): every stage carries the k-block's A / B tiles
-// and their 128 + 128 fp32 scales; the consumers compute the k-block's four MMAs into a fresh accumulator and add it with
+// The tile at index `tile` of a BLOCKWISE walk: the DENSE rasterisation (tile_coord, every tile valid, all k_blocks) or
+// the grouped modes' gemm::get_tile (GROUPED_M: -1 tiles invalid; GROUPED_K: the expert's rows from k_begin).
+template <int MODE, int BLOCK_N>
+__device__ __forceinline__ gemm::TileCoord blockwise_tile(const Params& p, int tile, int m_tiles, int n_tiles, int k_blocks) {
+  if constexpr (MODE == gemm::DENSE) {
+    gemm::TileCoord t;
+    tile_coord(tile, m_tiles, n_tiles, t.m_blk, t.n_blk);
+    t.group = 0;
+    t.k_begin = 0;
+    t.k_blocks = k_blocks;
+    t.valid = true;
+    return t;
+  } else {
+    return gemm::get_tile<MODE, BLOCK_N, BLOCK_M, BLOCK_K>(p, tile);
+  }
+}
+
+// One CTA's work in the BLOCKWISE scaling (BLOCK_N = 128): every stage carries the k-block's A / B tiles and their
+// 128 + 128 fp32 scales; the consumers compute the k-block's four MMAs into a fresh accumulator and add it with
 // acc = fma(part, sa[row] * sb[col], acc).  Tails: TMA zero-fills a partial last k-block and the rows / columns of A / B
 // past M / N (their scales are never applied to a stored element), and the TMA store clips D to [M, N].
+// The scales of k-block kb (all k-block-major, row pitch round_up(rows, 128)):
+//   DENSE      scale_a [ceil(K/128), M], scale_b [ceil(K/128), N]: row kb of both
+//   GROUPED_M  scale_a [ceil(K/128), M] (M = capacity): row kb; scale_b [E, ceil(K/128), N]: row kb of expert e's plane
+//   GROUPED_K  scale_a [R/128, M], scale_b [R/128, N] (128-token groups): row group_offsets[e] / 128 + kb of both
 // The consumers raised their register budget (acc + part = 128 fp32 registers), so they wait with mbar_wait_flag and a
 // timed-out wait traps after their region (see mbar_wait_flag).
-template <int BLOCK_N, int EPI>
+template <int BLOCK_N, int MODE, int EPI>
 __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap& tmap_d,
                                                 const Params& p) {
   using C = Cfg<BLOCK_N, BLOCKWISE>;
-  static_assert(EPI == gemm::EPI_BF16 || EPI == gemm::EPI_F32, "BLOCKWISE: bf16 or fp32 store");
-  constexpr bool OUT_BF16 = (EPI == gemm::EPI_BF16);
+  static_assert(MODE == gemm::DENSE ? (EPI == gemm::EPI_BF16 || EPI == gemm::EPI_F32)
+                                    : (EPI == gemm::EPI_BF16 || EPI == gemm::EPI_BF16_ACC ||
+                                       (MODE == gemm::GROUPED_K && (EPI == gemm::EPI_F32 || EPI == gemm::EPI_F32_ACC))),
+                "BLOCKWISE DENSE: bf16 or fp32 store; GROUPED_M: bf16 store / accumulate; GROUPED_K: fp32 / bf16 store / accumulate");
+  constexpr bool OUT_BF16 = (EPI == gemm::EPI_BF16 || EPI == gemm::EPI_BF16_ACC);
+  constexpr bool REDUCE = (EPI == gemm::EPI_F32_ACC || EPI == gemm::EPI_BF16_ACC);
   constexpr int CHUNK_COLS = OUT_BF16 ? 64 : 32;  // one 128-byte staging row
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -290,8 +316,8 @@ __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const
 
   const int warp = threadIdx.x >> 5;
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M, n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int total_tiles = m_tiles * n_tiles;
-  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int total_tiles = m_tiles * n_tiles * (MODE == gemm::GROUPED_K ? p.num_groups : 1);
+  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;  // DENSE / GROUPED_M
   // k-block-major scales: rows padded to whole tiles, so a tile's scales are one aligned 512-byte copy inside the tensor
   const long long lds_a = static_cast<long long>(m_tiles) * BLOCK_M, lds_b = static_cast<long long>(n_tiles) * BLOCK_N;
 
@@ -316,17 +342,40 @@ __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        int m_blk, n_blk;
-        tile_coord(tile, m_tiles, n_tiles, m_blk, n_blk);
-        const int m_idx = m_blk * BLOCK_M, n_idx = n_blk * BLOCK_N;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait_wg(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-          tma_load_2d(smem_a + stage * C::A_STAGE_BYTES, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_idx);
-          tma_load_2d(smem_b + stage * C::B_STAGE_BYTES, &tmap_b, &full_bar[stage], kb * BLOCK_K, n_idx);
-          bulk_load_1d(smem_sa + stage * BLOCK_M, p.scale_a + kb * lds_a + m_idx, C::SFA_STAGE_BYTES, &full_bar[stage]);
-          bulk_load_1d(smem_sb + stage * BLOCK_N, p.scale_b + kb * lds_b + n_idx, C::SFB_STAGE_BYTES, &full_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if constexpr (MODE == gemm::DENSE) {
+          int m_blk, n_blk;
+          tile_coord(tile, m_tiles, n_tiles, m_blk, n_blk);
+          const int m_idx = m_blk * BLOCK_M, n_idx = n_blk * BLOCK_N;
+          for (int kb = 0; kb < k_blocks; ++kb) {
+            mbar_wait_wg(&empty_bar[stage], phase ^ 1);
+            mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+            tma_load_2d(smem_a + stage * C::A_STAGE_BYTES, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_idx);
+            tma_load_2d(smem_b + stage * C::B_STAGE_BYTES, &tmap_b, &full_bar[stage], kb * BLOCK_K, n_idx);
+            bulk_load_1d(smem_sa + stage * BLOCK_M, p.scale_a + kb * lds_a + m_idx, C::SFA_STAGE_BYTES, &full_bar[stage]);
+            bulk_load_1d(smem_sb + stage * BLOCK_N, p.scale_b + kb * lds_b + n_idx, C::SFB_STAGE_BYTES, &full_bar[stage]);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        } else {
+          const gemm::TileCoord t = gemm::get_tile<MODE, BLOCK_N, BLOCK_M, BLOCK_K>(p, tile);
+          if (!t.valid) continue;  // GROUPED_M: an m-tile past the last expert's segment
+          const int m_idx = t.m_blk * BLOCK_M, n_idx = t.n_blk * BLOCK_N;
+          // the scale rows of k-block kb (see above): GROUPED_M scale_b is one [ceil(K/128), N] plane per expert; GROUPED_K
+          // reads the 128-token groups from the expert's first row
+          const long long sa_row0 = MODE == gemm::GROUPED_K ? t.k_begin / BLOCK_K : 0;
+          const long long sb_row0 = MODE == gemm::GROUPED_K ? t.k_begin / BLOCK_K : static_cast<long long>(t.group) * t.k_blocks;
+          for (int kb = 0; kb < t.k_blocks; ++kb) {
+            mbar_wait_wg(&empty_bar[stage], phase ^ 1);
+            mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+            const int k_idx = t.k_begin + kb * BLOCK_K;  // GROUPED_K: the expert's rows start at k_begin
+            tma_load_2d(smem_a + stage * C::A_STAGE_BYTES, &tmap_a, &full_bar[stage], k_idx, m_idx);
+            if constexpr (MODE == gemm::GROUPED_M)  // B: [E, N, K]
+              tma_load_3d(smem_b + stage * C::B_STAGE_BYTES, &tmap_b, &full_bar[stage], k_idx, n_idx, t.group);
+            else
+              tma_load_2d(smem_b + stage * C::B_STAGE_BYTES, &tmap_b, &full_bar[stage], k_idx, n_idx);
+            bulk_load_1d(smem_sa + stage * BLOCK_M, p.scale_a + (sa_row0 + kb) * lds_a + m_idx, C::SFA_STAGE_BYTES, &full_bar[stage]);
+            bulk_load_1d(smem_sb + stage * BLOCK_N, p.scale_b + (sb_row0 + kb) * lds_b + n_idx, C::SFB_STAGE_BYTES, &full_bar[stage]);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
         }
       }
     }
@@ -343,11 +392,11 @@ __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const
     uint32_t epi_chunk = 0;
     float acc[BLOCK_N / 2];
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int m_blk, n_blk;
-      tile_coord(tile, m_tiles, n_tiles, m_blk, n_blk);
+      const gemm::TileCoord t = blockwise_tile<MODE, BLOCK_N>(p, tile, m_tiles, n_tiles, k_blocks);
+      if (!t.valid) continue;
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < k_blocks; ++kb) {
+      for (int kb = 0; kb < t.k_blocks; ++kb) {
         mbar_wait_flag(&full_bar[stage], phase, stuck);
         const uint32_t a_addr = smem_u32(smem_a + stage * C::A_STAGE_BYTES) + cw * (64 * 128);
         const uint32_t b_addr = smem_u32(smem_b + stage * C::B_STAGE_BYTES);
@@ -378,9 +427,10 @@ __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if (REDUCE && t.k_blocks == 0) continue;  // an expert without rows (GROUPED_K) stores zeros but adds nothing
 
-      const int rbase = m_blk * BLOCK_M + cw * 64 + wq * 16;
-      const int col0 = n_blk * BLOCK_N;
+      const int rbase = t.m_blk * BLOCK_M + cw * 64 + wq * 16;
+      const int col0 = t.n_blk * BLOCK_N;
 #pragma unroll
       for (int c = 0; c < BLOCK_N / CHUNK_COLS; ++c) {
         const int cbase = col0 + c * CHUNK_COLS;
@@ -412,7 +462,9 @@ __device__ __forceinline__ void blockwise_tiles(const CUtensorMap& tmap_a, const
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) {
-          tma_store_3d(&tmap_d, stage_buf, cbase, rbase, 0);
+          const int g0 = (MODE == gemm::GROUPED_K) ? t.group : 0;  // GROUPED_K: D is [E, M, N]
+          if constexpr (REDUCE) tma_reduce_add_3d(&tmap_d, stage_buf, cbase, rbase, g0);
+          else tma_store_3d(&tmap_d, stage_buf, cbase, rbase, g0);
           tma_store_commit();
         }
       }
@@ -428,13 +480,13 @@ template <int BLOCK_N, int SCALING, int MODE = gemm::DENSE, int EPI = gemm::EPI_
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                 const __grid_constant__ CUtensorMap tmap_d, const Params p) {
-  static_assert(MODE == gemm::DENSE || SCALING == ROWCOL, "the grouped modes use row / column scaling");
+  static_assert(MODE == gemm::DENSE || SCALING != MX, "the grouped modes use row / column or blockwise scaling");
   static_assert(MODE != gemm::DENSE || EPI == gemm::EPI_BF16 || (SCALING == BLOCKWISE && EPI == gemm::EPI_F32),
                 "the dense kernel stores bf16 (BLOCKWISE: or fp32)");
-  if constexpr (MODE != gemm::DENSE) {
+  if constexpr (SCALING == BLOCKWISE) {
+    blockwise_tiles<BLOCK_N, MODE, EPI>(tmap_a, tmap_b, tmap_d, p);
+  } else if constexpr (MODE != gemm::DENSE) {
     grouped_tiles<BLOCK_N, MODE, EPI>(tmap_a, tmap_b, tmap_d, p);
-  } else if constexpr (SCALING == BLOCKWISE) {
-    blockwise_tiles<BLOCK_N, EPI>(tmap_a, tmap_b, tmap_d, p);
   } else {
     using C = Cfg<BLOCK_N, SCALING>;
     constexpr int STAGES = C::STAGES;
