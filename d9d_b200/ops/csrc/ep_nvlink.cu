@@ -98,6 +98,7 @@ void ep_push(const void* x, const float* probs, const int* dest_rank, const int*
              long long off_p, long long n_pairs, int k, int H, cudaStream_t stream) {
   if (n_pairs == 0) return;
   if (H % 8 != 0 || (off_x & 15) != 0) throw std::runtime_error("d9d ep_push: H % 8 == 0 and 16-byte aligned regions required");
+  if (probs != nullptr && (off_p & 3) != 0) throw std::runtime_error("d9d ep_push: the probability region must be 4-byte aligned");
   long long blocks = (n_pairs + 7) / 8;
   const long long cap = static_cast<long long>(sms()) * 8;
   if (blocks > cap) blocks = cap;
@@ -109,6 +110,7 @@ void ep_pull_sum(void* const* peer_base, long long off_y, long long off_dp, cons
                  float* dprobs, long long T, int k, int H, cudaStream_t stream) {
   if (T == 0) return;
   if (H % 8 != 0 || k > 32 || (off_y & 15) != 0) throw std::runtime_error("d9d ep_pull_sum: H % 8 == 0, k <= 32, aligned regions required");
+  if (dprobs != nullptr && (off_dp & 3) != 0) throw std::runtime_error("d9d ep_pull_sum: the d(prob) region must be 4-byte aligned");
   long long blocks = (T + 7) / 8;
   const long long cap = static_cast<long long>(sms()) * 8;
   if (blocks > cap) blocks = cap;
